@@ -130,6 +130,20 @@ void wmb_destroy(wmb_ctx *c);
 /* Start over with a new capture (same as destroy + create, without re-allocating). */
 int  wmb_reset(wmb_ctx *c);
 
+/* Receiver settings of one chain (WMB_CHAIN_*), for both of its algorithms -- the reference's two tuning constants
+ * that it marks as future options:
+ *   clock_lock          1..16, default 2: the time2 algorithm samples the data bit on the clock_lock-th clock sample
+ *                       after a rising edge of the clock, i.e. on sample m iff the clock reads low at m-L-1 and high at
+ *                       m-L..m (opts_CLOCK_LOCK_THRESHOLD_T1_C1 / _S1, rtl_wmbus.c:865-866, used at :1092-1111 and
+ *                       :1184-1203).  Before the first sample the clock reads low.
+ *   access_code_errors  default 0: a bit carries the access-code flag iff the shift register differs from the access
+ *                       code in at most this many bits (ACCESS_CODE_T1_C1_ERRORS / ACCESS_CODE_S1_ERRORS, :99, :103,
+ *                       compared at :688, :773, :822, :846).  At most 3 for T1/C1 (at 4 the preamble 0x5555 matches
+ *                       0x543D) and 6 for S1.
+ * Valid before the first push or right after wmb_reset / wmb_seek (else WMB_E_STATE); out-of-range values give
+ * WMB_E_INVAL.  The settings survive wmb_reset and wmb_seek and are part of wmb_boundary_state(). */
+int  wmb_set_receiver(wmb_ctx *c, int chain, uint32_t clock_lock, uint32_t access_code_errors);
+
 /* Page-locked host memory for input buffers (the reference reads stdin into a 4096-byte
  * stack array, rtl_wmbus.c:1249; a GPU pipeline wants to DMA straight out of the read
  * buffer).  wmb_push() accepts any host pointer; pinned ones are copied asynchronously. */

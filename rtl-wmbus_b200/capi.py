@@ -76,6 +76,7 @@ def _bind(lib):
     lib.wmb_debug_arith.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]
     lib.wmb_seek.argtypes = [C.c_void_p, C.c_uint64]
     lib.wmb_set_line_window.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64]
+    lib.wmb_set_receiver.argtypes = [C.c_void_p, C.c_int, C.c_uint32, C.c_uint32]
     lib.wmb_boundary_state.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
     lib.wmb_boundary_state.restype = C.c_long
     lib.wmb_pending_before.argtypes = [C.c_void_p, C.c_uint64]
@@ -86,7 +87,7 @@ def _bind(lib):
 EXPORTS = ["wmb_reset", "wmb_host_alloc", "wmb_host_free", "wmb_default_opts", "wmb_abi_version", "wmb_last_error", "wmb_version_string", "wmb_create",
            "wmb_destroy", "wmb_push", "wmb_push_device", "wmb_poll", "wmb_decode_frames", "wmb_take_lines",
            "wmb_process", "wmb_process_device", "wmb_get_stats", "wmb_debug_copy_stage", "wmb_debug_copy_bits", "wmb_debug_copy_events", "wmb_debug_arith",
-           "wmb_seek", "wmb_set_line_window", "wmb_boundary_state", "wmb_pending_before"]
+           "wmb_seek", "wmb_set_line_window", "wmb_boundary_state", "wmb_pending_before", "wmb_set_receiver"]
 
 
 def load_library(path: str | None = None):
@@ -128,9 +129,11 @@ def opts_from_flags(lib, flags: str = "", **kw) -> WmbOpts:
 
 
 class WmbusB200:
-    """One decoding context (== one rtl_wmbus process) on one GPU."""
+    """One decoding context (== one rtl_wmbus process) on one GPU.
+    clock_lock=(t1c1, s1), access_code_errors=(t1c1, s1): receiver settings, see wmb_set_receiver() (default (2, 2) and
+    (0, 0), the reference's).  They survive reset() and seek()."""
 
-    def __init__(self, flags: str = "", device: int = 0, lib=None, **tuning):
+    def __init__(self, flags: str = "", device: int = 0, lib=None, clock_lock=None, access_code_errors=None, **tuning):
         self.lib = lib or load_library()
         self.opts = opts_from_flags(self.lib, flags, **tuning)
         self._ctx = C.c_void_p()
@@ -138,6 +141,15 @@ class WmbusB200:
         if rc != 0:
             raise RuntimeError(f"wmb_create failed ({rc}): {self.lib.wmb_last_error().decode()}")
         self._out = C.create_string_buffer(1 << 22)
+        if clock_lock is not None or access_code_errors is not None:
+            lock = clock_lock if clock_lock is not None else (2, 2)
+            errs = access_code_errors if access_code_errors is not None else (0, 0)
+            try:
+                for chain in (0, 1):
+                    self.set_receiver(chain, lock[chain], errs[chain])
+            except Exception:
+                self.close()
+                raise
 
     def close(self):
         if self._ctx:
@@ -241,6 +253,10 @@ class WmbusB200:
     def seek(self, first_iq_sample: int):
         """reset + position the stream at an absolute IQ sample of the capture (time-chunk sharding)"""
         self._check(self.lib.wmb_seek(self._ctx, first_iq_sample))
+
+    def set_receiver(self, chain: int, clock_lock: int, access_code_errors: int):
+        """clock-lock threshold and access-code bit errors of one chain (before the first push, or after reset/seek)"""
+        self._check(self.lib.wmb_set_receiver(self._ctx, chain, clock_lock, access_code_errors))
 
     def set_line_window(self, sync_lo: int, sync_hi: int):
         self._check(self.lib.wmb_set_line_window(self._ctx, sync_lo, sync_hi))

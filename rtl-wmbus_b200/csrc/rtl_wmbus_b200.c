@@ -12,6 +12,11 @@
  * Extra environment knobs (not options, so the argv surface stays the reference's):
  *   WMBUS_B200_DEVICE=<n>      CUDA device (default 0)
  *   WMBUS_B200_BATCH_MIB=<n>   bytes gathered before a device pass (default 64)
+ *   WMBUS_B200_CLOCK_LOCK=<t1c1>[,<s1>]           clock-lock threshold of the time2 algorithm, 1..16 (default 2,
+ *                              the reference's opts_CLOCK_LOCK_THRESHOLD_*, rtl_wmbus.c:865-866)
+ *   WMBUS_B200_ACCESS_CODE_ERRORS=<t1c1>[,<s1>]   access-code bit errors accepted, T1/C1 0..3, S1 0..6 (default 0,
+ *                              ACCESS_CODE_*_ERRORS, rtl_wmbus.c:99, :103)
+ *   One value sets both chains.  A malformed or out-of-range value is an error at start-up (wmb_set_receiver).
  */
 #define _GNU_SOURCE
 #include <errno.h>
@@ -74,6 +79,20 @@ static void set_alarm(double seconds)
         if (it.it_value.tv_sec == 0 && it.it_value.tv_usec == 0) it.it_value.tv_usec = 1;
     }
     setitimer(ITIMER_REAL, &it, NULL);
+}
+
+/* "<a>" or "<a>,<b>" of decimal numbers -> v[0], v[1] (one number: both); 0 if malformed */
+static int parse_pair(const char *e, unsigned long v[2])
+{
+    char *end = NULL;
+    if (e[0] < '0' || e[0] > '9') return 0;
+    v[0] = v[1] = strtoul(e, &end, 10);
+    if (*end == ',') {
+        const char *f = end + 1;
+        if (f[0] < '0' || f[0] > '9') return 0;
+        v[1] = strtoul(f, &end, 10);
+    }
+    return *end == 0 && v[0] <= 0xFFFFFFFFul && v[1] <= 0xFFFFFFFFul;
 }
 
 static int emit_lines(wmb_ctx *ctx, char *out, size_t outcap)
@@ -151,11 +170,26 @@ int main(int argc, char *argv[])
     const size_t batch = (size_t)batch_mib * 1048576u;
     o.max_batch_mib = (uint32_t)batch_mib;
 
+    unsigned long lock[2] = { 2, 2 }, errors[2] = { 0, 0 };
+    if ((e = getenv("WMBUS_B200_CLOCK_LOCK")) != NULL && !parse_pair(e, lock)) {
+        fprintf(stderr, "rtl_wmbus_b200: WMBUS_B200_CLOCK_LOCK=%s: expected <t1c1>[,<s1>]\n", e);
+        return EXIT_FAILURE;
+    }
+    if ((e = getenv("WMBUS_B200_ACCESS_CODE_ERRORS")) != NULL && !parse_pair(e, errors)) {
+        fprintf(stderr, "rtl_wmbus_b200: WMBUS_B200_ACCESS_CODE_ERRORS=%s: expected <t1c1>[,<s1>]\n", e);
+        return EXIT_FAILURE;
+    }
+
     wmb_ctx *ctx = NULL;
     if (wmb_create(&o, device, &ctx) != WMB_OK) {
         fprintf(stderr, "rtl_wmbus_b200: %s\n", wmb_last_error());
         return EXIT_FAILURE;
     }
+    for (int ch = 0; ch < 2; ch++)
+        if (wmb_set_receiver(ctx, ch, (uint32_t)lock[ch], (uint32_t)errors[ch]) != WMB_OK) {
+            fprintf(stderr, "rtl_wmbus_b200: %s\n", wmb_last_error());
+            return EXIT_FAILURE;
+        }
     uint8_t *buf = wmb_host_alloc(batch);
     const size_t outcap = 1u << 20;
     char *out = malloc(outcap);

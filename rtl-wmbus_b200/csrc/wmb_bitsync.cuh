@@ -38,6 +38,7 @@ struct K2aParams {
     uint32_t dc, t2;            /* -o ; time2 enabled (else only the data bits are produced)  */
     uint32_t spec0;             /* lane 0 starts cold from the history too (its predecessor -- the previous batch's last
                                    lane -- may still be running); verified against the carried state like any lane  */
+    uint32_t lock;              /* clock-lock threshold L, 1..WMB_LOCK_MAX (wmb_set_receiver)                  */
 };
 
 /* registers of one clock-recovery lane */
@@ -148,6 +149,40 @@ WMB_D void k2a_block32(const float4 (&blk)[8], K2aRegs &r, uint32_t &dword, uint
     }
 }
 
+/* Clock lock on a whole word (rtl_wmbus.c:1092-1111): counting clock samples from a rising edge, the reference
+ * delivers the data bit on the L-th high sample after it (opts_CLOCK_LOCK_THRESHOLD_*, :865-866), i.e. on sample m iff
+ * the clock read low at m-L-1 and high at m-L..m.  `clk` holds the L+1 clock signs before the word, newest in bit 0
+ * (zero before the stream's first sample: the clock reads low there).  LK = 2: the reference's threshold as a
+ * constant, the default path; LK = 0: L from the launch, without a branch. */
+template <int LK>
+WMB_D uint32_t lock_strobes(uint32_t clk, uint32_t cword, uint32_t L)
+{
+    if (LK == 2) {
+        const uint64_t hist3 = ((clk & 1u) << 2) | (clk & 2u) | ((clk >> 2) & 1u);   /* bit2 = m-1 */
+        const uint64_t H = ((uint64_t)cword << 3) | hist3;
+        return (uint32_t)((H >> 3) & (H >> 2) & (H >> 1) & ~H);
+    }
+    /* time order: bit L+1+i = sample i of the word, bit j = sample j-L-1 for j <= L */
+    const uint64_t H = ((uint64_t)cword << (L + 1)) | (wmb_brev(clk) >> (31 - L));
+    uint64_t high = H >> 1;
+#pragma unroll
+    for (uint32_t j = 2; j <= WMB_LOCK_MAX + 1; j++) high &= (j <= L + 1) ? (H >> j) : ~0ull;
+    return (uint32_t)(high & ~H);
+}
+
+/* the clock history after a word of n samples (bits 0..n-1 of cword; none above) */
+template <int LK>
+WMB_D uint32_t lock_history(uint32_t clk, uint32_t cword, int n, uint32_t L)
+{
+    if (LK == 2) {
+        if (n == 32) return ((cword >> 31) & 1u) | (((cword >> 30) & 1u) << 1) | (((cword >> 29) & 1u) << 2);
+        for (int i = 0; i < n; i++) clk = ((clk << 1) | ((cword >> i) & 1u)) & 7u;
+        return clk;
+    }
+    const uint32_t mask = (2u << L) - 1u, r = wmb_brev(cword);      /* r: bit k = sample 31 - k */
+    return (n == 32 ? r : (clk << n) | (r >> (32 - n))) & mask;
+}
+
 WMB_D void k2a_load(float4 (&blk)[8], const float *src)
 {
     const float4 *s4 = (const float4 *)src;
@@ -164,7 +199,7 @@ WMB_D void k2a_save(IirState &st, const K2aRegs &r)
 
 #define K2A_L2_AHEAD 16
 
-template <class CH, bool DC, bool T2>
+template <class CH, bool DC, bool T2, int LK>
 WMB_D void k2a_lane_t(const K2aParams &p, uint32_t lane)
 {
     if (lane >= p.lanes) return;
@@ -210,15 +245,8 @@ WMB_D void k2a_lane_t(const K2aParams &p, uint32_t lane)
          * two 20 KB unrolled bodies thrash the instruction cache) */
         if (n == 32) k2a_block32<CH, DC, T2>(cur, r, dword, cword);
         else k2a_block<CH, DC, T2, false>(cur, n, r, dword, cword);
-        /* lock stencil on the whole word: sample the data bit where the clock reads
-         * low, high, high, high at m-3..m (rtl_wmbus.c:1092-1111) */
-        const uint64_t hist3 = ((r.clk3 & 1u) << 2) | (r.clk3 & 2u) | ((r.clk3 >> 2) & 1u);   /* bit2 = m-1 */
-        const uint64_t H = ((uint64_t)cword << 3) | hist3;
-        const uint32_t sword = (uint32_t)((H >> 3) & (H >> 2) & (H >> 1) & ~H);
-        if (n == 32) r.clk3 = ((cword >> 31) & 1u) | (((cword >> 30) & 1u) << 1) | (((cword >> 29) & 1u) << 2);
-        else {
-            for (int i = 0; i < n; i++) r.clk3 = ((r.clk3 << 1) | ((cword >> i) & 1u)) & 7u;
-        }
+        const uint32_t sword = lock_strobes<LK>(r.clk3, cword, p.lock);
+        r.clk3 = lock_history<LK>(r.clk3, cword, n, p.lock);
         if (m >= s0) {
             const uint32_t keep = (n == 32) ? 0xFFFFFFFFu : ((1u << n) - 1u);
             p.dbits[m >> 5] = dword & keep;
@@ -237,8 +265,9 @@ WMB_D void k2a_lane_t(const K2aParams &p, uint32_t lane)
 template <class CH>
 WMB_D void k2a_lane(const K2aParams &p, uint32_t lane)
 {
-    if (p.dc) { if (p.t2) k2a_lane_t<CH, true, true>(p, lane); else k2a_lane_t<CH, true, false>(p, lane); }
-    else      { if (p.t2) k2a_lane_t<CH, false, true>(p, lane); else k2a_lane_t<CH, false, false>(p, lane); }
+    if (!p.t2) { if (p.dc) k2a_lane_t<CH, true, false, 2>(p, lane); else k2a_lane_t<CH, false, false, 2>(p, lane); }
+    else if (p.lock == 2) { if (p.dc) k2a_lane_t<CH, true, true, 2>(p, lane); else k2a_lane_t<CH, false, true, 2>(p, lane); }
+    else { if (p.dc) k2a_lane_t<CH, true, true, 0>(p, lane); else k2a_lane_t<CH, false, true, 0>(p, lane); }
 }
 
 #ifndef WMB_HOSTSIM
@@ -304,7 +333,7 @@ __device__ __forceinline__ void k2a2_step(K2a2Thread &t, const float xs, const i
     }
 }
 
-template <class CH>
+template <class CH, int LK>
 __global__ void __launch_bounds__(K2A2_THREADS) k2a2_lanes_kernel(const K2aParams p)
 {
     const int lid = threadIdx.x & 31;
@@ -377,12 +406,8 @@ __global__ void __launch_bounds__(K2A2_THREADS) k2a2_lanes_kernel(const K2aParam
         const int jb = j - 1;
         uint32_t sword = 0;
         if (t.r2) {
-            /* lock stencil on the whole word: sample the data bit where the clock reads low, high, high, high at
-             * m-3..m (rtl_wmbus.c:1092-1111) */
-            const uint64_t hist3 = ((clk3 & 1u) << 2) | (clk3 & 2u) | ((clk3 >> 2) & 1u);
-            const uint64_t H = ((uint64_t)A << 3) | hist3;
-            sword = (uint32_t)((H >> 3) & (H >> 2) & (H >> 1) & ~H);
-            clk3 = ((A >> 31) & 1u) | (((A >> 30) & 1u) << 1) | (((A >> 29) & 1u) << 2);
+            sword = lock_strobes<LK>(clk3, A, p.lock);
+            clk3 = lock_history<LK>(clk3, A, 32, p.lock);
             if (j == jw && m0 + 32 * (int64_t)jw <= -p.hist) clk3 = 0;     /* the lane starts at the stream's first sample: no clock history */
         }
         if (valid && jb >= jw && jb < je) {
@@ -410,7 +435,7 @@ WMB_D bool iir_state_equal(const IirState &a, const IirState &b, uint32_t dc, ui
     if (dc) eq = eq && wmb_f2u(a.dc_x) == wmb_f2u(b.dc_x) && wmb_f2u(a.dc_y) == wmb_f2u(b.dc_y);
     if (t2) {
         for (int i = 0; i < 6; i++) eq = eq && wmb_f2u(a.h[i]) == wmb_f2u(b.h[i]);
-        eq = eq && a.clk3 == b.clk3;
+        eq = eq && a.clk3 == b.clk3;                 /* the L+1 signs the lock stencil reads, no other bit is set */
     }
     return eq;
 }
@@ -434,6 +459,14 @@ WMB_D void k2a_verify_lane(const K2aParams &p, uint32_t lane, uint32_t *n_fail)
 /* ------------------------------------------------------------------------------------- */
 /* K2t: time2 bit stream                                                                 */
 /* ------------------------------------------------------------------------------------- */
+
+/* access-code match with up to `errors` bit errors: count_set_bits((bitstream & MASK) ^ CODE) <= ERRORS (rtl_wmbus.c:688,
+ * :773, :822, :846; ACCESS_CODE_*_ERRORS, :99, :103) */
+template <class CH>
+WMB_D uint32_t ac_match(uint32_t sr, uint32_t errors)
+{
+    return (uint32_t)wmb_popc((sr & CH::CODE_MASK) ^ CH::CODE) <= errors ? 1u : 0u;
+}
 
 struct StreamDev {                  /* device-resident bookkeeping of one (chain, algo) stream */
     uint64_t total;                 /* events appended so far (== next ordinal)            */
@@ -459,6 +492,7 @@ struct K2tParams {
     uint64_t *ring; uint64_t ring_mask;
     StreamDev *sd;
     uint64_t *cand; uint32_t cand_cap;
+    uint32_t ac_err;                /* access-code bit errors accepted (wmb_set_receiver)     */
 };
 
 WMB_HD uint32_t k2t_words(const K2tParams &p) { return (uint32_t)((p.M + 31) >> 5); }
@@ -662,7 +696,7 @@ WMB_D void k2t_write(const K2tParams &p, uint32_t lane)
                 s &= s - 1;
                 const uint32_t bit = (d >> i) & 1u;
                 sr = ((sr << 1) | bit) & CH::CODE_MASK;              /* rtl_wmbus.c:820 */
-                const uint32_t sync = (sr == CH::CODE) ? 1u : 0u;    /* rtl_wmbus.c:822 */
+                const uint32_t sync = ac_match<CH>(sr, p.ac_err);    /* rtl_wmbus.c:822 */
                 const int64_t m = (int64_t)(wb + q) * 32 + i;
                 const u32x4 rq = rs[2 * q + (i >> 4)];
                 const uint32_t rw = ((i >> 2) & 3) == 0 ? rq.x : ((i >> 2) & 3) == 1 ? rq.y : ((i >> 2) & 3) == 2 ? rq.z : rq.w;
@@ -706,6 +740,7 @@ struct K2mParams {
     uint32_t mode;
     const uint32_t *run_if;     /* optional: the whole pass happens only if this word is nonzero (T1/C1 fallback
                                    from the two-phase path, decided on the device)                */
+    uint32_t ac_err;            /* access-code bit errors accepted (wmb_set_receiver)         */
 };
 
 struct K2Out { uint32_t *ev; uint32_t cap; uint32_t n; uint32_t overflow; };
@@ -739,7 +774,7 @@ WMB_D bool k2m_edge(const K2mParams &p, RlState &s, uint32_t st, int64_t m, uint
                     rl -= s.a;
                     s.sr = ((s.sr << 1) | level) & CH::CODE_MASK;
                     if (n < K2_EDGE_EMIT_CAP) {
-                        k2_emit(o, live, off, rssi, (s.flags >> 1) & 1u, s.sr == CH::CODE, level);
+                        k2_emit(o, live, off, rssi, (s.flags >> 1) & 1u, ac_match<CH>(s.sr, p.ac_err), level);
                         s.flags &= ~2u;
                     }
                     n++;
@@ -762,7 +797,7 @@ WMB_D bool k2m_edge(const K2mParams &p, RlState &s, uint32_t st, int64_t m, uint
                 rl -= spb;
                 s.sr = ((s.sr << 1) | level) & CH::CODE_MASK;
                 if (n < K2_EDGE_EMIT_CAP) {
-                    k2_emit(o, live, off, rssi, (s.flags >> 1) & 1u, s.sr == CH::CODE, level);
+                    k2_emit(o, live, off, rssi, (s.flags >> 1) & 1u, ac_match<CH>(s.sr, p.ac_err), level);
                     s.flags &= ~2u;
                 }
                 n++;
@@ -1098,6 +1133,7 @@ struct K2p2Params {
     const RlState *carry;       /* exact state at batch start                               */
     RlState *p2_out;            /* out: a/b/sr after the last record, run = 1 marks it valid */
     uint64_t *agg;
+    uint32_t ac_err;            /* access-code bit errors accepted (wmb_set_receiver)       */
 };
 
 #define K2P2_BLK 8                   /* records fetched together (memory-level parallelism) */
@@ -1281,7 +1317,7 @@ WMB_D void k2p2w_c(const K2p2Params &p, uint32_t lane, uint32_t tid, const uint3
         const uint64_t head = ((uint64_t)(p.m_base + m[j]) << 24) | ((uint64_t)rs[j] << 16) | level;
         for (uint32_t k = 0; k < nn[j]; k++) {
             sr = ((sr << 1) | level) & 0xFFFFu;
-            const uint32_t sync = (sr == 0x543Du) ? 1u : 0u;
+            const uint32_t sync = ac_match<ChainT1C1>(sr, p.ac_err);
             p.ring[ord & p.ring_mask] = head | (pend << 2) | (sync << 1);
             pend = 0;
             if (sync) {

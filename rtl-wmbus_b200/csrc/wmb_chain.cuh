@@ -44,12 +44,17 @@
 #define WMB_MAXBITS_S1   (1 + 16 + 290 * 16)
 #define WMB_MAXBITS      WMB_MAXBITS_S1
 
+/* receiver settings (wmb_set_receiver): clock-lock threshold 1..WMB_LOCK_MAX, default 2 (rtl_wmbus.c:865-866); access-code
+ * bit errors up to CH::AC_ERR_MAX, default 0 (:99, :103) */
+#define WMB_LOCK_MAX     16
+
 struct ChainT1C1 {
     static constexpr int ID = 0;
     static constexpr int BOX = 8;                 /* rtl_wmbus.c:167 */
     static constexpr int NTAPS = 11;              /* rtl_wmbus.c:371 */
     static constexpr uint32_t CODE = 0x543Du;     /* rtl_wmbus.c:97  */
     static constexpr uint32_t CODE_MASK = 0xFFFFu;
+    static constexpr uint32_t AC_ERR_MAX = 3;     /* at 4 the preamble 0x5555 matches too          */
     static constexpr uint32_t RAW_MASK = 0x3Fu;   /* rtl_wmbus.c:733 */
     /* Chebyshev-I band-pass, per section {b1, b2, a1, a2} (rtl_wmbus.c:340-341); literals so that
      * they become instruction immediates */
@@ -64,6 +69,7 @@ struct ChainS1 {
     static constexpr int NTAPS = 46;              /* rtl_wmbus.c:383 */
     static constexpr uint32_t CODE = 0x547696u;   /* rtl_wmbus.c:101 */
     static constexpr uint32_t CODE_MASK = 0xFFFFFFu;
+    static constexpr uint32_t AC_ERR_MAX = 6;
     static constexpr uint32_t RAW_MASK = 0xFu;    /* rtl_wmbus.c:644 */
     /* rtl_wmbus.c:355-356 */
     static constexpr float B10 = 1.999994187, B20 = 0.9999941867, A10 = -1.92151475, A20 = 0.9918135499;
@@ -128,7 +134,8 @@ WMB_CONSTANT float c_iir_gain = 1.874981046e-06;
 struct IirState {
     float    dc_x, dc_y;        /* DC block (-o)           rtl_wmbus.c:497-515            */
     float    h[6];              /* biquad memories h1,h2 x 3 sections   iir.h:67-71       */
-    uint32_t clk3;              /* last three clock signs (bit0 newest) rtl_wmbus.c:1092  */
+    uint32_t clk3;              /* last L+1 clock signs (bit0 newest, L the clock-lock threshold, 2 by default; no
+                                   other bit set) rtl_wmbus.c:1092                                               */
     uint32_t pad;
 };
 

@@ -202,6 +202,10 @@ struct wmb_ctx {
     int64_t last_M = 0, prev_M = 0;
     int last_set = 0;
 
+    /* receiver settings per chain (wmb_set_receiver; they survive wmb_reset) */
+    uint32_t lock[WMB_N_CHAINS] = {2, 2};            /* clock-lock threshold, rtl_wmbus.c:865-866 */
+    uint32_t ac_err[WMB_N_CHAINS] = {0, 0};          /* access-code bit errors, :99, :103         */
+
     /* results */
     uint64_t win_lo = 0, win_hi = ~0ull;             /* line window (access-code match sample) */
     /* manual mode (opts.manual_frames): frames wait here for wmb_poll */
@@ -264,8 +268,13 @@ static int launch_k2a_lanes(wmb_ctx *c, int chain, const K2aParams &p, cudaStrea
     if (g_k2a_coop && p.t2 && !p.dc && p.M % 32 == 0 && p.W % 32 == 0 && p.C % 32 == 0 && p.hist % 32 == 0) {
         const unsigned per = (K2A2_THREADS / 32) * K2A2_LPW;
         const unsigned grid = (p.lanes + per - 1) / per;
-        if (chain == 0) k2a2_lanes_kernel<ChainT1C1><<<grid, K2A2_THREADS, 0, st>>>(p);
-        else            k2a2_lanes_kernel<ChainS1><<<grid, K2A2_THREADS, 0, st>>>(p);
+        if (p.lock == 2) {
+            if (chain == 0) k2a2_lanes_kernel<ChainT1C1, 2><<<grid, K2A2_THREADS, 0, st>>>(p);
+            else            k2a2_lanes_kernel<ChainS1, 2><<<grid, K2A2_THREADS, 0, st>>>(p);
+        } else {
+            if (chain == 0) k2a2_lanes_kernel<ChainT1C1, 0><<<grid, K2A2_THREADS, 0, st>>>(p);
+            else            k2a2_lanes_kernel<ChainS1, 0><<<grid, K2A2_THREADS, 0, st>>>(p);
+        }
         CUDA_TRY(cudaGetLastError());
         c->st.kernel_launches += 1;
         return WMB_OK;
@@ -971,7 +980,7 @@ static int run_batch(wmb_ctx *c, const uint8_t *src, size_t nbytes, cudaEvent_t 
             p.dbits = sb.dbits + wofs; p.sbits = sb.sbits + wofs;
             p.cbits = sb.cbits ? sb.cbits + wofs : nullptr;
             p.st_start = sb.ia_start; p.st_end = sb.ia_end; p.carry = b.ia_carry; p.rerun = sb.rerun_a;
-            p.dc = c->o.remove_dc; p.t2 = c->o.t2_enabled;
+            p.dc = c->o.remove_dc; p.t2 = c->o.t2_enabled; p.lock = c->lock[ch];
             p.mode = 0;
             p.spec0 = first ? 0u : 1u;                   /* the previous batch's lanes may still be running */
             c->st.lanes_run += lanes_a;
@@ -1033,6 +1042,7 @@ static int run_batch(wmb_ctx *c, const uint8_t *src, size_t nbytes, cudaEvent_t 
                 p.agg_cnt = s.agg; p.agg_tail = b.t2_agg_tail; p.agg_len = b.t2_agg_len;
                 p.m_base = (int64_t)c->m_consumed;
                 p.ring = s.ring; p.ring_mask = s.ring_cap - 1; p.sd = s.sd; p.cand = s.cand; p.cand_cap = c->cand_cap;
+                p.ac_err = c->ac_err[ch];
                 TRY(launch_k2t(c, ch, p));
             }
             CUDA_TRY(cudaEventRecord(c->ev_join, c->ts));
@@ -1056,7 +1066,7 @@ static int run_batch(wmb_ctx *c, const uint8_t *src, size_t nbytes, cudaEvent_t 
                 p.ev = b.s[WMB_ALGO_RLA].ev; p.cnt = b.s[WMB_ALGO_RLA].cnt;
                 p.st_start = b.rl_start; p.st_end = b.rl_end; p.carry = b.rl_carry; p.rerun = b.rerun;
                 p.errors = c->d_errors; p.lane_err = b.lane_err;
-                p.mode = 0; p.run_if = run_if;
+                p.mode = 0; p.run_if = run_if; p.ac_err = c->ac_err[ch];
                 if (!run_if) c->st.lanes_run += lanes;
                 return WMB_OK;
             };
@@ -1108,7 +1118,7 @@ static int run_batch(wmb_ctx *c, const uint8_t *src, size_t nbytes, cudaEvent_t 
                 if (p2.lanes > c->p2_lanes_max) return set_err(WMB_E_INVAL, "internal: phase-2 lanes");
                 p2.cnt = b.p2_cnt; p2.base = b.p2_base; p2.rssi = b.set[set].rssi + c->W; p2.m_base = (int64_t)c->m_consumed;
                 p2.ring = s.ring; p2.ring_mask = s.ring_cap - 1; p2.sd = s.sd; p2.cand = s.cand; p2.cand_cap = c->cand_cap;
-                p2.carry = b.rl_carry; p2.p2_out = b.p2_out; p2.agg = s.agg;
+                p2.carry = b.rl_carry; p2.p2_out = b.p2_out; p2.agg = s.agg; p2.ac_err = c->ac_err[0];
                 TRY(launch_k2p_rest(c, pc, p2));
                 /* the second reset rule (rtl_wmbus.c:756-762) fired somewhere in this batch (pd->fallback, set by phase
                  * 2, which then wrote nothing): redo T1/C1 with the exact monolithic lanes.  The kernels are always
@@ -1814,6 +1824,23 @@ extern "C" int wmb_seek(wmb_ctx *c, uint64_t first_iq_sample)
     return WMB_OK;
 }
 
+extern "C" int wmb_set_receiver(wmb_ctx *c, int chain, uint32_t clock_lock, uint32_t access_code_errors)
+{
+    if (!c) return set_err(WMB_E_INVAL, "null argument");
+    if (chain != WMB_CHAIN_T1C1 && chain != WMB_CHAIN_S1) return set_err(WMB_E_INVAL, "chain %d: 0 (T1/C1) or 1 (S1)", chain);
+    if (clock_lock < 1 || clock_lock > WMB_LOCK_MAX)
+        return set_err(WMB_E_INVAL, "clock lock %u out of range 1..%u", clock_lock, (unsigned)WMB_LOCK_MAX);
+    const uint32_t emax = chain == WMB_CHAIN_T1C1 ? ChainT1C1::AC_ERR_MAX : ChainS1::AC_ERR_MAX;
+    if (access_code_errors > emax)
+        return set_err(WMB_E_INVAL, "access-code errors %u out of range 0..%u for the %s chain", access_code_errors, emax,
+                       chain == WMB_CHAIN_T1C1 ? "T1/C1" : "S1");
+    if (c->batch_no != 0 || !c->remainder.empty())
+        return set_err(WMB_E_STATE, "wmb_set_receiver after samples were pushed (call it before the first push or after wmb_reset / wmb_seek)");
+    c->lock[chain] = clock_lock;
+    c->ac_err[chain] = access_code_errors;
+    return WMB_OK;
+}
+
 extern "C" int wmb_set_line_window(wmb_ctx *c, uint64_t sync_lo, uint64_t sync_hi)
 {
     if (!c || sync_lo > sync_hi) return set_err(WMB_E_INVAL, "bad window");
@@ -1850,6 +1877,8 @@ extern "C" long wmb_boundary_state(wmb_ctx *c, uint8_t *buf, size_t cap)
         ia.pad = 0;
         put(&ia, sizeof(ia));
         put(&rl, sizeof(rl));
+        const uint32_t rx[2] = { c->lock[ch], c->ac_err[ch] };        /* contexts with other receiver settings never agree */
+        put(rx, sizeof(rx));
         for (int a = 0; a < WMB_N_ALGOS; a++) {
             if ((a == WMB_ALGO_RLA && !c->o.rla_enabled) || (a == WMB_ALGO_T2A && !c->o.t2_enabled)) continue;
             Stream &s = b.s[a];

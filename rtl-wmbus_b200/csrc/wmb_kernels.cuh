@@ -934,7 +934,10 @@ WMB_D void k3_plan(const K3Params &p)
 /* last step of a batch (one thread, after K4): the record the host reads */
 WMB_D void k3_publish(const K3Params &p)
 {
-    const GatherDev &g = *p.gd;
+    GatherDev &g = *p.gd;
+    /* k3_carry counts every incomplete candidate but stores only pend_cap of them (and flags 64): the next gather and
+     * the host read n_pend entries of the list.  (A frame-word overflow marks every candidate of the batch incomplete.) */
+    for (int k = 0; k < WMB_N_STREAMS; k++) if (g.n_pend[k] > p.pend_cap) g.n_pend[k] = p.pend_cap;
     BatchRec r;
     r.n = g.n; r.n_words = g.n_words; r.pool_n = g.pool_n; r.errors = *p.errors;
     /* the capacity overflows (lane event buffer 1, frame words 4, datagram pool 8, matches 16, ring 32, pending candidates 64)

@@ -110,6 +110,7 @@ class Emitter:
     start_s: float = 0.01
     manufacturer: int = 0x5068
     seed: int = 1
+    sync_flips: tuple = ()       # chips of the access code sent inverted in every telegram, counted back from its last chip
     chip_rate: float = field(init=False)
 
     def __post_init__(self):
@@ -134,6 +135,14 @@ class Emitter:
         return bytes(p)
 
     def chips(self, k: int) -> np.ndarray:
+        c = self._chips(k)
+        if self.sync_flips:      # a receiver accepts these only with access-code errors allowed (wmb_set_receiver)
+            end = 2 * 40 + len(SYNC_S1) if self.mode == "S1" else 2 * 24 + len(SYNC_T1C1)
+            c = c.copy()
+            c[end - 1 - np.asarray(self.sync_flips)] ^= 1
+        return c
+
+    def _chips(self, k: int) -> np.ndarray:
         p = self.payload(k)
         if self.mode == "T1":
             return chips_t1(frame_a(p))
