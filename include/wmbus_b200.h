@@ -186,6 +186,33 @@ int  wmb_decode_frames(wmb_ctx *c, const wmb_frame *frames, size_t n);
  * sorting by it merges lines of several contexts (time-chunk sharding) into the reference's print order. */
 size_t wmb_take_lines(wmb_ctx *c, char *buf, size_t cap, size_t *n_lines, int timestamp_mode);
 
+/* What the receiver measured for one line, beside its text.  The carrier offset is the mean discriminator output over
+ * 32 nominal chips of the telegram's preamble, in decimated samples (800 kS/s) before the access-code match s:
+ * T1/C1 [s-384, s-128), S1 [s-1367, s-586), clipped to the samples pushed since the last wmb_reset / wmb_seek (n of
+ * them are left).  sum = sum over that window of rint(dphi * 2^24), dphi the post-FIR, pre-DC-block discriminator
+ * output (wmb_debug_copy_stage); exact, whatever the batch cut or thread order.
+ *   offset_hz = sum / n / 2^24 * 400 kHz / G, G the DC gain (sum of taps) of the chain's post-demod FIR,
+ * relative to carrier_hz, the carrier the chain listens to (0; +-325 kHz with -s; carrier_25khz[chain] * 25 kHz with
+ * simultaneous = 2).  Positive: the telegram lies above that carrier.  valid = 0 (offset_hz NaN) when n = 0, with -a
+ * (the cross-product discriminator is not a frequency), and for lines of frames handed to wmb_decode_frames. */
+typedef struct wmb_line_info {
+    uint64_t sync_sample;     /* decimated sample of the access-code match                                   */
+    uint64_t end_sample;      /* decimated sample of the telegram's last bit                                 */
+    uint8_t  chain;           /* WMB_CHAIN_*                                                                 */
+    uint8_t  algo;            /* WMB_ALGO_*                                                                  */
+    uint8_t  crc_ok;
+    uint8_t  valid;
+    uint32_t n;               /* samples in the window                                                      */
+    int64_t  sum;             /* sum of rint(dphi * 2^24) over the window                                    */
+    double   carrier_hz;
+    double   offset_hz;
+} wmb_line_info;
+
+/* wmb_take_lines that also fills info[i] for the i-th line taken; it takes at most info_cap lines (info == NULL: no
+ * records, no limit -- wmb_take_lines is this call).  Lines not taken stay queued. */
+size_t wmb_take_lines_info(wmb_ctx *c, char *buf, size_t cap, size_t *n_lines, int timestamp_mode,
+                           wmb_line_info *info, size_t info_cap);
+
 /* Convenience for offline captures: push + flush + decode + take_lines in one call.
  * `flush` as in wmb_poll.  Returns bytes written to out or a negative error. */
 long wmb_process(wmb_ctx *c, const uint8_t *cu8, size_t nbytes, int flush,

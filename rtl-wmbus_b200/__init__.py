@@ -10,8 +10,8 @@ missing.
 Import with ``importlib.import_module("rtl-wmbus_b200")`` (the directory name carries the
 reference's hyphen).
 """
-from .capi import (WmbOpts, WmbStats, WmbFrame, WmbusB200, load_library, library_path, build,
-                   opts_from_flags, LIB_NAME)
+from .capi import (WmbOpts, WmbStats, WmbFrame, WmbLineInfo, WmbusB200, load_library, library_path, build,
+                   opts_from_flags, line_info_dtype, LIB_NAME)
 
-__all__ = ["WmbOpts", "WmbStats", "WmbFrame", "WmbusB200", "load_library", "library_path", "build",
-           "opts_from_flags", "LIB_NAME"]
+__all__ = ["WmbOpts", "WmbStats", "WmbFrame", "WmbLineInfo", "WmbusB200", "load_library", "library_path", "build",
+           "opts_from_flags", "line_info_dtype", "LIB_NAME"]

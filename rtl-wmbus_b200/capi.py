@@ -24,6 +24,22 @@ class WmbFrame(C.Structure):
                 ("nbits", C.c_uint32), ("bits", C.POINTER(C.c_uint32))]
 
 
+class WmbLineInfo(C.Structure):
+    _fields_ = [("sync_sample", C.c_uint64), ("end_sample", C.c_uint64), ("chain", C.c_uint8), ("algo", C.c_uint8),
+                ("crc_ok", C.c_uint8), ("valid", C.c_uint8), ("n", C.c_uint32), ("sum", C.c_int64),
+                ("carrier_hz", C.c_double), ("offset_hz", C.c_double)]
+
+
+# numpy mirror of wmb_line_info (one record per line; see include/wmbus_b200.h)
+LINE_INFO_FIELDS = [("sync_sample", "<u8"), ("end_sample", "<u8"), ("chain", "u1"), ("algo", "u1"), ("crc_ok", "u1"),
+                    ("valid", "u1"), ("n", "<u4"), ("sum", "<i8"), ("carrier_hz", "<f8"), ("offset_hz", "<f8")]
+
+
+def line_info_dtype():
+    import numpy as np
+    return np.dtype(LINE_INFO_FIELDS)
+
+
 class WmbStats(C.Structure):
     _fields_ = [("input_samples", C.c_uint64), ("decimated_samples", C.c_uint64), ("batches", C.c_uint64),
                 ("kernel_launches", C.c_uint64), ("lanes_run", C.c_uint64), ("lanes_rerun", C.c_uint64),
@@ -61,6 +77,9 @@ def _bind(lib):
     lib.wmb_decode_frames.argtypes = [C.c_void_p, C.POINTER(WmbFrame), C.c_size_t]
     lib.wmb_take_lines.argtypes = [C.c_void_p, C.c_char_p, C.c_size_t, C.POINTER(C.c_size_t), C.c_int]
     lib.wmb_take_lines.restype = C.c_size_t
+    lib.wmb_take_lines_info.argtypes = [C.c_void_p, C.c_char_p, C.c_size_t, C.POINTER(C.c_size_t), C.c_int, C.c_void_p,
+                                        C.c_size_t]
+    lib.wmb_take_lines_info.restype = C.c_size_t
     lib.wmb_process.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.c_char_p, C.c_size_t,
                                 C.POINTER(C.c_size_t), C.c_int]
     lib.wmb_process.restype = C.c_long
@@ -87,7 +106,8 @@ def _bind(lib):
 EXPORTS = ["wmb_reset", "wmb_host_alloc", "wmb_host_free", "wmb_default_opts", "wmb_abi_version", "wmb_last_error", "wmb_version_string", "wmb_create",
            "wmb_destroy", "wmb_push", "wmb_push_device", "wmb_poll", "wmb_decode_frames", "wmb_take_lines",
            "wmb_process", "wmb_process_device", "wmb_get_stats", "wmb_debug_copy_stage", "wmb_debug_copy_bits", "wmb_debug_copy_events", "wmb_debug_arith",
-           "wmb_seek", "wmb_set_line_window", "wmb_boundary_state", "wmb_pending_before", "wmb_set_receiver"]
+           "wmb_seek", "wmb_set_line_window", "wmb_boundary_state", "wmb_pending_before", "wmb_set_receiver",
+           "wmb_take_lines_info"]
 
 
 def load_library(path: str | None = None):
@@ -177,22 +197,32 @@ class WmbusB200:
         """wmb_process* hands out only the lines that fit the buffer; the rest stay queued -- fetch them too"""
         return self.take_lines(timestamp_mode) if taken else []
 
-    def process(self, host_ptr, nbytes, flush=True, timestamp_mode=1, raw=False):
-        """host_ptr: int address / ctypes pointer of cu8 bytes in host memory."""
+    def process(self, host_ptr, nbytes, flush=True, timestamp_mode=1, raw=False, info=False):
+        """host_ptr: int address / ctypes pointer of cu8 bytes in host memory.
+        info=True: (lines, records), records a numpy structured array of wmb_line_info (line_info_dtype()), one per line"""
         nl = C.c_size_t(0)
+        if info:                                            # nothing taken by the call itself: every line gets its record
+            self._check(self.lib.wmb_process(self._ctx, host_ptr, nbytes, int(flush), self._out, 0, C.byref(nl),
+                                             timestamp_mode))
+            return self.take_lines(timestamp_mode, info=True)
         n = self._check(self.lib.wmb_process(self._ctx, host_ptr, nbytes, int(flush), self._out,
                                              len(self._out), C.byref(nl), timestamp_mode))
         if raw:
             return self._raw(n, nl.value, timestamp_mode)
         return self._lines(n) + self._drain(nl.value, timestamp_mode)
 
-    def process_bytes(self, data: bytes, flush=True, timestamp_mode=1):
+    def process_bytes(self, data: bytes, flush=True, timestamp_mode=1, info=False):
         buf = (C.c_uint8 * len(data)).from_buffer_copy(data)
-        return self.process(C.cast(buf, C.c_void_p), len(data), flush, timestamp_mode)
+        return self.process(C.cast(buf, C.c_void_p), len(data), flush, timestamp_mode, info=info)
 
-    def process_device(self, dev_ptr: int, nbytes: int, flush=True, timestamp_mode=1, raw=False):
-        """raw=True: the text exactly as the C ABI hands it out (bytes, one line per datagram), not a list of str"""
+    def process_device(self, dev_ptr: int, nbytes: int, flush=True, timestamp_mode=1, raw=False, info=False):
+        """raw=True: the text exactly as the C ABI hands it out (bytes, one line per datagram), not a list of str
+        info=True: (lines, records) as in process()"""
         nl = C.c_size_t(0)
+        if info:
+            self._check(self.lib.wmb_process_device(self._ctx, C.c_void_p(dev_ptr), nbytes, int(flush), self._out, 0,
+                                                    C.byref(nl), timestamp_mode))
+            return self.take_lines(timestamp_mode, info=True)
         n = self._check(self.lib.wmb_process_device(self._ctx, C.c_void_p(dev_ptr), nbytes, int(flush),
                                                     self._out, len(self._out), C.byref(nl), timestamp_mode))
         if raw:
@@ -237,15 +267,29 @@ class WmbusB200:
     def decode_frames(self, arr, n):
         self._check(self.lib.wmb_decode_frames(self._ctx, arr, n))
 
-    def take_lines(self, timestamp_mode=1):
+    def take_lines(self, timestamp_mode=1, info=False):
+        """info=True: (lines, records), records a numpy structured array of wmb_line_info, one per line"""
         nl = C.c_size_t(0)
         out = []
+        if not info:
+            while True:
+                n = self.lib.wmb_take_lines(self._ctx, self._out, len(self._out), C.byref(nl), timestamp_mode)
+                if not nl.value:
+                    break
+                out += self._lines(n)
+            return out
+        import numpy as np
+        cap = 1 << 14
+        recs = []
         while True:
-            n = self.lib.wmb_take_lines(self._ctx, self._out, len(self._out), C.byref(nl), timestamp_mode)
+            r = np.zeros(cap, line_info_dtype())
+            n = self.lib.wmb_take_lines_info(self._ctx, self._out, len(self._out), C.byref(nl), timestamp_mode,
+                                             r.ctypes.data, cap)
             if not nl.value:
                 break
             out += self._lines(n)
-        return out
+            recs.append(r[:nl.value])
+        return out, (np.concatenate(recs) if recs else np.zeros(0, line_info_dtype()))
 
     def reset(self):
         self._check(self.lib.wmb_reset(self._ctx))

@@ -17,6 +17,10 @@
  *   WMBUS_B200_ACCESS_CODE_ERRORS=<t1c1>[,<s1>]   access-code bit errors accepted, T1/C1 0..3, S1 0..6 (default 0,
  *                              ACCESS_CODE_*_ERRORS, rtl_wmbus.c:99, :103)
  *   One value sets both chains.  A malformed or out-of-range value is an error at start-up (wmb_set_receiver).
+ *   WMBUS_B200_LINE_INFO=<path>  write one record per stdout line, in the same order and flushed with it:
+ *                              ALGO;MODE;CRC_OK;LINK_LAYER_IDENT_NO;SYNC_SAMPLE;CARRIER_HZ;OFFSET_HZ (ALGO rla / t2a,
+ *                              OFFSET_HZ the telegram's carrier offset from CARRIER_HZ, or nan; wmb_line_info).  A path
+ *                              that cannot be opened is an error at start-up.  stdout does not change.
  */
 #define _GNU_SOURCE
 #include <errno.h>
@@ -95,14 +99,54 @@ static int parse_pair(const char *e, unsigned long v[2])
     return *end == 0 && v[0] <= 0xFFFFFFFFul && v[1] <= 0xFFFFFFFFul;
 }
 
-static int emit_lines(wmb_ctx *ctx, char *out, size_t outcap)
+/* WMBUS_B200_LINE_INFO: one record per stdout line, in the same order */
+static FILE *g_info_file = NULL;
+#define INFO_CAP 4096
+static wmb_line_info g_info[INFO_CAP];
+
+/* ALGO;MODE;CRC_OK;LINK_LAYER_IDENT_NO;SYNC_SAMPLE;CARRIER_HZ;OFFSET_HZ of each line of out[0..n) */
+static void write_info(const char *out, size_t n, size_t nl, int show_algorithm)
+{
+    const char *l = out;
+    for (size_t i = 0; i < nl && l < out + n; i++) {
+        const char *e = memchr(l, '\n', (size_t)(out + n - l));
+        if (!e) e = out + n;
+        /* fields of the line: [ALGO;]MODE;CRC_OK;3OUTOF6OK;TIMESTAMP;PACKET_RSSI;CURRENT_RSSI;LINK_LAYER_IDENT_NO;DATAGRAM */
+        const char *f[9];
+        int nf = 0;
+        const char *p = l;
+        if (show_algorithm) { p = memchr(p, ';', (size_t)(e - p)); p = p ? p + 1 : e; }
+        while (nf < 9) {
+            f[nf++] = p;
+            const char *q = memchr(p, ';', (size_t)(e - p));
+            if (!q) break;
+            p = q + 1;
+        }
+        const wmb_line_info *r = &g_info[i];
+        char off[32];
+        if (r->valid) snprintf(off, sizeof(off), "%.0f", r->offset_hz);
+        else snprintf(off, sizeof(off), "nan");
+        if (nf >= 8)
+            fprintf(g_info_file, "%s;%.*s;%u;%.*s;%llu;%.0f;%s\n", r->algo == WMB_ALGO_RLA ? "rla" : "t2a",
+                    (int)(f[1] - f[0] - 1), f[0], (unsigned)r->crc_ok, (int)(f[7] - f[6] - 1), f[6],
+                    (unsigned long long)r->sync_sample, r->carrier_hz, off);
+        l = e + 1;
+    }
+}
+
+static int emit_lines(wmb_ctx *ctx, char *out, size_t outcap, int show_algorithm)
 {
     for (;;) {
         size_t nl = 0;
-        const size_t n = wmb_take_lines(ctx, out, outcap, &nl, 0);
+        const size_t n = g_info_file ? wmb_take_lines_info(ctx, out, outcap, &nl, 0, g_info, INFO_CAP)
+                                     : wmb_take_lines(ctx, out, outcap, &nl, 0);
         if (!nl) return 0;
         fwrite(out, 1, n, stdout);
         fflush(stdout);                                 /* t1_c1_packet_decoder.h:698-699 */
+        if (g_info_file) {
+            write_info(out, n, nl, show_algorithm);
+            fflush(g_info_file);
+        }
     }
 }
 
@@ -180,6 +224,11 @@ int main(int argc, char *argv[])
         return EXIT_FAILURE;
     }
 
+    if ((e = getenv("WMBUS_B200_LINE_INFO")) != NULL && (g_info_file = fopen(e, "w")) == NULL) {
+        fprintf(stderr, "rtl_wmbus_b200: WMBUS_B200_LINE_INFO=%s: %s\n", e, strerror(errno));
+        return EXIT_FAILURE;
+    }
+
     wmb_ctx *ctx = NULL;
     if (wmb_create(&o, device, &ctx) != WMB_OK) {
         fprintf(stderr, "rtl_wmbus_b200: %s\n", wmb_last_error());
@@ -236,13 +285,13 @@ int main(int argc, char *argv[])
                 set_alarm(0);
                 const double t_in = now_s();
                 rc = wmb_push(ctx, buf, fill);
-                if (rc == WMB_OK) emit_lines(ctx, out, outcap);
+                if (rc == WMB_OK) emit_lines(ctx, out, outcap, o.show_algorithm);
                 deadline += now_s() - t_in;             /* the item's two seconds do not run during the hand-over */
                 const double left = deadline - now_s();
                 set_alarm(left > 1e-3 ? left : 1e-3);
             } else {
                 rc = wmb_push(ctx, buf, fill);
-                if (rc == WMB_OK) emit_lines(ctx, out, outcap);
+                if (rc == WMB_OK) emit_lines(ctx, out, outcap, o.show_algorithm);
             }
             if (rc != WMB_OK) break;
             fill = 0;
@@ -253,11 +302,15 @@ int main(int argc, char *argv[])
     if (rc == WMB_OK) {
         size_t nframes = 0;
         rc = wmb_poll(ctx, NULL, 0, &nframes, 1);       /* EOF: flush */
-        emit_lines(ctx, out, outcap);
+        emit_lines(ctx, out, outcap, o.show_algorithm);
     }
     if (rc != WMB_OK) fprintf(stderr, "rtl_wmbus_b200: %s\n", wmb_last_error());
     free(out);
     wmb_host_free(buf);
     wmb_destroy(ctx);
+    if (g_info_file && fclose(g_info_file) != 0 && rc == WMB_OK) {
+        fprintf(stderr, "rtl_wmbus_b200: WMBUS_B200_LINE_INFO: %s\n", strerror(errno));
+        return EXIT_FAILURE;
+    }
     return rc == WMB_OK ? EXIT_SUCCESS : EXIT_FAILURE;
 }

@@ -74,6 +74,7 @@ struct Stream {                     /* one (chain, algo) bit stream */
     StreamDev *sd = nullptr;        /* device bookkeeping                         */
     uint64_t *cand = nullptr;       /* device: new access-code matches (ordinals, unordered) */
     uint64_t *pend = nullptr;       /* device: candidates waiting for more bits   */
+    OfsAcc *pend_ofs = nullptr;     /* device: their carrier-offset sums          */
     uint64_t *agg = nullptr;        /* scan scratch [tiles]                       */
     uint64_t total = 0;             /* host mirror of sd->total at the last read  */
     uint64_t total_prev = 0;        /* ... before the last batch (stage tap)      */
@@ -118,7 +119,11 @@ struct QueuedLine {
     uint64_t end_sample;
     int prio;                       /* chain*2 + (algo == T2A) */
     wmb_decoded d;
-    uint8_t algo;
+    uint8_t algo, chain;
+    uint8_t ofs_valid;              /* 0: the frame came from the caller (wmb_decode_frames), no sum */
+    uint64_t sync_sample;           /* access-code match */
+    int64_t ofs_sum;                /* carrier-offset window (FrameHdr) */
+    uint32_t ofs_n;
 };
 
 struct wmb_ctx {
@@ -200,7 +205,9 @@ struct wmb_ctx {
     uint64_t batch_no = 0;          /* batches enqueued since create / reset: set = batch_no & 1 */
     uint64_t gather_no = 0;         /* gathers enqueued: result slot = gather_no % WMB_NSLOT    */
     int64_t last_M = 0, prev_M = 0;
+    int64_t last_hist = 0;          /* samples before the last batch's first one that exist since reset / seek (<= W) */
     int last_set = 0;
+    double fir_gain[WMB_N_CHAINS] = {1.0, 1.0};     /* DC gain of each chain's post-demod FIR (wmb_line_info.offset_hz) */
 
     /* receiver settings per chain (wmb_set_receiver; they survive wmb_reset) */
     uint32_t lock[WMB_N_CHAINS] = {2, 2};            /* clock-lock threshold, rtl_wmbus.c:865-866 */
@@ -685,6 +692,7 @@ static int ctx_alloc(wmb_ctx *c)
             TRY(dev_alloc(c, &s.sd, 1, true));
             TRY(dev_alloc(c, &s.cand, c->cand_cap));
             TRY(dev_alloc(c, &s.pend, c->pend_cap));
+            TRY(dev_alloc(c, &s.pend_ofs, c->pend_cap));
             TRY(dev_alloc(c, &s.agg, n_agg));
         }
     }
@@ -747,6 +755,31 @@ extern "C" int wmb_create(const wmb_opts *o, int cuda_device, wmb_ctx **out)
         if (!(c->chains & (1u << ch))) continue;
         c->W = std::max(c->W, c->W_a[ch]);
         if (o->rla_enabled) c->W = std::max(c->W, c->W_m[ch]);
+    }
+    /* the carrier-offset window of a match early in a batch reaches back into the dphi history prefix (S1: 1367
+     * samples).  A longer prefix changes no lane: they reach back W_a / W_m samples, clipped at the first sample pushed */
+    static_assert(WMB_OFS_HIST >= WMB_OFS_S1_LO && WMB_OFS_HIST >= WMB_OFS_T1C1_LO && WMB_OFS_HIST % 256 == 0,
+                  "the dphi history prefix must hold the longest carrier-offset window, in whole lane words");
+    c->W = std::max<uint32_t>(c->W, WMB_OFS_HIST);
+    {
+        /* DC gain of the post-demod FIR, from the tables the demod kernel uses */
+        float t[2][46];
+#ifdef WMB_HOSTSIM
+        memcpy(t[0], c_fir_t1c1, sizeof(c_fir_t1c1));
+        memcpy(t[1], c_fir_s1, sizeof(c_fir_s1));
+#else
+        if (cudaMemcpyFromSymbol(t[0], c_fir_t1c1, sizeof(c_fir_t1c1)) != cudaSuccess ||
+            cudaMemcpyFromSymbol(t[1], c_fir_s1, sizeof(c_fir_s1)) != cudaSuccess) {
+            delete c;
+            return set_err(WMB_E_CUDA, "cannot read the FIR tables");
+        }
+#endif
+        for (int ch = 0; ch < WMB_N_CHAINS; ch++) {
+            const int nt = ch == 0 ? ChainT1C1::NTAPS : ChainS1::NTAPS;
+            double g = 0.0;
+            for (int i = 0; i < nt; i++) g += (double)t[ch][i];
+            c->fir_gain[ch] = g;
+        }
     }
     c->manual = o->manual_frames != 0;
     c->taps = (o->reserved[1] & 1u) != 0;
@@ -1140,6 +1173,7 @@ static int run_batch(wmb_ctx *c, const uint8_t *src, size_t nbytes, cudaEvent_t 
         CUDA_TRY(cudaEventRecord(evt[3], c->cs));
     }
 
+    c->last_hist = c->hist_m;
     c->hist_m = std::min<int64_t>(c->hist_m + M, c->W);
     c->iq_consumed += (uint64_t)n_iq;
     c->m_consumed += (uint64_t)M;
@@ -1174,9 +1208,15 @@ static int enqueue_gather(wmb_ctx *c, bool final, bool after_batch)
                 Stream &s = c->cb[ch].s[a];
                 const int k = ch * WMB_N_ALGOS + a;
                 p.ring[k] = s.ring; p.ring_mask[k] = s.ring_cap - 1; p.sd[k] = s.sd; p.cand[k] = s.cand; p.pend[k] = s.pend;
+                p.pend_ofs[k] = s.pend_ofs;
             }
+            p.dphi[ch] = c->cb[ch].set[c->last_set].dphi;
         }
         p.pend_cap = c->pend_cap; p.cand_cap = c->cand_cap;
+        /* new matches are those of the batch just enqueued (a gather that closes no batch has none); k3_fill reads their
+         * carrier-offset windows from its dphi set */
+        p.m_first = (c->m_consumed - (uint64_t)c->last_M) & EVG_M_MASK;
+        p.prefix = c->W; p.clip = (uint32_t)c->last_hist; p.batch_m = after_batch ? (uint32_t)c->last_M : 0u;
         p.gd = c->d_gd; p.rec = c->d_rec + slot;
         p.hdr_log = c->d_hdr; p.dec_log = c->d_dec; p.log_base = (uint32_t)lb; p.log_cap = c->slot_cap;
         p.words = c->d_words; p.words_cap = c->frame_words_cap;
@@ -1197,6 +1237,8 @@ static int enqueue_gather(wmb_ctx *c, bool final, bool after_batch)
         }
     }
     CUDA_TRY(cudaEventRecord(c->ev_res[slot], c->cs));
+    /* ev_chain[set] releases the batch's set to the demod kernel of batch i+2 (run_batch waits for it on k1s): it is
+     * recorded here, behind the gather on cs, so k3_fill's reads of the set's dphi come before that kernel's writes */
     if (after_batch) {
         CUDA_TRY(cudaEventRecord(c->ev_chain[c->last_set], c->cs));
         c->chain_recorded[c->last_set] = true;
@@ -1521,7 +1563,7 @@ extern "C" int wmb_poll(wmb_ctx *c, wmb_frame *out, size_t cap, size_t *n, int f
  * that is receiving ignores further access-code matches (t1_c1_packet_decoder.h:272-278 honours the
  * flag only in idle), so a candidate inside the telegram of an earlier one is dropped; the rest
  * become lines, queued in the order the reference prints them. */
-struct FrameMeta { uint8_t chain, algo, partial, truncated; uint64_t ordinal, sync_sample; };
+struct FrameMeta { uint8_t chain, algo, partial, truncated, ofs_valid; uint64_t ordinal, sync_sample; int64_t ofs_sum; uint32_t ofs_n; };
 struct DecLite { int status; uint32_t consumed; uint64_t end_sample; uint8_t crc_ok; };
 
 template <class Meta, class Lite, class Fill>
@@ -1583,6 +1625,9 @@ static int book_frames(wmb_ctx *c, size_t n, Meta meta, Lite lite, Fill fill)
     for (size_t i = 0; i < fresh.size(); i++) {
         QueuedLine &q = c->lines[base + i];
         q.end_sample = fresh[i].end_sample; q.prio = (int)fresh[i].prio; q.algo = fresh[i].algo;
+        const FrameMeta m = meta(fresh[i].fi);
+        q.chain = m.chain; q.sync_sample = m.sync_sample;
+        q.ofs_valid = m.ofs_valid; q.ofs_sum = m.ofs_sum; q.ofs_n = m.ofs_n;
         fill(fresh[i].fi, q.d);
     }
     return WMB_OK;
@@ -1601,6 +1646,7 @@ static int book_device_frames(wmb_ctx *c, const FrameHdr *hdr, const DecHdr *dec
             const FrameHdr &h = hdr[idx[k]];
             FrameMeta m;
             m.chain = h.chain; m.algo = h.algo; m.ordinal = h.ordinal; m.sync_sample = h.sync_sample;
+            m.ofs_valid = 1; m.ofs_sum = h.ofs_sum; m.ofs_n = h.ofs_n;
             m.partial = (uint8_t)((!h.complete && !final) ? 1 : 0);
             m.truncated = (uint8_t)((h.complete && !h.cut) ? 0 : 1);
             return m;
@@ -1704,6 +1750,7 @@ extern "C" int wmb_decode_frames(wmb_ctx *c, const wmb_frame *frames, size_t n)
             FrameMeta m;
             m.chain = v[i]->chain; m.algo = v[i]->algo; m.ordinal = v[i]->ordinal; m.sync_sample = v[i]->sync_sample;
             m.partial = v[i]->reserved; m.truncated = v[i]->truncated;
+            m.ofs_valid = 0; m.ofs_sum = 0; m.ofs_n = 0;                   /* a caller's frame carries no sum */
             return m;
         },
         [&](size_t i) {
@@ -1714,13 +1761,23 @@ extern "C" int wmb_decode_frames(wmb_ctx *c, const wmb_frame *frames, size_t n)
         [&](size_t i, wmb_decoded &o) { o = dec[i]; });
 }
 
-extern "C" size_t wmb_take_lines(wmb_ctx *c, char *buf, size_t cap, size_t *n_lines, int timestamp_mode)
+/* the carrier a chain listens to, relative to the capture's centre frequency (the mixer of run_batch) */
+static double chain_carrier_hz(const wmb_ctx *c, int chain)
+{
+    if (c->o.simultaneous == 2) return 25e3 * (double)c->o.carrier_25khz[chain];
+    if (c->o.simultaneous) return chain == 0 ? 325e3 : -325e3;
+    return 0.0;
+}
+
+extern "C" size_t wmb_take_lines_info(wmb_ctx *c, char *buf, size_t cap, size_t *n_lines, int timestamp_mode,
+                                      wmb_line_info *info, size_t info_cap)
 {
     size_t len = 0, taken = 0;
     if (n_lines) *n_lines = 0;
     if (!c || !buf) return 0;
     char ts[64];
     for (; taken < c->lines.size(); taken++) {
+        if (info && taken >= info_cap) break;
         const QueuedLine &q = c->lines[taken];
         if (timestamp_mode == 1) snprintf(ts, sizeof(ts), "TS");
         else if (timestamp_mode == 2) snprintf(ts, sizeof(ts), "@%014llu.%d", (unsigned long long)q.end_sample, q.prio);
@@ -1731,11 +1788,27 @@ extern "C" size_t wmb_take_lines(wmb_ctx *c, char *buf, size_t cap, size_t *n_li
         if (len + l + 1 > cap) break;
         memcpy(buf + len, line, l);
         len += l;
+        if (info) {
+            wmb_line_info &r = info[taken];
+            memset(&r, 0, sizeof(r));
+            r.sync_sample = q.sync_sample; r.end_sample = q.end_sample;
+            r.chain = q.chain; r.algo = q.algo; r.crc_ok = q.d.crc_ok;
+            /* -a: the cross-product discriminator is not a frequency */
+            r.valid = (uint8_t)(q.ofs_valid && q.ofs_n > 0 && c->o.accurate_atan ? 1 : 0);
+            r.n = q.ofs_n; r.sum = q.ofs_sum;
+            r.carrier_hz = chain_carrier_hz(c, q.chain);
+            r.offset_hz = r.valid ? (double)q.ofs_sum / (double)q.ofs_n / (double)WMB_OFS_SCALE * 400e3 / c->fir_gain[q.chain] : NAN;
+        }
     }
     if (len < cap) buf[len] = 0;
     c->lines.erase(c->lines.begin(), c->lines.begin() + (long)taken);
     if (n_lines) *n_lines = taken;
     return len;
+}
+
+extern "C" size_t wmb_take_lines(wmb_ctx *c, char *buf, size_t cap, size_t *n_lines, int timestamp_mode)
+{
+    return wmb_take_lines_info(c, buf, cap, n_lines, timestamp_mode, nullptr, 0);
 }
 
 extern "C" long wmb_process(wmb_ctx *c, const uint8_t *cu8, size_t nbytes, int flush,
@@ -1785,7 +1858,7 @@ extern "C" int wmb_reset(wmb_ctx *c)
         if (st && cudaStreamQuery(st) != cudaSuccess) CUDA_TRY(cudaStreamSynchronize(st));
     c->iq_consumed = 0; c->m_consumed = 0; c->hist_m = 0; c->hist_iq = 0;
     c->remainder.clear(); c->lines.clear(); c->held.clear(); c->held_prev.clear();
-    c->batch_no = 0; c->last_M = 0; c->prev_M = 0; c->last_set = 0; c->inflight.clear();
+    c->batch_no = 0; c->last_M = 0; c->prev_M = 0; c->last_hist = 0; c->last_set = 0; c->inflight.clear();
     c->chain_recorded[0] = c->chain_recorded[1] = false;
     c->stat_rerun_seen = 0; c->stat_fallback_seen = 0;
     for (int ch = 0; ch < WMB_N_CHAINS; ch++)

@@ -842,16 +842,34 @@ WMB_D void k2c_compact(const K2cParams &p, uint32_t lane, int tid, int nthr)
 
 #define WMB_N_STREAMS (WMB_N_CHAINS * WMB_N_ALGOS)          /* stream k = chain * WMB_N_ALGOS + algo */
 
+/* Carrier offset of a candidate (DESIGN §8): the sum of rint(dphi * 2^24) over 32 nominal preamble chips that end one
+ * access-code length before the match, in decimated samples before it -- T1/C1 (8 samples per chip) [s-384, s-128),
+ * S1 (24.414 samples per chip) [s-1367, s-586) -- clipped to the samples pushed since the last reset / seek */
+#define WMB_OFS_T1C1_LO 384
+#define WMB_OFS_T1C1_HI 128
+#define WMB_OFS_S1_LO   1367
+#define WMB_OFS_S1_HI   586
+#define WMB_OFS_HIST    1536        /* least dphi history prefix (samples): the longest window, in whole 256-sample units */
+#define WMB_OFS_SCALE   16777216.f  /* 2^24: exact scaling, integer terms, a sum that does not depend on the order */
+
+struct OfsAcc {                     /* a carried candidate's sum (beside its ordinal in pend[k]) */
+    int64_t  sum;
+    uint32_t n;
+    uint32_t pad;
+};
+
 struct FrameHdr {                   /* one per candidate, device -> host                   */
     uint64_t ordinal;
     uint64_t sync_sample;
+    int64_t  ofs_sum;               /* carrier offset: sum of rint(dphi * 2^24) over the window */
     uint32_t nbits;                 /* events shipped (>= 1)                               */
     uint32_t word_off;              /* offset into the frame word buffer                   */
     uint8_t  chain, algo;
     uint8_t  complete;              /* 1: all bits the header can ask for (or cut by a reset) */
     uint8_t  overflow;              /* (unused)                                            */
     uint8_t  cut;                   /* 1: list ends at a run-length reset                  */
-    uint8_t  pad[3];
+    uint8_t  pad;
+    uint16_t ofs_n;                 /* samples in the carrier-offset window after clipping  */
 };
 
 struct GatherDev {                  /* device-resident state of the gather, one per context */
@@ -882,7 +900,13 @@ struct K3Params {
     StreamDev *sd[WMB_N_STREAMS];   /* null: stream not enabled                             */
     const uint64_t *cand[WMB_N_STREAMS];   /* new matches, unordered                        */
     uint64_t *pend[WMB_N_STREAMS];  /* carried candidates, ordered                          */
+    OfsAcc *pend_ofs[WMB_N_STREAMS];/* their carrier-offset sums, same slots                */
     uint32_t pend_cap, cand_cap;
+    /* the carrier-offset windows of new matches are read from this batch's dphi set: [prefix | batch_m samples], batch
+     * sample 0 = decimated sample m_first (40 bits); `clip` samples before it exist since the last reset / seek */
+    const float *dphi[WMB_N_CHAINS];
+    uint64_t m_first;
+    uint32_t prefix, clip, batch_m;
     GatherDev *gd;
     BatchRec *rec;                  /* this batch's record (its result slot)                */
     FrameHdr *hdr_log; DecHdr *dec_log;
@@ -966,14 +990,43 @@ WMB_D void k3_fill(const K3Params &p, uint32_t i, uint32_t part, uint32_t nparts
     uint32_t rank = 0;
     for (uint32_t q = part; q < np; q += nparts) rank += (p.pend[k][q] < key) ? 1u : 0u;
     for (uint32_t q = part; q < nn; q += nparts) rank += (p.cand[k][q] < key) ? 1u : 0u;
+    /* a new match: the sum over its carrier-offset window (a carried one brings its sum along).  The match lies in this
+     * batch; the window may reach back into the set's history prefix, never past the first sample pushed */
+    const bool fresh = live && j >= np;
+    const int chain = k / WMB_N_ALGOS;
+    int64_t lo = 0, hi = 0;
+    if (fresh) {
+        const uint64_t s = EVG_M(p.ring[k][key & p.ring_mask[k]]);
+        const int64_t rel = (int64_t)((s - p.m_first) & EVG_M_MASK);
+        if (rel < (int64_t)p.batch_m) {
+            lo = rel - (chain == 0 ? WMB_OFS_T1C1_LO : WMB_OFS_S1_LO);
+            hi = rel - (chain == 0 ? WMB_OFS_T1C1_HI : WMB_OFS_S1_HI);
+            if (lo < -(int64_t)p.clip) lo = -(int64_t)p.clip;
+            if (hi < lo) hi = lo;
+        }
+    }
+    const float *dphi = fresh ? p.dphi[chain] + p.prefix : nullptr;
+    int64_t sum = 0;
+    for (int64_t q = lo + (int64_t)part; q < hi; q += nparts) {
+#ifdef WMB_HOSTSIM
+        sum += (int64_t)llrintf(dphi[q] * WMB_OFS_SCALE);
+#else
+        sum += __float2ll_rn(dphi[q] * WMB_OFS_SCALE);    /* 64-bit: -a's cross products reach 2^15 before scaling */
+#endif
+    }
 #ifndef WMB_HOSTSIM
-    for (uint32_t d = nparts >> 1; d > 0; d >>= 1) rank += __shfl_xor_sync(0xFFFFFFFFu, rank, d);
+    for (uint32_t d = nparts >> 1; d > 0; d >>= 1) {
+        rank += __shfl_xor_sync(0xFFFFFFFFu, rank, d);
+        sum += __shfl_xor_sync(0xFFFFFFFFu, sum, d);
+    }
 #endif
     if (!live || part != 0) return;
     FrameHdr h;
     h.ordinal = key; h.sync_sample = 0; h.nbits = 0; h.word_off = 0; h.complete = 0; h.overflow = 0; h.cut = 0;
-    h.pad[0] = h.pad[1] = h.pad[2] = 0;
-    h.chain = (uint8_t)(k / WMB_N_ALGOS); h.algo = (uint8_t)(k % WMB_N_ALGOS);
+    h.pad = 0;
+    if (fresh) { h.ofs_sum = sum; h.ofs_n = (uint16_t)(hi - lo); }
+    else { const OfsAcc a = p.pend_ofs[k][j]; h.ofs_sum = a.sum; h.ofs_n = (uint16_t)a.n; }
+    h.chain = (uint8_t)chain; h.algo = (uint8_t)(k % WMB_N_ALGOS);
     p.hdr_log[g.base + g.off[k] + rank] = h;
 }
 
@@ -1143,7 +1196,11 @@ WMB_D void k3_carry(const K3Params &p, uint32_t i)
 #else
     const uint32_t slot = atomicAdd(&g.n_pend[k], 1u);
 #endif
-    if (slot < p.pend_cap) p.pend[k][slot] = h.ordinal;
+    if (slot < p.pend_cap) {
+        p.pend[k][slot] = h.ordinal;
+        OfsAcc a; a.sum = h.ofs_sum; a.n = h.ofs_n; a.pad = 0;
+        p.pend_ofs[k][slot] = a;
+    }
     else k3_flag(p.errors, 64u);
 }
 

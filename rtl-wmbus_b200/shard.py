@@ -62,13 +62,21 @@ def blank_position(line: str) -> str:
     return ";".join(f)
 
 
-def merge_lines(parts):
+def merge_lines(parts, infos=None):
     """Lines of several time chunks (each taken with timestamp_mode=2) -> the sequential run's print order, with the
     TIMESTAMP column blanked.  Within one chunk the order is already right; across chunks a telegram that started in
-    chunk g may finish after one that started in chunk g+1, so the merge is by print position (stable)."""
+    chunk g may finish after one that started in chunk g+1, so the merge is by print position (stable).
+    infos: the chunks' line records (numpy arrays of wmb_line_info, one per line): returns (lines, records) then, the
+    records in the same order."""
     flat = [l for part in parts for l in part]
-    flat.sort(key=line_key)
-    return [blank_position(l) for l in flat]
+    order = sorted(range(len(flat)), key=lambda i: line_key(flat[i]))
+    lines = [blank_position(flat[i]) for i in order]
+    if infos is None:
+        return lines
+    import numpy as np
+    recs = np.concatenate(infos)
+    assert len(recs) == len(flat), "one record per line"
+    return lines, recs[np.asarray(order, np.int64)]
 
 
 def chunk_bounds(n_bytes: int, d: int, world: int):
@@ -78,12 +86,22 @@ def chunk_bounds(n_bytes: int, d: int, world: int):
     return [min(n_iq, (n_iq * g // world) // gran * gran) for g in range(world)] + [n_iq]
 
 
-def decode_time_chunk(ctx, push, n_bytes: int, d: int, rank: int, world: int, halo_m: int = 1 << 18):
+def decode_time_chunk(ctx, push, n_bytes: int, d: int, rank: int, world: int, halo_m: int = 1 << 18, info=False):
     """Decode rank `rank`'s chunk of a capture of n_bytes cu8 bytes.  `push(byte_lo, byte_hi)` feeds that byte
     range of the capture to ctx (host or device memory: the caller's business).
     Returns (lines, digest_start, digest_end, halo_start_iq): digest_start is None for a chunk that starts at 0.
-    The lines carry their print position in the TIMESTAMP column (timestamp_mode 2) for merge_lines()."""
+    The lines carry their print position in the TIMESTAMP column (timestamp_mode 2) for merge_lines().
+    info=True: lines is (lines, records), the records (wmb_line_info) of the lines.  A line's carrier-offset window lies
+    in the chunk that holds its match, far behind the halo's start, so the records are the sequential run's."""
     import hashlib
+    recs = []
+
+    def take():
+        if not info:
+            return ctx.take_lines(2)
+        got, r = ctx.take_lines(2, info=True)
+        recs.append(r)
+        return got
     k = chunk_bounds(n_bytes, d, world)
     lo, hi = k[rank], k[rank + 1]
     gran = 2048 * d
@@ -94,11 +112,11 @@ def decode_time_chunk(ctx, push, n_bytes: int, d: int, rank: int, world: int, ha
     dig_start = None
     if start < lo:
         push(2 * start, 2 * lo)
-        lines += ctx.take_lines(2)
+        lines += take()
     if lo > 0:
         dig_start = hashlib.sha256(ctx.boundary_state()).digest()
     push(2 * lo, 2 * hi)
-    lines += ctx.take_lines(2)
+    lines += take()
     dig_end = hashlib.sha256(ctx.boundary_state()).digest()
     if rank + 1 < world:                              # finish the telegrams that started in the chunk
         step = (MAX_TELEGRAM_M * d + gran - 1) // gran * gran
@@ -116,13 +134,16 @@ def decode_time_chunk(ctx, push, n_bytes: int, d: int, rank: int, world: int, ha
         if n_bytes > 2 * hi:
             push(2 * hi, n_bytes)                     # the ragged end of the capture (the reference drops a short item)
         ctx.poll_flush()
-    lines += ctx.take_lines(2)
+    lines += take()
+    if info:
+        import numpy as np
+        lines = (lines, np.concatenate(recs))
     return lines, dig_start, dig_end, start
 
 
-def decode_time_sharded(ctx, push, n_bytes: int, d: int, halo_m: int = 1 << 18):
+def decode_time_sharded(ctx, push, n_bytes: int, d: int, halo_m: int = 1 << 18, info=False):
     """All ranks: decode one capture in time chunks, exact by construction (see module docstring).
-    Returns (my_lines, rounds)."""
+    Returns (my_lines, rounds); info=True: my_lines is (lines, records) as in decode_time_chunk."""
     rank = dist.get_rank() if dist.is_initialized() else 0
     world = dist.get_world_size() if dist.is_initialized() else 1
     rounds = 0
@@ -131,7 +152,7 @@ def decode_time_sharded(ctx, push, n_bytes: int, d: int, halo_m: int = 1 << 18):
     while True:
         rounds += 1
         if redo:
-            lines, ds, de, start = decode_time_chunk(ctx, push, n_bytes, d, rank, world, halo_m)
+            lines, ds, de, start = decode_time_chunk(ctx, push, n_bytes, d, rank, world, halo_m, info=info)
         mine = torch.zeros(65, dtype=torch.uint8)
         mine[:32] = torch.frombuffer(bytearray(ds or bytes(32)), dtype=torch.uint8)
         mine[32:64] = torch.frombuffer(bytearray(de), dtype=torch.uint8)
