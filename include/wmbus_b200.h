@@ -213,6 +213,55 @@ typedef struct wmb_line_info {
 size_t wmb_take_lines_info(wmb_ctx *c, char *buf, size_t cap, size_t *n_lines, int timestamp_mode,
                            wmb_line_info *info, size_t info_cap);
 
+/* ---- burst report: every signal burst on a chain, decoded or not ------------------------------------------------
+ * Off by default.  wmb_set_bursts(ctx, chain, level) with level 1..255 turns it on for a chain.  On the chain's
+ * (unsigned)rssi[m] (the scale of the PACKET_RSSI column; wmb_debug_copy_stage) and dphi[m], in decimated samples
+ * (800 kS/s):
+ *   1. above[m] = rssi[m] >= level.  Samples before the first one pushed since wmb_reset / wmb_seek are below.
+ *   2. Bridge: a stretch of fewer than G below samples with an above sample on both sides counts as above.  This gives
+ *      maximal runs [s, e), e one past the last above sample.
+ *   3. Cut: a run is cut at every multiple of P = 2^16 (global decimated index) at least Q = 2^17 samples after its
+ *      start s.  No telegram is that long, so none is cut; and a piece depends on at most Q + P + G earlier samples, so
+ *      a time chunk with a 2^18-sample left halo reports the pieces of the sequential run.  A piece after a cut has
+ *      WMB_BURST_CONTINUED, a piece ending at one WMB_BURST_CUT.
+ *   4. Pieces of at least Lmin samples are reported, with peak = max rssi, rssi_sum = sum of rssi over [start, end),
+ *      and the carrier offset as in wmb_line_info over the window [start + g0, min(end, start + g0 + w)) (n samples,
+ *      sum = sum of rint(dphi * 2^24)): offset_hz = sum / n / 2^24 * 400 kHz / G_fir relative to carrier_hz.
+ *      valid = 0 (offset_hz NaN) with -a or when n = 0.
+ *   5. At end of input (flush) a run still open is closed one past its last above sample, WMB_BURST_AT_END.
+ *              G (bridge)   Lmin   g0    w
+ *     T1/C1    64           256    64    256      (8 chips, 32 chips, 8 chips, 32 chips)
+ *     S1       196          782    196   781
+ * A piece is handed out once it is closed and no piece still to come can start before it: wmb_take_bursts returns
+ * them ordered by (start_sample, chain).  Join them with lines on sync_sample in [start_sample, end_sample) of the same
+ * chain. */
+#define WMB_BURST_CONTINUED 1u
+#define WMB_BURST_CUT       2u
+#define WMB_BURST_AT_END    4u
+
+typedef struct wmb_burst {
+    uint64_t start_sample;    /* decimated sample of the piece's first sample                                */
+    uint64_t end_sample;      /* one past its last sample                                                    */
+    uint64_t rssi_sum;        /* sum of (unsigned)rssi over [start_sample, end_sample)                       */
+    int64_t  sum;             /* sum of rint(dphi * 2^24) over the offset window                             */
+    double   carrier_hz;
+    double   offset_hz;
+    uint32_t n;               /* samples in the offset window                                                */
+    uint8_t  chain;           /* WMB_CHAIN_*                                                                 */
+    uint8_t  peak;            /* max (unsigned)rssi                                                          */
+    uint8_t  valid;
+    uint8_t  flags;           /* WMB_BURST_*                                                                 */
+} wmb_burst;
+
+/* level 0 (default): off; 1..255: on.  Valid before the first push or right after wmb_reset / wmb_seek (else
+ * WMB_E_STATE); a bad chain or level > 255 gives WMB_E_INVAL.  The level survives wmb_reset and wmb_seek.  A chain
+ * that the options turn off reports nothing. */
+int wmb_set_bursts(wmb_ctx *c, int chain, uint32_t level);
+
+/* Copy up to cap closed pieces into out, ordered by (start_sample, chain); *n receives their number.  Pieces not
+ * taken stay queued. */
+int wmb_take_bursts(wmb_ctx *c, wmb_burst *out, size_t cap, size_t *n);
+
 /* Convenience for offline captures: push + flush + decode + take_lines in one call.
  * `flush` as in wmb_poll.  Returns bytes written to out or a negative error. */
 long wmb_process(wmb_ctx *c, const uint8_t *cu8, size_t nbytes, int flush,

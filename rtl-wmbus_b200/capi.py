@@ -40,6 +40,18 @@ def line_info_dtype():
     return np.dtype(LINE_INFO_FIELDS)
 
 
+# numpy mirror of wmb_burst (one record per burst piece; see include/wmbus_b200.h)
+BURST_FIELDS = [("start_sample", "<u8"), ("end_sample", "<u8"), ("rssi_sum", "<u8"), ("sum", "<i8"),
+                ("carrier_hz", "<f8"), ("offset_hz", "<f8"), ("n", "<u4"), ("chain", "u1"), ("peak", "u1"),
+                ("valid", "u1"), ("flags", "u1")]
+BURST_CONTINUED, BURST_CUT, BURST_AT_END = 1, 2, 4
+
+
+def burst_dtype():
+    import numpy as np
+    return np.dtype(BURST_FIELDS)
+
+
 class WmbStats(C.Structure):
     _fields_ = [("input_samples", C.c_uint64), ("decimated_samples", C.c_uint64), ("batches", C.c_uint64),
                 ("kernel_launches", C.c_uint64), ("lanes_run", C.c_uint64), ("lanes_rerun", C.c_uint64),
@@ -96,6 +108,8 @@ def _bind(lib):
     lib.wmb_seek.argtypes = [C.c_void_p, C.c_uint64]
     lib.wmb_set_line_window.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64]
     lib.wmb_set_receiver.argtypes = [C.c_void_p, C.c_int, C.c_uint32, C.c_uint32]
+    lib.wmb_set_bursts.argtypes = [C.c_void_p, C.c_int, C.c_uint32]
+    lib.wmb_take_bursts.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
     lib.wmb_boundary_state.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
     lib.wmb_boundary_state.restype = C.c_long
     lib.wmb_pending_before.argtypes = [C.c_void_p, C.c_uint64]
@@ -107,7 +121,7 @@ EXPORTS = ["wmb_reset", "wmb_host_alloc", "wmb_host_free", "wmb_default_opts", "
            "wmb_destroy", "wmb_push", "wmb_push_device", "wmb_poll", "wmb_decode_frames", "wmb_take_lines",
            "wmb_process", "wmb_process_device", "wmb_get_stats", "wmb_debug_copy_stage", "wmb_debug_copy_bits", "wmb_debug_copy_events", "wmb_debug_arith",
            "wmb_seek", "wmb_set_line_window", "wmb_boundary_state", "wmb_pending_before", "wmb_set_receiver",
-           "wmb_take_lines_info"]
+           "wmb_take_lines_info", "wmb_set_bursts", "wmb_take_bursts"]
 
 
 def load_library(path: str | None = None):
@@ -151,9 +165,12 @@ def opts_from_flags(lib, flags: str = "", **kw) -> WmbOpts:
 class WmbusB200:
     """One decoding context (== one rtl_wmbus process) on one GPU.
     clock_lock=(t1c1, s1), access_code_errors=(t1c1, s1): receiver settings, see wmb_set_receiver() (default (2, 2) and
-    (0, 0), the reference's).  They survive reset() and seek()."""
+    (0, 0), the reference's).  They survive reset() and seek().
+    burst_level=(t1c1, s1): the burst report's level per chain, see wmb_set_bursts() (0: off, the default); it survives
+    reset() and seek() too.  take_bursts() hands out the closed pieces."""
 
-    def __init__(self, flags: str = "", device: int = 0, lib=None, clock_lock=None, access_code_errors=None, **tuning):
+    def __init__(self, flags: str = "", device: int = 0, lib=None, clock_lock=None, access_code_errors=None,
+                 burst_level=None, **tuning):
         self.lib = lib or load_library()
         self.opts = opts_from_flags(self.lib, flags, **tuning)
         self._ctx = C.c_void_p()
@@ -167,6 +184,13 @@ class WmbusB200:
             try:
                 for chain in (0, 1):
                     self.set_receiver(chain, lock[chain], errs[chain])
+            except Exception:
+                self.close()
+                raise
+        if burst_level is not None:
+            try:
+                for chain in (0, 1):
+                    self.set_bursts(chain, burst_level[chain])
             except Exception:
                 self.close()
                 raise
@@ -301,6 +325,26 @@ class WmbusB200:
     def set_receiver(self, chain: int, clock_lock: int, access_code_errors: int):
         """clock-lock threshold and access-code bit errors of one chain (before the first push, or after reset/seek)"""
         self._check(self.lib.wmb_set_receiver(self._ctx, chain, clock_lock, access_code_errors))
+
+    def set_bursts(self, chain: int, level: int):
+        """burst report level of one chain, 0 = off (before the first push, or after reset/seek)"""
+        self._check(self.lib.wmb_set_bursts(self._ctx, chain, level))
+
+    def take_bursts(self):
+        """the closed burst pieces not taken yet, ordered by (start_sample, chain): a numpy structured array of
+        wmb_burst (burst_dtype())"""
+        import numpy as np
+        cap = 1 << 14
+        parts = []
+        while True:
+            r = np.zeros(cap, burst_dtype())
+            n = C.c_size_t(0)
+            self._check(self.lib.wmb_take_bursts(self._ctx, r.ctypes.data, cap, C.byref(n)))
+            if n.value:
+                parts.append(r[:n.value])
+            if n.value < cap:
+                break
+        return np.concatenate(parts) if parts else np.zeros(0, burst_dtype())
 
     def set_line_window(self, sync_lo: int, sync_hi: int):
         self._check(self.lib.wmb_set_line_window(self._ctx, sync_lo, sync_hi))

@@ -21,6 +21,11 @@
  *                              ALGO;MODE;CRC_OK;LINK_LAYER_IDENT_NO;SYNC_SAMPLE;CARRIER_HZ;OFFSET_HZ (ALGO rla / t2a,
  *                              OFFSET_HZ the telegram's carrier offset from CARRIER_HZ, or nan; wmb_line_info).  A path
  *                              that cannot be opened is an error at start-up.  stdout does not change.
+ *   WMBUS_B200_BURSTS=<path>   write one record per burst piece of either chain, decoded or not (wmb_take_bursts),
+ *                              flushed after each hand-over: CHAIN;START_SAMPLE;END_SAMPLE;PEAK_RSSI;MEAN_RSSI;CARRIER_HZ;
+ *                              OFFSET_HZ;FLAGS (CHAIN T1C1 / S1, OFFSET_HZ nan when not valid, FLAGS 1 continued, 2 cut,
+ *                              4 at end of input).  A path that cannot be opened is an error at start-up.
+ *   WMBUS_B200_BURST_LEVEL=<t1c1>[,<s1>]  the bursts' rssi level, 1..255 (0: that chain off; default 14).
  */
 #define _GNU_SOURCE
 #include <errno.h>
@@ -134,8 +139,37 @@ static void write_info(const char *out, size_t n, size_t nl, int show_algorithm)
     }
 }
 
+/* WMBUS_B200_BURSTS: one record per closed burst piece, CHAIN;START_SAMPLE;END_SAMPLE;PEAK_RSSI;MEAN_RSSI;CARRIER_HZ;
+ * OFFSET_HZ;FLAGS.  The default level: the lowest at which the committed captures show no burst of noise alone, with
+ * every CRC-ok line inside a burst (DESIGN.md 8) */
+#define BURST_LEVEL_DEFAULT 14ul
+static FILE *g_burst_file = NULL;
+#define BURST_CAP 1024
+static wmb_burst g_bursts[BURST_CAP];
+
+static void emit_bursts(wmb_ctx *ctx)
+{
+    if (!g_burst_file) return;
+    for (;;) {
+        size_t n = 0;
+        if (wmb_take_bursts(ctx, g_bursts, BURST_CAP, &n) != WMB_OK || !n) break;
+        for (size_t i = 0; i < n; i++) {
+            const wmb_burst *b = &g_bursts[i];
+            char off[32];
+            if (b->valid) snprintf(off, sizeof(off), "%.0f", b->offset_hz);
+            else snprintf(off, sizeof(off), "nan");
+            fprintf(g_burst_file, "%s;%llu;%llu;%u;%.1f;%.0f;%s;%u\n", b->chain == WMB_CHAIN_T1C1 ? "T1C1" : "S1",
+                    (unsigned long long)b->start_sample, (unsigned long long)b->end_sample, (unsigned)b->peak,
+                    (double)b->rssi_sum / (double)(b->end_sample - b->start_sample), b->carrier_hz, off, (unsigned)b->flags);
+        }
+        if (n < BURST_CAP) break;
+    }
+    fflush(g_burst_file);
+}
+
 static int emit_lines(wmb_ctx *ctx, char *out, size_t outcap, int show_algorithm)
 {
+    emit_bursts(ctx);
     for (;;) {
         size_t nl = 0;
         const size_t n = g_info_file ? wmb_take_lines_info(ctx, out, outcap, &nl, 0, g_info, INFO_CAP)
@@ -224,6 +258,16 @@ int main(int argc, char *argv[])
         return EXIT_FAILURE;
     }
 
+    unsigned long burst_level[2] = { BURST_LEVEL_DEFAULT, BURST_LEVEL_DEFAULT };
+    if ((e = getenv("WMBUS_B200_BURST_LEVEL")) != NULL && (!parse_pair(e, burst_level) || burst_level[0] > 255 || burst_level[1] > 255)) {
+        fprintf(stderr, "rtl_wmbus_b200: WMBUS_B200_BURST_LEVEL=%s: expected <t1c1>[,<s1>], 0 (off) .. 255\n", e);
+        return EXIT_FAILURE;
+    }
+    if ((e = getenv("WMBUS_B200_BURSTS")) != NULL && (g_burst_file = fopen(e, "w")) == NULL) {
+        fprintf(stderr, "rtl_wmbus_b200: WMBUS_B200_BURSTS=%s: %s\n", e, strerror(errno));
+        return EXIT_FAILURE;
+    }
+
     if ((e = getenv("WMBUS_B200_LINE_INFO")) != NULL && (g_info_file = fopen(e, "w")) == NULL) {
         fprintf(stderr, "rtl_wmbus_b200: WMBUS_B200_LINE_INFO=%s: %s\n", e, strerror(errno));
         return EXIT_FAILURE;
@@ -239,6 +283,12 @@ int main(int argc, char *argv[])
             fprintf(stderr, "rtl_wmbus_b200: %s\n", wmb_last_error());
             return EXIT_FAILURE;
         }
+    if (g_burst_file)
+        for (int ch = 0; ch < 2; ch++)
+            if (wmb_set_bursts(ctx, ch, (uint32_t)burst_level[ch]) != WMB_OK) {
+                fprintf(stderr, "rtl_wmbus_b200: %s\n", wmb_last_error());
+                return EXIT_FAILURE;
+            }
     uint8_t *buf = wmb_host_alloc(batch);
     const size_t outcap = 1u << 20;
     char *out = malloc(outcap);
@@ -308,6 +358,10 @@ int main(int argc, char *argv[])
     free(out);
     wmb_host_free(buf);
     wmb_destroy(ctx);
+    if (g_burst_file && fclose(g_burst_file) != 0 && rc == WMB_OK) {
+        fprintf(stderr, "rtl_wmbus_b200: WMBUS_B200_BURSTS: %s\n", strerror(errno));
+        return EXIT_FAILURE;
+    }
     if (g_info_file && fclose(g_info_file) != 0 && rc == WMB_OK) {
         fprintf(stderr, "rtl_wmbus_b200: WMBUS_B200_LINE_INFO: %s\n", strerror(errno));
         return EXIT_FAILURE;

@@ -39,6 +39,7 @@
 #include "wmbus_b200.h"
 #include "wmb_framer.h"
 #include "wmb_kernels.cuh"
+#include "wmb_bursts.cuh"
 
 #ifndef WMB_VERSION
 #define WMB_VERSION "wmbus-b200 0.1 (sm_90a)"
@@ -190,7 +191,7 @@ struct wmb_ctx {
     uint32_t *d_cut_n = nullptr;
     uint64_t *d_k3_agg = nullptr;
     uint32_t spec_n = 0, spec_pool = 0;              /* entries / bytes copied before their counts are known */
-    struct InFlight { int slot; bool final; bool has_timers; uint64_t m_end; };
+    struct InFlight { int slot; bool final; bool has_timers; uint64_t m_end; bool bursts; uint32_t burst_spec; };
     std::vector<InFlight> inflight;                  /* gathered batches whose results the host has not read yet */
     uint64_t stat_rerun_seen = 0, stat_fallback_seen = 0;
     double acc_demod_ms = 0, acc_bitsync_ms = 0, acc_pass_ms = 0;    /* timers of the current push */
@@ -212,6 +213,18 @@ struct wmb_ctx {
     /* receiver settings per chain (wmb_set_receiver; they survive wmb_reset) */
     uint32_t lock[WMB_N_CHAINS] = {2, 2};            /* clock-lock threshold, rtl_wmbus.c:865-866 */
     uint32_t ac_err[WMB_N_CHAINS] = {0, 0};          /* access-code bit errors, :99, :103         */
+
+    /* burst report (wmb_set_bursts; the levels survive wmb_reset).  Level 0: off, nothing is allocated or launched */
+    uint32_t burst_level[WMB_N_CHAINS] = {0, 0};
+    struct BurstBuf { uint32_t *mask = nullptr, *cnt = nullptr; uint64_t *base = nullptr, *agg = nullptr; int64_t *ev = nullptr;
+                      BurstDev *bd = nullptr; BurstItem *items = nullptr; } bb[WMB_N_CHAINS];
+    bool burst_allocated = false;
+    uint32_t burst_cap = 0;                          /* records per slot and chain: pieces >= 256 samples of one batch */
+    uint32_t burst_spec = 64;                        /* records copied per slot and chain before their count is known */
+    BurstRec *d_brec = nullptr, *h_brec = nullptr;   /* [WMB_NSLOT][chain][burst_cap] */
+    BurstSlot *d_bslot = nullptr, *h_bslot = nullptr;
+    std::vector<wmb_burst> bursts;                   /* closed pieces not taken yet */
+    uint64_t burst_frontier = 0;                     /* no piece still to come starts before this sample */
 
     /* results */
     uint64_t win_lo = 0, win_hi = ~0ull;             /* line window (access-code match sample) */
@@ -449,6 +462,56 @@ static int launch_k4(wmb_ctx *c, const K4Params &p)
     return WMB_OK;
 }
 #endif
+
+/* the burst pass of one chain (wmb_bursts.cuh), on cs; p.M == 0: the end-of-input gather (only kb_runs + kb_reduce) */
+static int launch_bursts(wmb_ctx *c, const BurstParams &p, uint64_t *agg)
+{
+#ifdef WMB_HOSTSIM
+    if (p.M > 0) {
+        hs_for(WMB_BURST_LOOK + p.nw, [&](uint32_t wi) { kb_mask(p, wi); });
+        hs_for(p.units, [&](uint32_t u) { p.cnt[u] = kb_events(p, u, false); });
+        launch_cscan(c, p.cnt, p.base, p.units, agg, &p.bd->n_ev, nullptr, nullptr, 1);
+        hs_for(p.units, [&](uint32_t u) { kb_events(p, u, true); });
+        c->st.kernel_launches += 3;
+    }
+    {
+        BurstRunCtx r;
+        kb_run_ctx(p, r);
+        static uint32_t cnt[WMB_BURST_BLOCK];
+        uint32_t total = 0;
+        const uint32_t chunks = (r.n_runs + WMB_BURST_BLOCK - 1) / WMB_BURST_BLOCK;
+        for (uint32_t ch = 0; ch < chunks; ch++) {
+            hs_for(WMB_BURST_BLOCK, [&](uint32_t t) { kb_runs_count(p, r, ch, t, cnt); });
+            kb_runs_scan(cnt, &total);
+            hs_for(WMB_BURST_BLOCK, [&](uint32_t t) { kb_runs_write(p, r, ch, t, cnt); });
+        }
+        kb_runs_finish(p, r, total);
+    }
+    {
+        static BurstPart part[WMB_BURST_BLOCK];
+        hs_for(p.bd->n_items, [&](uint32_t it) {
+            hs_for(WMB_BURST_BLOCK, [&](uint32_t t) { kb_reduce_part(p, it, t, WMB_BURST_BLOCK, part); });
+            kb_reduce_finish(p, it, part, WMB_BURST_BLOCK);
+        });
+    }
+    c->st.kernel_launches += 2;
+#else
+    static int sms = 0;
+    if (!sms) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c->device);
+    if (p.M > 0) {
+        kb_mask_kernel<<<(WMB_BURST_LOOK + p.nw + 255) / 256, 256, 0, c->cs>>>(p);
+        kb_count_kernel<<<(p.units + 255) / 256, 256, 0, c->cs>>>(p);
+        launch_cscan(c, p.cnt, p.base, p.units, agg, &p.bd->n_ev, nullptr, nullptr, 1);
+        kb_write_kernel<<<(p.units + 255) / 256, 256, 0, c->cs>>>(p);
+        c->st.kernel_launches += 3;
+    }
+    kb_runs_kernel<<<1, WMB_BURST_BLOCK, 0, c->cs>>>(p);
+    kb_reduce_kernel<<<sms * 4, WMB_BURST_BLOCK, 0, c->cs>>>(p);
+    CUDA_TRY(cudaGetLastError());
+    c->st.kernel_launches += 2;
+#endif
+    return WMB_OK;
+}
 
 /* --------------------------------------------------------------------------- */
 /* set-up                                                                      */
@@ -700,6 +763,43 @@ static int ctx_alloc(wmb_ctx *c)
      * kernel on the context's non-blocking streams can read them */
     CUDA_TRY(cudaDeviceSynchronize());
     c->allocated = true;
+    return WMB_OK;
+}
+
+static bool bursts_on(const wmb_ctx *c)
+{
+    for (int ch = 0; ch < WMB_N_CHAINS; ch++) if (c->burst_level[ch] && (c->chains & (1u << ch))) return true;
+    return false;
+}
+
+/* the burst pass's buffers, at the first batch that needs them.  The record table of a slot holds every piece one
+ * batch can close: pieces are disjoint and >= 256 samples long, and all but the first lie in [-G, M) */
+static int burst_alloc(wmb_ctx *c)
+{
+    if (c->burst_allocated) return WMB_OK;
+    const size_t M = (size_t)c->M_max;
+    const size_t nw = M / 32 + 2, units = M / WMB_BURST_UNIT + 2;
+    c->burst_cap = (uint32_t)(M / 256 + 4);
+    for (int ch = 0; ch < WMB_N_CHAINS; ch++) {
+        if (!(c->chains & (1u << ch))) continue;
+        wmb_ctx::BurstBuf &b = c->bb[ch];
+        /* events: a start needs G below samples before it, an end G after it */
+        const size_t ev_cap = 2 * (M / (size_t)(burst_G((uint32_t)ch) + 1) + 2) + 64;
+        TRY(dev_alloc(c, &b.mask, WMB_BURST_LOOK + nw));
+        TRY(dev_alloc(c, &b.cnt, units));
+        TRY(dev_alloc(c, &b.base, units));
+        TRY(dev_alloc(c, &b.agg, scan_tiles((uint32_t)units) + 1));
+        TRY(dev_alloc(c, &b.ev, ev_cap));
+        TRY(dev_alloc(c, &b.bd, 1, true));
+        TRY(dev_alloc(c, &b.items, (size_t)c->burst_cap + 1));
+    }
+    TRY(dev_alloc(c, &c->d_brec, (size_t)WMB_NSLOT * WMB_N_CHAINS * c->burst_cap));
+    TRY(host_alloc(c, &c->h_brec, (size_t)WMB_NSLOT * WMB_N_CHAINS * c->burst_cap));
+    TRY(dev_alloc(c, &c->d_bslot, WMB_NSLOT, true));
+    TRY(host_alloc(c, &c->h_bslot, WMB_NSLOT));
+    c->burst_spec = std::min<uint32_t>(64, c->burst_cap);
+    CUDA_TRY(cudaDeviceSynchronize());
+    c->burst_allocated = true;
     return WMB_OK;
 }
 
@@ -1187,6 +1287,52 @@ static int run_batch(wmb_ctx *c, const uint8_t *src, size_t nbytes, cudaEvent_t 
 
 static int consume_oldest(wmb_ctx *c);
 
+/* the carrier a chain listens to, relative to the capture's centre frequency (the mixer of run_batch) */
+static double chain_carrier_hz(const wmb_ctx *c, int chain)
+{
+    if (c->o.simultaneous == 2) return 25e3 * (double)c->o.carrier_25khz[chain];
+    if (c->o.simultaneous) return chain == 0 ? 325e3 : -325e3;
+    return 0.0;
+}
+
+/* one slot's burst records -> the queue; the frontier: where the next piece of any chain may start */
+static int book_bursts(wmb_ctx *c, int slot, uint64_t m_end, uint32_t spec)
+{
+    const BurstSlot bs = c->h_bslot[slot];
+    uint64_t frontier = m_end;
+    uint32_t most = 0;
+    for (int ch = 0; ch < WMB_N_CHAINS; ch++) {
+        if (!c->burst_level[ch] || !(c->chains & (1u << ch))) continue;
+        const uint32_t n = bs.n[ch];
+        if (n > c->burst_cap) return set_err(WMB_E_STATE, "internal: burst records beyond their table");
+        const size_t at = ((size_t)slot * WMB_N_CHAINS + ch) * c->burst_cap;
+        if (n > spec) {
+            CUDA_TRY(cudaMemcpyAsync(c->h_brec + at + spec, c->d_brec + at + spec, (size_t)(n - spec) * sizeof(BurstRec),
+                                     cudaMemcpyDeviceToHost, c->xs));
+            CUDA_TRY(cudaStreamSynchronize(c->xs));
+        }
+        c->st.d2h_bytes += (uint64_t)std::max(n, spec) * sizeof(BurstRec);
+        most = std::max(most, n);
+        for (uint32_t i = 0; i < n; i++) {
+            const BurstRec &r = c->h_brec[at + i];
+            wmb_burst b;
+            memset(&b, 0, sizeof(b));
+            b.start_sample = r.start; b.end_sample = r.end; b.rssi_sum = r.rssi_sum; b.sum = r.sum; b.n = r.n;
+            b.chain = r.chain; b.peak = r.peak; b.flags = r.flags;
+            /* -a: the cross-product discriminator is not a frequency */
+            b.valid = (uint8_t)(r.n > 0 && c->o.accurate_atan ? 1 : 0);
+            b.carrier_hz = chain_carrier_hz(c, ch);
+            b.offset_hz = b.valid ? (double)r.sum / (double)r.n / (double)WMB_OFS_SCALE * 400e3 / c->fir_gain[ch] : NAN;
+            c->bursts.push_back(b);
+        }
+        if (bs.open[ch] && (uint64_t)bs.ps[ch] < frontier) frontier = (uint64_t)bs.ps[ch];
+    }
+    c->st.d2h_bytes += sizeof(BurstSlot);
+    if (most > c->burst_spec) c->burst_spec = std::min<uint32_t>(c->burst_cap, most + most / 4 + 64);
+    c->burst_frontier = frontier;
+    return WMB_OK;
+}
+
 /* Enqueue the frame gather (K3), the device framer (K4) and the copies of their results into the host mirror of the
  * next result slot, for everything the streams hold: the candidates carried over plus the new access-code matches.
  * after_batch: this gather closes the batch just enqueued (its set may be reused once it is done).  final: end of
@@ -1236,6 +1382,34 @@ static int enqueue_gather(wmb_ctx *c, bool final, bool after_batch)
             CUDA_TRY(cudaMemcpyAsync(c->h_pool + pb, c->d_pool + pb, c->spec_pool, cudaMemcpyDeviceToHost, c->cs));
         }
     }
+    /* the burst report: behind the demod kernel of the batch (cs waited for it), before ev_chain[set] releases the set */
+    const bool bursts = bursts_on(c) && (after_batch || final);
+    if (bursts) {
+        TRY(burst_alloc(c));
+        for (int ch = 0; ch < WMB_N_CHAINS; ch++) {
+            if (!c->burst_level[ch] || !(c->chains & (1u << ch))) continue;
+            const wmb_ctx::BurstBuf &b = c->bb[ch];
+            BurstParams p;
+            memset(&p, 0, sizeof(p));
+            const SetBuf &sb = c->cb[ch].set[c->last_set];
+            p.rssi = sb.rssi + c->W; p.dphi = sb.dphi + c->W;
+            p.M = after_batch ? c->last_M : 0;
+            p.clip = c->last_hist;
+            p.m_first = (int64_t)(c->m_consumed - (uint64_t)p.M);
+            p.level = c->burst_level[ch]; p.chain = (uint32_t)ch; p.final_ = final ? 1u : 0u;
+            p.nw = (uint32_t)((p.M + 31) / 32); p.units = (uint32_t)((p.M + WMB_BURST_UNIT - 1) / WMB_BURST_UNIT);
+            p.mask = b.mask; p.cnt = b.cnt; p.base = b.base; p.ev = b.ev; p.bd = b.bd; p.items = b.items;
+            p.out = c->d_brec + ((size_t)slot * WMB_N_CHAINS + ch) * c->burst_cap;
+            p.slot = c->d_bslot + slot;
+            TRY(launch_bursts(c, p, b.agg));
+        }
+        CUDA_TRY(cudaMemcpyAsync(c->h_bslot + slot, c->d_bslot + slot, sizeof(BurstSlot), cudaMemcpyDeviceToHost, c->cs));
+        for (int ch = 0; ch < WMB_N_CHAINS; ch++) {
+            if (!c->burst_level[ch] || !(c->chains & (1u << ch))) continue;
+            const size_t at = ((size_t)slot * WMB_N_CHAINS + ch) * c->burst_cap;
+            CUDA_TRY(cudaMemcpyAsync(c->h_brec + at, c->d_brec + at, (size_t)c->burst_spec * sizeof(BurstRec), cudaMemcpyDeviceToHost, c->cs));
+        }
+    }
     CUDA_TRY(cudaEventRecord(c->ev_res[slot], c->cs));
     /* ev_chain[set] releases the batch's set to the demod kernel of batch i+2 (run_batch waits for it on k1s): it is
      * recorded here, behind the gather on cs, so k3_fill's reads of the set's dphi come before that kernel's writes */
@@ -1244,7 +1418,8 @@ static int enqueue_gather(wmb_ctx *c, bool final, bool after_batch)
         c->chain_recorded[c->last_set] = true;
     }
     wmb_ctx::InFlight f;
-    f.slot = slot; f.final = final; f.has_timers = after_batch; f.m_end = c->m_consumed;
+    f.slot = slot; f.final = final; f.has_timers = after_batch; f.m_end = c->m_consumed; f.bursts = bursts;
+    f.burst_spec = c->burst_spec;                    /* records the copies above fetched (burst_spec may grow before they are read) */
     c->inflight.push_back(f);
     c->gather_no++;
     return WMB_OK;
@@ -1274,6 +1449,7 @@ static int consume_oldest(wmb_ctx *c)
         /* the whole per-sample pass of the push so far: first demod kernel -> this batch's last bit-sync kernel */
         if (cudaEventElapsedTime(&ms, c->ev_push_start, evt[3]) == cudaSuccess) c->acc_pass_ms = ms;
     }
+    if (f.bursts) TRY(book_bursts(c, f.slot, f.m_end, f.burst_spec));
     if (!any_sync) return WMB_OK;
     const bool dev_decode = !c->manual;
     const size_t lb = (size_t)f.slot * c->slot_cap, pb = (size_t)f.slot * c->slot_pool;
@@ -1761,14 +1937,6 @@ extern "C" int wmb_decode_frames(wmb_ctx *c, const wmb_frame *frames, size_t n)
         [&](size_t i, wmb_decoded &o) { o = dec[i]; });
 }
 
-/* the carrier a chain listens to, relative to the capture's centre frequency (the mixer of run_batch) */
-static double chain_carrier_hz(const wmb_ctx *c, int chain)
-{
-    if (c->o.simultaneous == 2) return 25e3 * (double)c->o.carrier_25khz[chain];
-    if (c->o.simultaneous) return chain == 0 ? 325e3 : -325e3;
-    return 0.0;
-}
-
 extern "C" size_t wmb_take_lines_info(wmb_ctx *c, char *buf, size_t cap, size_t *n_lines, int timestamp_mode,
                                       wmb_line_info *info, size_t info_cap)
 {
@@ -1861,6 +2029,7 @@ extern "C" int wmb_reset(wmb_ctx *c)
     c->batch_no = 0; c->last_M = 0; c->prev_M = 0; c->last_hist = 0; c->last_set = 0; c->inflight.clear();
     c->chain_recorded[0] = c->chain_recorded[1] = false;
     c->stat_rerun_seen = 0; c->stat_fallback_seen = 0;
+    c->bursts.clear(); c->burst_frontier = 0;
     for (int ch = 0; ch < WMB_N_CHAINS; ch++)
         for (int a = 0; a < WMB_N_ALGOS; a++) { Stream &s = c->cb[ch].s[a]; s.total = 0; s.total_prev = 0; s.busy_until = -1; }
     if (c->allocated) {
@@ -1880,6 +2049,9 @@ extern "C" int wmb_reset(wmb_ctx *c)
         wmb_reset_kernel<<<1, 32, 0, c->cs>>>(r);
         CUDA_TRY(cudaGetLastError());
 #endif
+        if (c->burst_allocated)                  /* no run open */
+            for (int ch = 0; ch < WMB_N_CHAINS; ch++)
+                if (c->bb[ch].bd) CUDA_TRY(cudaMemsetAsync(c->bb[ch].bd, 0, sizeof(BurstDev), c->cs));
         CUDA_TRY(cudaEventRecord(c->ev_reset, c->cs));
         c->reset_pending = true;
     }
@@ -1911,6 +2083,33 @@ extern "C" int wmb_set_receiver(wmb_ctx *c, int chain, uint32_t clock_lock, uint
         return set_err(WMB_E_STATE, "wmb_set_receiver after samples were pushed (call it before the first push or after wmb_reset / wmb_seek)");
     c->lock[chain] = clock_lock;
     c->ac_err[chain] = access_code_errors;
+    return WMB_OK;
+}
+
+extern "C" int wmb_set_bursts(wmb_ctx *c, int chain, uint32_t level)
+{
+    if (!c) return set_err(WMB_E_INVAL, "null argument");
+    if (chain != WMB_CHAIN_T1C1 && chain != WMB_CHAIN_S1) return set_err(WMB_E_INVAL, "chain %d: 0 (T1/C1) or 1 (S1)", chain);
+    if (level > 255) return set_err(WMB_E_INVAL, "burst level %u out of range 0 (off) .. 255", level);
+    if (c->batch_no != 0 || !c->remainder.empty())
+        return set_err(WMB_E_STATE, "wmb_set_bursts after samples were pushed (call it before the first push or after wmb_reset / wmb_seek)");
+    c->burst_level[chain] = level;
+    return WMB_OK;
+}
+
+extern "C" int wmb_take_bursts(wmb_ctx *c, wmb_burst *out, size_t cap, size_t *n)
+{
+    if (!c || !n || (!out && cap)) return set_err(WMB_E_INVAL, "null argument");
+    /* per chain the queue is in start order (pieces of a chain are disjoint and close in order); across chains a
+     * piece closed later may start earlier */
+    std::stable_sort(c->bursts.begin(), c->bursts.end(), [](const wmb_burst &a, const wmb_burst &b) {
+        return a.start_sample != b.start_sample ? a.start_sample < b.start_sample : a.chain < b.chain;
+    });
+    size_t k = 0;
+    while (k < cap && k < c->bursts.size() && c->bursts[k].start_sample < c->burst_frontier) k++;
+    if (k) memcpy(out, c->bursts.data(), k * sizeof(wmb_burst));
+    c->bursts.erase(c->bursts.begin(), c->bursts.begin() + (long)k);
+    *n = k;
     return WMB_OK;
 }
 

@@ -86,15 +86,33 @@ def chunk_bounds(n_bytes: int, d: int, world: int):
     return [min(n_iq, (n_iq * g // world) // gran * gran) for g in range(world)] + [n_iq]
 
 
-def decode_time_chunk(ctx, push, n_bytes: int, d: int, rank: int, world: int, halo_m: int = 1 << 18, info=False):
+def merge_bursts(parts):
+    """Burst records (wmb_burst arrays) of several time chunks, each holding the pieces that start in its chunk ->
+    the sequential run's records, ordered by (start_sample, chain)."""
+    import numpy as np
+    recs = np.concatenate(parts)
+    return recs[np.lexsort((recs["chain"], recs["start_sample"]))]
+
+
+def decode_time_chunk(ctx, push, n_bytes: int, d: int, rank: int, world: int, halo_m: int = 1 << 18, info=False,
+                      bursts=False):
     """Decode rank `rank`'s chunk of a capture of n_bytes cu8 bytes.  `push(byte_lo, byte_hi)` feeds that byte
     range of the capture to ctx (host or device memory: the caller's business).
     Returns (lines, digest_start, digest_end, halo_start_iq): digest_start is None for a chunk that starts at 0.
     The lines carry their print position in the TIMESTAMP column (timestamp_mode 2) for merge_lines().
     info=True: lines is (lines, records), the records (wmb_line_info) of the lines.  A line's carrier-offset window lies
-    in the chunk that holds its match, far behind the halo's start, so the records are the sequential run's."""
+    in the chunk that holds its match, far behind the halo's start, so the records are the sequential run's.
+    bursts=True (ctx made with a burst level): lines is (lines[, records], bursts), bursts the chunk's burst pieces -- those
+    that start in [lo, hi) of decimated samples.  A piece depends on its samples and at most 2^17 + 2^16 + 196 before it
+    (DESIGN.md §8), inside the left halo, and one that starts before hi is closed within as many samples after hi, inside
+    the right halo, so they are the sequential run's pieces."""
     import hashlib
     recs = []
+    brecs = []
+
+    def take_b():
+        if bursts:
+            brecs.append(ctx.take_bursts())
 
     def take():
         if not info:
@@ -113,10 +131,12 @@ def decode_time_chunk(ctx, push, n_bytes: int, d: int, rank: int, world: int, ha
     if start < lo:
         push(2 * start, 2 * lo)
         lines += take()
+        take_b()
     if lo > 0:
         dig_start = hashlib.sha256(ctx.boundary_state()).digest()
     push(2 * lo, 2 * hi)
     lines += take()
+    take_b()
     dig_end = hashlib.sha256(ctx.boundary_state()).digest()
     if rank + 1 < world:                              # finish the telegrams that started in the chunk
         step = (MAX_TELEGRAM_M * d + gran - 1) // gran * gran
@@ -135,15 +155,23 @@ def decode_time_chunk(ctx, push, n_bytes: int, d: int, rank: int, world: int, ha
             push(2 * hi, n_bytes)                     # the ragged end of the capture (the reference drops a short item)
         ctx.poll_flush()
     lines += take()
+    take_b()
     if info:
         import numpy as np
         lines = (lines, np.concatenate(recs))
+    if bursts:
+        import numpy as np
+        b = np.concatenate(brecs)
+        m_lo, m_hi = lo // d, (hi // d if rank + 1 < world else 1 << 63)
+        b = b[(b["start_sample"] >= m_lo) & (b["start_sample"] < m_hi)]
+        lines = (lines + (b,)) if info else (lines, b)
     return lines, dig_start, dig_end, start
 
 
-def decode_time_sharded(ctx, push, n_bytes: int, d: int, halo_m: int = 1 << 18, info=False):
+def decode_time_sharded(ctx, push, n_bytes: int, d: int, halo_m: int = 1 << 18, info=False, bursts=False):
     """All ranks: decode one capture in time chunks, exact by construction (see module docstring).
-    Returns (my_lines, rounds); info=True: my_lines is (lines, records) as in decode_time_chunk."""
+    Returns (my_lines, rounds); info=True / bursts=True: my_lines carries the records / burst pieces as in
+    decode_time_chunk."""
     rank = dist.get_rank() if dist.is_initialized() else 0
     world = dist.get_world_size() if dist.is_initialized() else 1
     rounds = 0
@@ -152,7 +180,7 @@ def decode_time_sharded(ctx, push, n_bytes: int, d: int, halo_m: int = 1 << 18, 
     while True:
         rounds += 1
         if redo:
-            lines, ds, de, start = decode_time_chunk(ctx, push, n_bytes, d, rank, world, halo_m, info=info)
+            lines, ds, de, start = decode_time_chunk(ctx, push, n_bytes, d, rank, world, halo_m, info=info, bursts=bursts)
         mine = torch.zeros(65, dtype=torch.uint8)
         mine[:32] = torch.frombuffer(bytearray(ds or bytes(32)), dtype=torch.uint8)
         mine[32:64] = torch.frombuffer(bytearray(de), dtype=torch.uint8)
