@@ -262,6 +262,52 @@ int wmb_set_bursts(wmb_ctx *c, int chain, uint32_t level);
  * taken stay queued. */
 int wmb_take_bursts(wmb_ctx *c, wmb_burst *out, size_t cap, size_t *n);
 
+/* ---- band survey: a power spectrum of the whole captured band, to find the carriers to decode --------------------
+ * Off by default.  wmb_set_spectrum(ctx, N, B) with N bins (256, 512, 1024 or 2048) and B blocks per record (1 .. 2^20)
+ * turns it on.  It works on the raw cu8 input, before any mixer, prefilter or decimation, so it does not depend on -s,
+ * the prefilter or the chain options, and it runs with no chain enabled.
+ *   1. Block b covers global IQ samples [b N, (b + 1) N) (the index wmb_seek sets; pushes, batches and seek positions
+ *      are multiples of 2048 IQ samples, so no block straddles them).  A block is counted when it was pushed since the
+ *      last wmb_reset / wmb_seek and its first decimated sample floor(b N / d) lies in the line window
+ *      (wmb_set_line_window), which lets time chunks split the blocks between them.
+ *   2. Per block, every operation a separately rounded fp32 operation:
+ *        i = (int)(u - 127.5f) for I (even byte) and Q (odd byte) -- the front end's u - 127 - (u >= 128);
+ *        x_re = (float)i_I * hann[n], x_im = (float)i_Q * hann[n], hann[n] = (float)(0.5 - 0.5 cos(2 pi n / N)) (double);
+ *        X[k] = sum x[n] e^(-2 pi i k n / N): radix-2 decimation in time on bit-reversed input; at stage s (half
+ *          2^(s-1)) butterfly j uses tw[j N / 2^s] = ((float)cos(2 pi k / N), (float)-sin(2 pi k / N)) (double),
+ *          t_re = w_re b_re - w_im b_im, t_im = w_re b_im + w_im b_re (each product rounded, then the sum),
+ *          a' = a + t, b' = a - t componentwise;
+ *        p = re re + im im.
+ *   3. Record r covers blocks [r B, (r + 1) B).  Per bin k in frequency order (fftshifted: bin k lies (k - N/2) fs / N
+ *      from the capture's centre, fs = 0.8 d MHz) it holds sum[k] = sum of rint(p) (uint64: integer terms, exact in any
+ *      order; below 2^55 at N = 2048, B = 2^20) and peak[k] = max p, and blocks = the blocks counted.
+ *   4. A record is handed out once a block of a later record has been pushed, or at flush (partial).  Records with no
+ *      block counted are not handed out; records come out in record order.
+ *   5. Time chunks: a chunk's rows are the sequential run's rows restricted to its blocks.  Adding sum and blocks and
+ *      taking the max of peak over rows of the same record gives the sequential rows.
+ * Device memory: (batch blocks / B + 2) rows of N bins (12 bytes each) in a ring and in each of 4 result slots (and
+ * pinned host memory for the slots). */
+typedef struct wmb_spectrum_row {
+    uint64_t record;          /* r                                                                             */
+    uint64_t start_iq;        /* r B N: the record's first IQ sample (its first counted block may lie later)  */
+    uint32_t blocks;          /* blocks counted                                                                */
+    uint32_t bins;            /* N                                                                             */
+    double   hz_low;          /* frequency of bin 0 relative to the capture's centre: -fs / 2                  */
+    double   hz_step;         /* fs / N                                                                        */
+} wmb_spectrum_row;
+
+/* bins 0: off (the default); else bins 256, 512, 1024 or 2048 and blocks_per_record 1 .. 2^20, and at most 2^23 bins in
+ * a table ((batch blocks / B + 2) N, batch blocks = max_batch_mib MiB / 2N), else WMB_E_INVAL.  Valid before the first
+ * push or right after wmb_reset / wmb_seek (else WMB_E_STATE).  The setting survives wmb_reset and wmb_seek. */
+int wmb_set_spectrum(wmb_ctx *c, uint32_t bins, uint32_t blocks_per_record);
+
+/* Copy up to cap closed records: rows[i], sum[i * bins ...], peak[i * bins ...] (sum and peak hold cap x bins);
+ * *n receives their number.  Records not taken stay queued. */
+int wmb_take_spectrum(wmb_ctx *c, wmb_spectrum_row *rows, uint64_t *sum, float *peak, size_t cap, size_t *n);
+
+/* Test hook: the survey's window and twiddle tables for N bins: hann[N], tw[N / 2][2] = (cos, -sin). */
+int wmb_debug_spectrum_tables(uint32_t bins, float *hann, float *tw);
+
 /* Convenience for offline captures: push + flush + decode + take_lines in one call.
  * `flush` as in wmb_poll.  Returns bytes written to out or a negative error. */
 long wmb_process(wmb_ctx *c, const uint8_t *cu8, size_t nbytes, int flush,

@@ -11,7 +11,9 @@ Import with ``importlib.import_module("rtl-wmbus_b200")`` (the directory name ca
 reference's hyphen).
 """
 from .capi import (WmbOpts, WmbStats, WmbFrame, WmbLineInfo, WmbusB200, load_library, library_path, build,
-                   opts_from_flags, line_info_dtype, burst_dtype, BURST_CONTINUED, BURST_CUT, BURST_AT_END, LIB_NAME)
+                   opts_from_flags, line_info_dtype, burst_dtype, BURST_CONTINUED, BURST_CUT, BURST_AT_END, spectrum_dtype,
+                   LIB_NAME)
 
 __all__ = ["WmbOpts", "WmbStats", "WmbFrame", "WmbLineInfo", "WmbusB200", "load_library", "library_path", "build",
-           "opts_from_flags", "line_info_dtype", "burst_dtype", "BURST_CONTINUED", "BURST_CUT", "BURST_AT_END", "LIB_NAME"]
+           "opts_from_flags", "line_info_dtype", "burst_dtype", "BURST_CONTINUED", "BURST_CUT", "BURST_AT_END", "spectrum_dtype",
+           "LIB_NAME"]

@@ -52,6 +52,16 @@ def burst_dtype():
     return np.dtype(BURST_FIELDS)
 
 
+# numpy mirror of wmb_spectrum_row (one record of the band survey; see include/wmbus_b200.h)
+SPECTRUM_FIELDS = [("record", "<u8"), ("start_iq", "<u8"), ("blocks", "<u4"), ("bins", "<u4"), ("hz_low", "<f8"),
+                   ("hz_step", "<f8")]
+
+
+def spectrum_dtype():
+    import numpy as np
+    return np.dtype(SPECTRUM_FIELDS)
+
+
 class WmbStats(C.Structure):
     _fields_ = [("input_samples", C.c_uint64), ("decimated_samples", C.c_uint64), ("batches", C.c_uint64),
                 ("kernel_launches", C.c_uint64), ("lanes_run", C.c_uint64), ("lanes_rerun", C.c_uint64),
@@ -110,6 +120,9 @@ def _bind(lib):
     lib.wmb_set_receiver.argtypes = [C.c_void_p, C.c_int, C.c_uint32, C.c_uint32]
     lib.wmb_set_bursts.argtypes = [C.c_void_p, C.c_int, C.c_uint32]
     lib.wmb_take_bursts.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
+    lib.wmb_set_spectrum.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32]
+    lib.wmb_take_spectrum.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
+    lib.wmb_debug_spectrum_tables.argtypes = [C.c_uint32, C.c_void_p, C.c_void_p]
     lib.wmb_boundary_state.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
     lib.wmb_boundary_state.restype = C.c_long
     lib.wmb_pending_before.argtypes = [C.c_void_p, C.c_uint64]
@@ -121,7 +134,8 @@ EXPORTS = ["wmb_reset", "wmb_host_alloc", "wmb_host_free", "wmb_default_opts", "
            "wmb_destroy", "wmb_push", "wmb_push_device", "wmb_poll", "wmb_decode_frames", "wmb_take_lines",
            "wmb_process", "wmb_process_device", "wmb_get_stats", "wmb_debug_copy_stage", "wmb_debug_copy_bits", "wmb_debug_copy_events", "wmb_debug_arith",
            "wmb_seek", "wmb_set_line_window", "wmb_boundary_state", "wmb_pending_before", "wmb_set_receiver",
-           "wmb_take_lines_info", "wmb_set_bursts", "wmb_take_bursts"]
+           "wmb_take_lines_info", "wmb_set_bursts", "wmb_take_bursts", "wmb_set_spectrum", "wmb_take_spectrum",
+           "wmb_debug_spectrum_tables"]
 
 
 def load_library(path: str | None = None):
@@ -167,10 +181,12 @@ class WmbusB200:
     clock_lock=(t1c1, s1), access_code_errors=(t1c1, s1): receiver settings, see wmb_set_receiver() (default (2, 2) and
     (0, 0), the reference's).  They survive reset() and seek().
     burst_level=(t1c1, s1): the burst report's level per chain, see wmb_set_bursts() (0: off, the default); it survives
-    reset() and seek() too.  take_bursts() hands out the closed pieces."""
+    reset() and seek() too.  take_bursts() hands out the closed pieces.
+    spectrum=(bins, blocks_per_record): the band survey, see wmb_set_spectrum() (None: off, the default); it survives
+    reset() and seek().  take_spectrum() hands out the closed records."""
 
     def __init__(self, flags: str = "", device: int = 0, lib=None, clock_lock=None, access_code_errors=None,
-                 burst_level=None, **tuning):
+                 burst_level=None, spectrum=None, **tuning):
         self.lib = lib or load_library()
         self.opts = opts_from_flags(self.lib, flags, **tuning)
         self._ctx = C.c_void_p()
@@ -191,6 +207,12 @@ class WmbusB200:
             try:
                 for chain in (0, 1):
                     self.set_bursts(chain, burst_level[chain])
+            except Exception:
+                self.close()
+                raise
+        if spectrum is not None:
+            try:
+                self.set_spectrum(*spectrum)
             except Exception:
                 self.close()
                 raise
@@ -345,6 +367,37 @@ class WmbusB200:
             if n.value < cap:
                 break
         return np.concatenate(parts) if parts else np.zeros(0, burst_dtype())
+
+    def set_spectrum(self, bins: int, blocks_per_record: int):
+        """band survey: bins 256 .. 2048 (0 = off), blocks per record (before the first push, or after reset/seek)"""
+        self._check(self.lib.wmb_set_spectrum(self._ctx, bins, blocks_per_record))
+        self._spec_bins = bins
+
+    def take_spectrum(self):
+        """the closed survey records not taken yet, in record order: (rows, sum, peak) -- rows a numpy structured array
+        of wmb_spectrum_row (spectrum_dtype()), sum a [n, bins] uint64 array, peak a [n, bins] float32 array"""
+        import numpy as np
+        cap = 256                                           # rows per call; sum / peak sized for the largest N
+        rows, sums, peaks = [], [], []
+        while True:
+            r = np.zeros(cap, spectrum_dtype())
+            s = np.zeros((cap, 2048), np.uint64)
+            p = np.zeros((cap, 2048), np.float32)
+            n = C.c_size_t(0)
+            self._check(self.lib.wmb_take_spectrum(self._ctx, r.ctypes.data, s.ctypes.data, p.ctypes.data, cap,
+                                                   C.byref(n)))
+            k = n.value
+            if k:
+                nb = int(r["bins"][0])
+                rows.append(r[:k])
+                sums.append(s.reshape(-1)[:k * nb].reshape(k, nb))
+                peaks.append(p.reshape(-1)[:k * nb].reshape(k, nb))
+            if k < cap:
+                break
+        if not rows:
+            nb = getattr(self, "_spec_bins", 0)              # (no record: [0, bins] arrays, so parts concatenate)
+            return np.zeros(0, spectrum_dtype()), np.zeros((0, nb), np.uint64), np.zeros((0, nb), np.float32)
+        return np.concatenate(rows), np.concatenate(sums), np.concatenate(peaks)
 
     def set_line_window(self, sync_lo: int, sync_hi: int):
         self._check(self.lib.wmb_set_line_window(self._ctx, sync_lo, sync_hi))

@@ -26,9 +26,17 @@
  *                              OFFSET_HZ;FLAGS (CHAIN T1C1 / S1, OFFSET_HZ nan when not valid, FLAGS 1 continued, 2 cut,
  *                              4 at end of input).  A path that cannot be opened is an error at start-up.
  *   WMBUS_B200_BURST_LEVEL=<t1c1>[,<s1>]  the bursts' rssi level, 1..255 (0: that chain off; default 14).
+ *   WMBUS_B200_SPECTRUM=<path> survey the whole captured band (wmb_set_spectrum) and write two lines per record, flushed
+ *                              after each hand-over: mean;RECORD;START_IQ_SAMPLE;BLOCKS;HZ_LOW;HZ_STEP;dB_0;...;dB_{N-1}
+ *                              with 10 log10(sum / blocks) per bin, then the same with peak and 10 log10(peak); HZ_LOW is
+ *                              bin 0's frequency relative to the capture's centre.  tools/find_carriers.py reads the file.
+ *   WMBUS_B200_SPECTRUM_BINS=<n>    bins N: 256, 512, 1024 (default) or 2048
+ *   WMBUS_B200_SPECTRUM_BLOCKS=<n>  blocks of N IQ samples per record, 1 .. 2^20 (default 16384: 10.5 s at 1.6 MS/s)
+ *   A path that cannot be opened or a bad value is an error at start-up.  stdout does not change.
  */
 #define _GNU_SOURCE
 #include <errno.h>
+#include <math.h>
 #include <getopt.h>
 #include <poll.h>
 #include <signal.h>
@@ -167,9 +175,41 @@ static void emit_bursts(wmb_ctx *ctx)
     fflush(g_burst_file);
 }
 
+/* WMBUS_B200_SPECTRUM: a mean line and a peak line per closed record of the band survey */
+static FILE *g_spec_file = NULL;
+#define SPEC_CAP 16
+static wmb_spectrum_row g_spec_rows[SPEC_CAP];
+static uint64_t g_spec_sum[SPEC_CAP * 2048];
+static float g_spec_peak[SPEC_CAP * 2048];
+
+static void emit_spectrum(wmb_ctx *ctx)
+{
+    if (!g_spec_file) return;
+    for (;;) {
+        size_t n = 0;
+        if (wmb_take_spectrum(ctx, g_spec_rows, g_spec_sum, g_spec_peak, SPEC_CAP, &n) != WMB_OK || !n) break;
+        for (size_t i = 0; i < n; i++) {
+            const wmb_spectrum_row *r = &g_spec_rows[i];
+            for (int pk = 0; pk < 2; pk++) {
+                fprintf(g_spec_file, "%s;%llu;%llu;%u;%.2f;%.2f", pk ? "peak" : "mean", (unsigned long long)r->record,
+                        (unsigned long long)r->start_iq, (unsigned)r->blocks, r->hz_low, r->hz_step);
+                for (uint32_t k = 0; k < r->bins; k++) {
+                    const double v = pk ? (double)g_spec_peak[i * r->bins + k]
+                                        : (double)g_spec_sum[i * r->bins + k] / (double)r->blocks;
+                    fprintf(g_spec_file, ";%.2f", 10.0 * log10(v));
+                }
+                fputc('\n', g_spec_file);
+            }
+        }
+        if (n < SPEC_CAP) break;
+    }
+    fflush(g_spec_file);
+}
+
 static int emit_lines(wmb_ctx *ctx, char *out, size_t outcap, int show_algorithm)
 {
     emit_bursts(ctx);
+    emit_spectrum(ctx);
     for (;;) {
         size_t nl = 0;
         const size_t n = g_info_file ? wmb_take_lines_info(ctx, out, outcap, &nl, 0, g_info, INFO_CAP)
@@ -268,6 +308,28 @@ int main(int argc, char *argv[])
         return EXIT_FAILURE;
     }
 
+    unsigned long spec_bins = 1024, spec_blocks = 16384;
+    if ((e = getenv("WMBUS_B200_SPECTRUM_BINS")) != NULL) {
+        char *end = NULL;
+        spec_bins = strtoul(e, &end, 10);
+        if (e[0] < '0' || e[0] > '9' || *end || (spec_bins != 256 && spec_bins != 512 && spec_bins != 1024 && spec_bins != 2048)) {
+            fprintf(stderr, "rtl_wmbus_b200: WMBUS_B200_SPECTRUM_BINS=%s: expected 256, 512, 1024 or 2048\n", e);
+            return EXIT_FAILURE;
+        }
+    }
+    if ((e = getenv("WMBUS_B200_SPECTRUM_BLOCKS")) != NULL) {
+        char *end = NULL;
+        spec_blocks = strtoul(e, &end, 10);
+        if (e[0] < '0' || e[0] > '9' || *end || spec_blocks < 1 || spec_blocks > (1ul << 20)) {
+            fprintf(stderr, "rtl_wmbus_b200: WMBUS_B200_SPECTRUM_BLOCKS=%s: expected 1 .. 1048576\n", e);
+            return EXIT_FAILURE;
+        }
+    }
+    if ((e = getenv("WMBUS_B200_SPECTRUM")) != NULL && (g_spec_file = fopen(e, "w")) == NULL) {
+        fprintf(stderr, "rtl_wmbus_b200: WMBUS_B200_SPECTRUM=%s: %s\n", e, strerror(errno));
+        return EXIT_FAILURE;
+    }
+
     if ((e = getenv("WMBUS_B200_LINE_INFO")) != NULL && (g_info_file = fopen(e, "w")) == NULL) {
         fprintf(stderr, "rtl_wmbus_b200: WMBUS_B200_LINE_INFO=%s: %s\n", e, strerror(errno));
         return EXIT_FAILURE;
@@ -289,6 +351,10 @@ int main(int argc, char *argv[])
                 fprintf(stderr, "rtl_wmbus_b200: %s\n", wmb_last_error());
                 return EXIT_FAILURE;
             }
+    if (g_spec_file && wmb_set_spectrum(ctx, (uint32_t)spec_bins, (uint32_t)spec_blocks) != WMB_OK) {
+        fprintf(stderr, "rtl_wmbus_b200: WMBUS_B200_SPECTRUM: %s\n", wmb_last_error());
+        return EXIT_FAILURE;
+    }
     uint8_t *buf = wmb_host_alloc(batch);
     const size_t outcap = 1u << 20;
     char *out = malloc(outcap);
@@ -358,6 +424,10 @@ int main(int argc, char *argv[])
     free(out);
     wmb_host_free(buf);
     wmb_destroy(ctx);
+    if (g_spec_file && fclose(g_spec_file) != 0 && rc == WMB_OK) {
+        fprintf(stderr, "rtl_wmbus_b200: WMBUS_B200_SPECTRUM: %s\n", strerror(errno));
+        return EXIT_FAILURE;
+    }
     if (g_burst_file && fclose(g_burst_file) != 0 && rc == WMB_OK) {
         fprintf(stderr, "rtl_wmbus_b200: WMBUS_B200_BURSTS: %s\n", strerror(errno));
         return EXIT_FAILURE;

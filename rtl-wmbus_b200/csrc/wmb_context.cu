@@ -40,6 +40,7 @@
 #include "wmb_framer.h"
 #include "wmb_kernels.cuh"
 #include "wmb_bursts.cuh"
+#include "wmb_spectrum.cuh"
 
 #ifndef WMB_VERSION
 #define WMB_VERSION "wmbus-b200 0.1 (sm_90a)"
@@ -191,7 +192,7 @@ struct wmb_ctx {
     uint32_t *d_cut_n = nullptr;
     uint64_t *d_k3_agg = nullptr;
     uint32_t spec_n = 0, spec_pool = 0;              /* entries / bytes copied before their counts are known */
-    struct InFlight { int slot; bool final; bool has_timers; uint64_t m_end; bool bursts; uint32_t burst_spec; };
+    struct InFlight { int slot; bool final; bool has_timers; uint64_t m_end; bool bursts; uint32_t burst_spec; bool spec; };
     std::vector<InFlight> inflight;                  /* gathered batches whose results the host has not read yet */
     uint64_t stat_rerun_seen = 0, stat_fallback_seen = 0;
     double acc_demod_ms = 0, acc_bitsync_ms = 0, acc_pass_ms = 0;    /* timers of the current push */
@@ -225,6 +226,26 @@ struct wmb_ctx {
     BurstSlot *d_bslot = nullptr, *h_bslot = nullptr;
     std::vector<wmb_burst> bursts;                   /* closed pieces not taken yet */
     uint64_t burst_frontier = 0;                     /* no piece still to come starts before this sample */
+
+    /* band survey (wmb_set_spectrum; the setting survives wmb_reset).  Bins 0: off, nothing is allocated or launched */
+    uint32_t spec_bins = 0, spec_B = 0;
+    uint32_t spec_R = 0;                             /* ring rows = rows of a result slot: batch blocks / B + 2 */
+    size_t spec_cap = 0;                             /* bins the ring and each slot table hold as allocated */
+    uint32_t spec_tab_n = 0;                         /* N of the tables on the device */
+    float *d_spec_tab = nullptr;                     /* hann[N] | tw[N / 2][2] */
+    uint64_t *d_ssum_ring = nullptr, *d_ssum = nullptr, *h_ssum = nullptr;    /* ring [R][N]; slots [WMB_NSLOT][R][N] */
+    uint32_t *d_speak_ring = nullptr, *d_speak = nullptr, *h_speak = nullptr;
+    cudaEvent_t ev_spec = nullptr;                   /* the batch's survey kernels are done (cs waits before its copies) */
+    cudaEvent_t ev_spec_flush = nullptr;             /* the flush's close is done (the next batch's survey waits) */
+    bool spec_flush_pending = false;
+    bool spec_enqueued = false;                      /* a batch's survey kernels are on the demod stream, cs not yet behind them */
+    int64_t spec_open = -1;                          /* record of the last block pushed, while it has blocks counted */
+    uint32_t spec_open_blocks = 0;
+    std::vector<wmb_spectrum_row> spec_batch_rows;   /* rows the last batch closed, until its gather takes them */
+    std::vector<wmb_spectrum_row> spec_slot_rows[WMB_NSLOT];
+    std::vector<wmb_spectrum_row> spec_rows;         /* closed records not taken yet, with their bins */
+    std::vector<uint64_t> spec_sum;
+    std::vector<uint32_t> spec_peak;
 
     /* results */
     uint64_t win_lo = 0, win_hi = ~0ull;             /* line window (access-code match sample) */
@@ -510,6 +531,60 @@ static int launch_bursts(wmb_ctx *c, const BurstParams &p, uint64_t *agg)
     CUDA_TRY(cudaGetLastError());
     c->st.kernel_launches += 2;
 #endif
+    return WMB_OK;
+}
+
+/* the band survey's FFT pass over one batch (wmb_spectrum.cuh), on the demod stream */
+static int launch_spectrum(wmb_ctx *c, const SpecParams &p, cudaStream_t st)
+{
+#ifdef WMB_HOSTSIM
+    static SpecSmem sm;
+    static SpecAcc acc[WMB_SPEC_THREADS];
+    hs_for(p.n_units, [&](uint32_t gi) {
+        const SpecUnit u = spec_unit(p, p.g_lo + gi);
+        hs_for(WMB_SPEC_THREADS, [&](uint32_t t) { ks_tables(p, sm, t); ks_acc_clear(acc[t]); });
+        const uint32_t L = p.logN;
+        const int64_t per = WMB_SPEC_POINTS / p.N, passes = (u.bb - u.ba + per - 1) / per;
+        for (int64_t pass = 0; pass < passes; pass++) {
+            hs_for(WMB_SPEC_THREADS, [&](uint32_t t) { ks_load(p, sm, u, pass, t, L); });
+            uint32_t lh = 0;
+            for (; lh + 2 <= L; lh += 2) hs_for(WMB_SPEC_THREADS, [&](uint32_t t) { ks_stage2(sm, lh, L, t); });
+            if (L & 1u) hs_for(WMB_SPEC_THREADS, [&](uint32_t t) { ks_stage1(sm, L - 1, L, t); });
+            const uint32_t nvalid = ks_pass_blocks(u, pass, L);
+            hs_for(WMB_SPEC_THREADS, [&](uint32_t t) { ks_power(sm, nvalid, t, acc[t], L); });
+        }
+        for (int pk = 0; pk < 2; pk++) {
+            hs_for(WMB_SPEC_THREADS, [&](uint32_t t) { ks_red_put(sm, acc[t], t, pk == 1); });
+            hs_for(WMB_SPEC_THREADS, [&](uint32_t t) { ks_red_flush(p, sm, u, t, pk == 1, L); });
+        }
+    });
+    (void)st;
+#else
+    static int sms = 0;
+    if (!sms) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c->device);
+    const uint32_t grid = std::min<uint32_t>(p.n_units, (uint32_t)sms * 4u);
+    switch (p.logN) {                                  /* one instance per N: shifts and masks of constants */
+    case 8:  ks_fft_kernel<8><<<grid, WMB_SPEC_THREADS, 0, st>>>(p); break;
+    case 9:  ks_fft_kernel<9><<<grid, WMB_SPEC_THREADS, 0, st>>>(p); break;
+    case 10: ks_fft_kernel<10><<<grid, WMB_SPEC_THREADS, 0, st>>>(p); break;
+    default: ks_fft_kernel<11><<<grid, WMB_SPEC_THREADS, 0, st>>>(p); break;
+    }
+    CUDA_TRY(cudaGetLastError());
+#endif
+    c->st.kernel_launches++;
+    return WMB_OK;
+}
+
+static int launch_spec_close(wmb_ctx *c, const SpecCloseParams &p, cudaStream_t st)
+{
+#ifdef WMB_HOSTSIM
+    hs_for(p.n, [&](uint32_t j) { hs_for(p.N, [&](uint32_t k) { ks_close(p, j, k); }); });
+    (void)st;
+#else
+    ks_close_kernel<<<p.n, 256, 0, st>>>(p);
+    CUDA_TRY(cudaGetLastError());
+#endif
+    c->st.kernel_launches++;
     return WMB_OK;
 }
 
@@ -803,6 +878,67 @@ static int burst_alloc(wmb_ctx *c)
     return WMB_OK;
 }
 
+/* the survey's window and twiddles for N bins, in double, rounded once: hann[N] | tw[N / 2][2] */
+static void spec_tables(uint32_t N, float *hann, float *tw)
+{
+    const double pi = 3.14159265358979323846;
+    for (uint32_t n = 0; n < N; n++) hann[n] = (float)(0.5 - 0.5 * cos(2.0 * pi * (double)n / (double)N));
+    for (uint32_t k = 0; k < N / 2; k++) {
+        tw[2 * k] = (float)cos(2.0 * pi * (double)k / (double)N);
+        tw[2 * k + 1] = (float)-sin(2.0 * pi * (double)k / (double)N);
+    }
+}
+
+/* rows of the ring and of a slot table: a batch closes the record left open before it and all but the last of its
+ * own, and touches at most batch blocks / B + 2 consecutive records */
+static uint32_t spec_rows_for(const wmb_ctx *c, uint32_t N, uint32_t B)
+{
+    return (uint32_t)(c->max_batch_bytes / (2 * (size_t)N) / B + 2);
+}
+
+static int spec_free(wmb_ctx *c, void *p, bool host)
+{
+    if (!p) return WMB_OK;
+    std::vector<void *> &v = host ? c->host_allocs : c->dev_allocs;
+    v.erase(std::remove(v.begin(), v.end(), p), v.end());
+    CUDA_TRY(host ? cudaFreeHost(p) : cudaFree(p));
+    return WMB_OK;
+}
+
+/* the survey's buffers, at the first batch that needs them (again when a new setting needs larger tables) */
+static int spec_alloc(wmb_ctx *c)
+{
+    const uint32_t N = c->spec_bins;
+    c->spec_R = spec_rows_for(c, N, c->spec_B);
+    const size_t need = (size_t)c->spec_R * N;
+    if (need > c->spec_cap) {
+        CUDA_TRY(cudaDeviceSynchronize());
+        TRY(spec_free(c, c->d_ssum_ring, false)); TRY(spec_free(c, c->d_speak_ring, false));
+        TRY(spec_free(c, c->d_ssum, false)); TRY(spec_free(c, c->d_speak, false));
+        TRY(spec_free(c, c->h_ssum, true)); TRY(spec_free(c, c->h_speak, true));
+        c->spec_cap = 0;
+        TRY(dev_alloc(c, &c->d_ssum_ring, need, true));
+        TRY(dev_alloc(c, &c->d_speak_ring, need, true));
+        TRY(dev_alloc(c, &c->d_ssum, need * WMB_NSLOT));
+        TRY(dev_alloc(c, &c->d_speak, need * WMB_NSLOT));
+        TRY(host_alloc(c, &c->h_ssum, need * WMB_NSLOT));
+        TRY(host_alloc(c, &c->h_speak, need * WMB_NSLOT));
+        c->spec_cap = need;
+    }
+    if (!c->d_spec_tab) {
+        TRY(dev_alloc(c, &c->d_spec_tab, 2 * (size_t)WMB_SPEC_MAXN));
+        cudaEventCreateWithFlags(&c->ev_spec, cudaEventDisableTiming);
+        cudaEventCreateWithFlags(&c->ev_spec_flush, cudaEventDisableTiming);
+    }
+    if (c->spec_tab_n != N) {
+        std::vector<float> tab(2 * (size_t)N);
+        spec_tables(N, tab.data(), tab.data() + N);
+        CUDA_TRY(cudaMemcpy(c->d_spec_tab, tab.data(), tab.size() * sizeof(float), cudaMemcpyHostToDevice));
+        c->spec_tab_n = N;
+    }
+    return WMB_OK;
+}
+
 extern "C" int wmb_create(const wmb_opts *o, int cuda_device, wmb_ctx **out)
 {
     if (!o || !out) return set_err(WMB_E_INVAL, "null argument");
@@ -940,6 +1076,8 @@ extern "C" void wmb_destroy(wmb_ctx *c)
     if (c->k1s) cudaStreamDestroy(c->k1s);
     if (c->ev_push_start) cudaEventDestroy(c->ev_push_start);
     if (c->ev_reset) cudaEventDestroy(c->ev_reset);
+    if (c->ev_spec) cudaEventDestroy(c->ev_spec);
+    if (c->ev_spec_flush) cudaEventDestroy(c->ev_spec_flush);
     for (int i = 0; i < WMB_NSLOT; i++) {
         if (c->ev_res[i]) cudaEventDestroy(c->ev_res[i]);
         for (int k = 0; k < 6; k++) if (c->ev_t[i][k]) cudaEventDestroy(c->ev_t[i][k]);
@@ -1010,6 +1148,77 @@ static uint32_t pick_chunk_coop(const wmb_ctx *c, int64_t M)
  * device: refuted speculative lanes are re-run by on-device fix-up kernels, and the fallback from the two-phase
  * run-length path to the monolithic lanes is a set of kernels that do nothing unless the device flag asks for them.
  * input_ready: event after which `src` holds the bytes (H2D copy), or null.  alone: no batch follows in this push. */
+/* the band survey of one batch (IQ samples [q0, q0 + n_iq), bytes at src), on the demod stream sk while the batch's
+ * input is still valid: the FFT pass over its counted blocks, then the rows it closes -> the slot rows, zeroed in the
+ * ring.  The host knows which blocks count and which records close; the rows wait in spec_batch_rows for the gather. */
+static int spec_batch(wmb_ctx *c, const uint8_t *src, uint64_t q0, uint64_t n_iq, cudaStream_t sk, int slot)
+{
+    const uint64_t N = c->spec_bins, B = c->spec_B;
+    const int64_t p0 = (int64_t)(q0 / N), p1 = (int64_t)((q0 + n_iq) / N);
+    c->spec_batch_rows.clear();
+    if (p1 <= p0) return WMB_OK;
+    TRY(spec_alloc(c));
+    if (c->spec_flush_pending) { CUDA_TRY(cudaStreamWaitEvent(sk, c->ev_spec_flush, 0)); c->spec_flush_pending = false; }
+    /* floor(b N / d) in [win_lo, win_hi)  <=>  b in [ceil(win_lo d / N), ceil(win_hi d / N)) */
+    auto first_b = [&](uint64_t m) {
+        const unsigned __int128 x = ((unsigned __int128)m * c->d + N - 1) / N;
+        return x > (unsigned __int128)INT64_MAX ? INT64_MAX : (int64_t)x;
+    };
+    const int64_t c0 = std::max(p0, first_b(c->win_lo)), c1 = std::min(p1, first_b(c->win_hi));
+    const int64_t r_last = (p1 - 1) / (int64_t)B;
+    auto counted = [&](int64_t r) {
+        const int64_t lo = std::max(c0, r * (int64_t)B), hi = std::min(c1, (r + 1) * (int64_t)B);
+        return (uint32_t)(hi > lo ? hi - lo : 0) + (r == c->spec_open ? c->spec_open_blocks : 0u);
+    };
+    int64_t lone = -1, r_lo = 0, r_hi = 0;          /* closed: lone (if any), then records [r_lo, r_hi) */
+    int64_t open = -1;
+    if (c1 > c0) {
+        SpecParams p;
+        memset(&p, 0, sizeof(p));
+        p.in = src; p.b_first = p0; p.c0 = c0; p.c1 = c1;
+        p.N = (uint32_t)N; p.logN = (uint32_t)__builtin_ctz((uint32_t)N); p.B = (uint32_t)B;
+        /* units: about 4 per SM-resident CTA slot of the largest batch; any size gives the same sums and maxima */
+        const uint32_t per = WMB_SPEC_POINTS / (uint32_t)N;
+        const uint64_t G = std::max<uint64_t>(per, ((uint64_t)(c1 - c0) / 2048 + per - 1) / per * per);
+        p.G = (uint32_t)std::min<uint64_t>(G, B); p.U = (uint32_t)((B + p.G - 1) / p.G);
+        p.g_lo = (c0 / (int64_t)B) * p.U + (c0 % (int64_t)B) / p.G;
+        const int64_t g_hi = ((c1 - 1) / (int64_t)B) * p.U + ((c1 - 1) % (int64_t)B) / p.G;
+        p.n_units = (uint32_t)(g_hi - p.g_lo + 1);
+        p.R = c->spec_R; p.hann = c->d_spec_tab; p.tw = c->d_spec_tab + N;
+        p.sum = c->d_ssum_ring; p.peak = c->d_speak_ring;
+        TRY(launch_spectrum(c, p, sk));
+        const int64_t rc0 = c0 / (int64_t)B, rc1 = (c1 - 1) / (int64_t)B;
+        if (c->spec_open >= 0 && c->spec_open != rc0) lone = c->spec_open;
+        r_lo = rc0; r_hi = std::min(rc1 + 1, r_last);
+        if (rc1 == r_last) open = rc1;
+    } else if (c->spec_open >= 0) {
+        if (c->spec_open < r_last) lone = c->spec_open; else open = c->spec_open;
+    }
+    const double fs = 0.8e6 * (double)c->d;
+    auto row = [&](int64_t r) {
+        wmb_spectrum_row w;
+        memset(&w, 0, sizeof(w));
+        w.record = (uint64_t)r; w.start_iq = (uint64_t)r * B * N; w.blocks = counted(r); w.bins = (uint32_t)N;
+        w.hz_low = -fs / 2; w.hz_step = fs / (double)N;
+        return w;
+    };
+    if (lone >= 0) c->spec_batch_rows.push_back(row(lone));
+    for (int64_t r = r_lo; r < r_hi; r++) c->spec_batch_rows.push_back(row(r));
+    const uint32_t open_blocks = open >= 0 ? counted(open) : 0u;
+    if (!c->spec_batch_rows.empty()) {
+        SpecCloseParams q;
+        memset(&q, 0, sizeof(q));
+        q.sum = c->d_ssum_ring; q.peak = c->d_speak_ring;
+        q.out_sum = c->d_ssum + (size_t)slot * c->spec_cap; q.out_peak = c->d_speak + (size_t)slot * c->spec_cap;
+        q.lone = lone; q.r_lo = r_lo; q.n = (uint32_t)c->spec_batch_rows.size(); q.N = (uint32_t)N; q.R = c->spec_R;
+        TRY(launch_spec_close(c, q, sk));
+    }
+    c->spec_open = open; c->spec_open_blocks = open_blocks;
+    CUDA_TRY(cudaEventRecord(c->ev_spec, sk));
+    c->spec_enqueued = true;
+    return WMB_OK;
+}
+
 static int run_batch(wmb_ctx *c, const uint8_t *src, size_t nbytes, cudaEvent_t input_ready, bool alone)
 {
     tr("batch-start");
@@ -1081,6 +1290,8 @@ static int run_batch(wmb_ctx *c, const uint8_t *src, size_t nbytes, cudaEvent_t 
         }
         c->hist_iq = std::min<int64_t>(c->hist_iq + n_iq, (int64_t)hb / 2);
     }
+    /* the band survey reads the input in place */
+    if (c->spec_bins) TRY(spec_batch(c, src, c->iq_consumed, (uint64_t)n_iq, sk, slot));
     /* the input buffer may be overwritten by the next H2D from here on */
     CUDA_TRY(cudaEventRecord(c->ev_k1done[c->buf_idx], sk));
 
@@ -1410,6 +1621,46 @@ static int enqueue_gather(wmb_ctx *c, bool final, bool after_batch)
             CUDA_TRY(cudaMemcpyAsync(c->h_brec + at, c->d_brec + at, (size_t)c->burst_spec * sizeof(BurstRec), cudaMemcpyDeviceToHost, c->cs));
         }
     }
+    /* the band survey: the rows the batch closed (its kernels ran on the demod stream), or at the end of input the
+     * record still open */
+    bool spec = false;
+    if (c->spec_bins) {
+        std::vector<wmb_spectrum_row> &rows = c->spec_slot_rows[slot];
+        rows.clear();
+        /* cs follows the demod stream only as far as the demod kernel; the survey kernels behind it may still be adding
+         * into the open record's ring row.  Every close that cs issues (the flush's, or the next solo batch's on sk = cs)
+         * and every copy of a slot comes after this wait, whether the batch closed a record or not */
+        if (c->spec_enqueued) {
+            CUDA_TRY(cudaStreamWaitEvent(c->cs, c->ev_spec, 0));
+            c->spec_enqueued = false;
+        }
+        if (after_batch && !c->spec_batch_rows.empty()) {
+            rows.swap(c->spec_batch_rows);
+        } else if (final && c->spec_open >= 0) {
+            const uint64_t N = c->spec_bins, B = c->spec_B;
+            const double fs = 0.8e6 * (double)c->d;
+            wmb_spectrum_row w;
+            memset(&w, 0, sizeof(w));
+            w.record = (uint64_t)c->spec_open; w.start_iq = w.record * B * N; w.blocks = c->spec_open_blocks;
+            w.bins = (uint32_t)N; w.hz_low = -fs / 2; w.hz_step = fs / (double)N;
+            rows.push_back(w);
+            SpecCloseParams q;
+            memset(&q, 0, sizeof(q));
+            q.sum = c->d_ssum_ring; q.peak = c->d_speak_ring;
+            q.out_sum = c->d_ssum + (size_t)slot * c->spec_cap; q.out_peak = c->d_speak + (size_t)slot * c->spec_cap;
+            q.lone = c->spec_open; q.n = 1; q.N = (uint32_t)N; q.R = c->spec_R;
+            TRY(launch_spec_close(c, q, c->cs));
+            CUDA_TRY(cudaEventRecord(c->ev_spec_flush, c->cs));
+            c->spec_flush_pending = true;
+            c->spec_open = -1; c->spec_open_blocks = 0;
+        }
+        if (!rows.empty()) {
+            const size_t at = (size_t)slot * c->spec_cap, n = rows.size() * (size_t)c->spec_bins;
+            CUDA_TRY(cudaMemcpyAsync(c->h_ssum + at, c->d_ssum + at, n * sizeof(uint64_t), cudaMemcpyDeviceToHost, c->cs));
+            CUDA_TRY(cudaMemcpyAsync(c->h_speak + at, c->d_speak + at, n * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->cs));
+            spec = true;
+        }
+    }
     CUDA_TRY(cudaEventRecord(c->ev_res[slot], c->cs));
     /* ev_chain[set] releases the batch's set to the demod kernel of batch i+2 (run_batch waits for it on k1s): it is
      * recorded here, behind the gather on cs, so k3_fill's reads of the set's dphi come before that kernel's writes */
@@ -1420,6 +1671,7 @@ static int enqueue_gather(wmb_ctx *c, bool final, bool after_batch)
     wmb_ctx::InFlight f;
     f.slot = slot; f.final = final; f.has_timers = after_batch; f.m_end = c->m_consumed; f.bursts = bursts;
     f.burst_spec = c->burst_spec;                    /* records the copies above fetched (burst_spec may grow before they are read) */
+    f.spec = spec;
     c->inflight.push_back(f);
     c->gather_no++;
     return WMB_OK;
@@ -1450,6 +1702,14 @@ static int consume_oldest(wmb_ctx *c)
         if (cudaEventElapsedTime(&ms, c->ev_push_start, evt[3]) == cudaSuccess) c->acc_pass_ms = ms;
     }
     if (f.bursts) TRY(book_bursts(c, f.slot, f.m_end, f.burst_spec));
+    if (f.spec) {                                    /* the slot's survey rows -> the queue */
+        const std::vector<wmb_spectrum_row> &rows = c->spec_slot_rows[f.slot];
+        const size_t at = (size_t)f.slot * c->spec_cap, n = rows.size() * (size_t)c->spec_bins;
+        c->spec_rows.insert(c->spec_rows.end(), rows.begin(), rows.end());
+        c->spec_sum.insert(c->spec_sum.end(), c->h_ssum + at, c->h_ssum + at + n);
+        c->spec_peak.insert(c->spec_peak.end(), c->h_speak + at, c->h_speak + at + n);
+        c->st.d2h_bytes += n * (sizeof(uint64_t) + sizeof(uint32_t));
+    }
     if (!any_sync) return WMB_OK;
     const bool dev_decode = !c->manual;
     const size_t lb = (size_t)f.slot * c->slot_cap, pb = (size_t)f.slot * c->slot_pool;
@@ -2030,6 +2290,8 @@ extern "C" int wmb_reset(wmb_ctx *c)
     c->chain_recorded[0] = c->chain_recorded[1] = false;
     c->stat_rerun_seen = 0; c->stat_fallback_seen = 0;
     c->bursts.clear(); c->burst_frontier = 0;
+    c->spec_open = -1; c->spec_open_blocks = 0; c->spec_batch_rows.clear(); c->spec_enqueued = false;
+    c->spec_rows.clear(); c->spec_sum.clear(); c->spec_peak.clear();
     for (int ch = 0; ch < WMB_N_CHAINS; ch++)
         for (int a = 0; a < WMB_N_ALGOS; a++) { Stream &s = c->cb[ch].s[a]; s.total = 0; s.total_prev = 0; s.busy_until = -1; }
     if (c->allocated) {
@@ -2052,6 +2314,10 @@ extern "C" int wmb_reset(wmb_ctx *c)
         if (c->burst_allocated)                  /* no run open */
             for (int ch = 0; ch < WMB_N_CHAINS; ch++)
                 if (c->bb[ch].bd) CUDA_TRY(cudaMemsetAsync(c->bb[ch].bd, 0, sizeof(BurstDev), c->cs));
+        if (c->spec_cap) {                       /* no record open */
+            CUDA_TRY(cudaMemsetAsync(c->d_ssum_ring, 0, c->spec_cap * sizeof(uint64_t), c->cs));
+            CUDA_TRY(cudaMemsetAsync(c->d_speak_ring, 0, c->spec_cap * sizeof(uint32_t), c->cs));
+        }
         CUDA_TRY(cudaEventRecord(c->ev_reset, c->cs));
         c->reset_pending = true;
     }
@@ -2110,6 +2376,51 @@ extern "C" int wmb_take_bursts(wmb_ctx *c, wmb_burst *out, size_t cap, size_t *n
     if (k) memcpy(out, c->bursts.data(), k * sizeof(wmb_burst));
     c->bursts.erase(c->bursts.begin(), c->bursts.begin() + (long)k);
     *n = k;
+    return WMB_OK;
+}
+
+extern "C" int wmb_set_spectrum(wmb_ctx *c, uint32_t bins, uint32_t blocks_per_record)
+{
+    if (!c) return set_err(WMB_E_INVAL, "null argument");
+    if (bins != 0) {
+        if (bins != 256 && bins != 512 && bins != 1024 && bins != 2048)
+            return set_err(WMB_E_INVAL, "spectrum bins %u: 256, 512, 1024 or 2048 (0: off)", bins);
+        if (blocks_per_record < 1 || blocks_per_record > (1u << 20))
+            return set_err(WMB_E_INVAL, "blocks per record %u out of range 1 .. 2^20", blocks_per_record);
+        const uint64_t table = (uint64_t)spec_rows_for(c, bins, blocks_per_record) * bins;
+        if (table > (1ull << 23))
+            return set_err(WMB_E_INVAL, "spectrum table of %llu bins for %zu MiB batches (at most 2^23): raise blocks per record "
+                           "or lower max_batch_mib", (unsigned long long)table, c->max_batch_bytes >> 20);
+    }
+    if (c->batch_no != 0 || !c->remainder.empty())
+        return set_err(WMB_E_STATE, "wmb_set_spectrum after samples were pushed (call it before the first push or after wmb_reset / wmb_seek)");
+    c->spec_bins = bins;
+    c->spec_B = bins ? blocks_per_record : 0;
+    return WMB_OK;
+}
+
+extern "C" int wmb_take_spectrum(wmb_ctx *c, wmb_spectrum_row *rows, uint64_t *sum, float *peak, size_t cap, size_t *n)
+{
+    if (!c || !n || (cap && (!rows || !sum || !peak))) return set_err(WMB_E_INVAL, "null argument");
+    const size_t k = std::min(cap, c->spec_rows.size());
+    size_t bins = 0;
+    for (size_t i = 0; i < k; i++) {
+        rows[i] = c->spec_rows[i];
+        memcpy(sum + bins, c->spec_sum.data() + bins, (size_t)rows[i].bins * sizeof(uint64_t));
+        memcpy(peak + bins, c->spec_peak.data() + bins, (size_t)rows[i].bins * sizeof(float));
+        bins += rows[i].bins;
+    }
+    c->spec_rows.erase(c->spec_rows.begin(), c->spec_rows.begin() + (long)k);
+    c->spec_sum.erase(c->spec_sum.begin(), c->spec_sum.begin() + (long)bins);
+    c->spec_peak.erase(c->spec_peak.begin(), c->spec_peak.begin() + (long)bins);
+    *n = k;
+    return WMB_OK;
+}
+
+extern "C" int wmb_debug_spectrum_tables(uint32_t bins, float *hann, float *tw)
+{
+    if (!hann || !tw || (bins != 256 && bins != 512 && bins != 1024 && bins != 2048)) return set_err(WMB_E_INVAL, "bad argument");
+    spec_tables(bins, hann, tw);
     return WMB_OK;
 }
 

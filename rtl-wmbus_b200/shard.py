@@ -94,8 +94,77 @@ def merge_bursts(parts):
     return recs[np.lexsort((recs["chain"], recs["start_sample"]))]
 
 
+def merge_spectrum(parts):
+    """Band-survey records (rows, sum, peak) of several time chunks -> the sequential run's records: sum and blocks
+    added, peak the max, over the rows of one record (a record that straddles a chunk border has a row in each)."""
+    import numpy as np
+    full = [p for p in parts if len(p[0])]                # (a chunk may hold no record)
+    if not full:
+        return parts[0]
+    rows = np.concatenate([p[0] for p in full])
+    sums = np.concatenate([p[1] for p in full])
+    peaks = np.concatenate([p[2] for p in full])
+    recs, inv = np.unique(rows["record"], return_inverse=True)
+    out = np.zeros(len(recs), rows.dtype)
+    first = np.full(len(recs), -1)
+    for i in range(len(rows)):
+        if first[inv[i]] < 0:
+            first[inv[i]] = i
+    out[:] = rows[first]
+    out["blocks"] = np.bincount(inv, weights=rows["blocks"], minlength=len(recs)).astype(np.uint32)
+    s = np.zeros((len(recs), sums.shape[1]), np.uint64)
+    p = np.zeros((len(recs), peaks.shape[1]), np.float32)
+    np.add.at(s, inv, sums)
+    np.maximum.at(p, inv, peaks)
+    return out, s, p
+
+
+def find_carriers(rows, sum, peak, fs: float, threshold_db: float = 15.0, bridge_hz: float = 110e3,
+                  tone_hz: float = 20e3):
+    """Carriers worth decoding in a band survey (take_spectrum / merge_spectrum output, or a CLI spectrum file read
+    with tools/find_carriers.py), fs the capture's sample rate (0.8 d MHz).  The bins' frequencies come from the rows'
+    hz_low and hz_step; fs is checked against them (a survey of another capture rate raises ValueError).
+      mean[k] = sum of sum / sum of blocks, hold[k] = max peak, floor = the median over k of mean;
+      a bin is hot when hold >= floor * 10^(T / 10), T = 15 dB: in the tests' captures a meter's FSK tones stand 30 dB
+        and more above the floor in the peak hold, while noise alone stays below 12 dB there (its hold over 16384 blocks
+        is about ln(16384) = 9.7 times, 9.9 dB, the mean);
+      hot bins within 110 kHz of each other are one region: S1's two tones lie 100 kHz apart (T1/C1's 80-100 kHz);
+      a region's carrier is its hold-weighted mean frequency -- between the two FSK tones -- rounded to the 25 kHz grid
+        of the mixer (rtl_wmbus.c:974-993); a region narrower than 20 kHz is a tone (a CW carrier, a spur), not a meter.
+    Returns (carriers, tones): carriers a list [(offset_khz, "T"), (offset_khz, "S"), ...] for decode_carriers() -- the
+    kind cannot be read off the spectrum, so each carrier gets a context with both chains on it -- and tones a list of
+    their frequencies in Hz."""
+    import numpy as np
+    rows = np.asarray(rows)
+    if not len(rows):
+        return [], []
+    if abs(-2.0 * float(rows["hz_low"][0]) - fs) > 1e-6 * fs:
+        raise ValueError(f"the survey covers {-2.0 * float(rows['hz_low'][0]):.0f} Hz, not fs = {fs:.0f} Hz")
+    n = rows["bins"][0]
+    mean = np.asarray(sum, np.float64).sum(axis=0) / float(rows["blocks"].sum())
+    hold = np.asarray(peak, np.float64).max(axis=0)
+    floor = float(np.median(mean))
+    freq = rows["hz_low"][0] + rows["hz_step"][0] * np.arange(n)
+    hot = np.flatnonzero(hold >= floor * 10 ** (threshold_db / 10))
+    carriers, tones = [], []
+    if not len(hot):
+        return carriers, tones
+    regions = np.split(hot, np.flatnonzero(np.diff(freq[hot]) >= bridge_hz) + 1)
+    step = float(rows["hz_step"][0])
+    for reg in regions:
+        width = freq[reg[-1]] - freq[reg[0]] + step
+        f = float((freq[reg] * hold[reg]).sum() / hold[reg].sum())
+        if width < tone_hz:
+            tones.append(f)
+            continue
+        off = int(round(f / 25e3)) * 25
+        if (off, "T") not in carriers:
+            carriers += [(off, "T"), (off, "S")]
+    return carriers, tones
+
+
 def decode_time_chunk(ctx, push, n_bytes: int, d: int, rank: int, world: int, halo_m: int = 1 << 18, info=False,
-                      bursts=False):
+                      bursts=False, spectrum=False):
     """Decode rank `rank`'s chunk of a capture of n_bytes cu8 bytes.  `push(byte_lo, byte_hi)` feeds that byte
     range of the capture to ctx (host or device memory: the caller's business).
     Returns (lines, digest_start, digest_end, halo_start_iq): digest_start is None for a chunk that starts at 0.
@@ -105,10 +174,17 @@ def decode_time_chunk(ctx, push, n_bytes: int, d: int, rank: int, world: int, ha
     bursts=True (ctx made with a burst level): lines is (lines[, records], bursts), bursts the chunk's burst pieces -- those
     that start in [lo, hi) of decimated samples.  A piece depends on its samples and at most 2^17 + 2^16 + 196 before it
     (DESIGN.md §8), inside the left halo, and one that starts before hi is closed within as many samples after hi, inside
-    the right halo, so they are the sequential run's pieces."""
+    the right halo, so they are the sequential run's pieces.
+    spectrum=True (ctx made with spectrum=...): the band survey's records (rows, sum, peak) come last in lines.  The line
+    window counts the chunk's blocks only, so merge_spectrum() over the chunks gives the sequential records."""
     import hashlib
     recs = []
     brecs = []
+    srecs = []
+
+    def take_s():
+        if spectrum:
+            srecs.append(ctx.take_spectrum())
 
     def take_b():
         if bursts:
@@ -132,11 +208,13 @@ def decode_time_chunk(ctx, push, n_bytes: int, d: int, rank: int, world: int, ha
         push(2 * start, 2 * lo)
         lines += take()
         take_b()
+        take_s()
     if lo > 0:
         dig_start = hashlib.sha256(ctx.boundary_state()).digest()
     push(2 * lo, 2 * hi)
     lines += take()
     take_b()
+    take_s()
     dig_end = hashlib.sha256(ctx.boundary_state()).digest()
     if rank + 1 < world:                              # finish the telegrams that started in the chunk
         step = (MAX_TELEGRAM_M * d + gran - 1) // gran * gran
@@ -156,6 +234,7 @@ def decode_time_chunk(ctx, push, n_bytes: int, d: int, rank: int, world: int, ha
         ctx.poll_flush()
     lines += take()
     take_b()
+    take_s()
     if info:
         import numpy as np
         lines = (lines, np.concatenate(recs))
@@ -165,10 +244,17 @@ def decode_time_chunk(ctx, push, n_bytes: int, d: int, rank: int, world: int, ha
         m_lo, m_hi = lo // d, (hi // d if rank + 1 < world else 1 << 63)
         b = b[(b["start_sample"] >= m_lo) & (b["start_sample"] < m_hi)]
         lines = (lines + (b,)) if info else (lines, b)
+    if spectrum:
+        import numpy as np
+        srecs = [x for x in srecs if len(x[0])] or srecs[:1]
+        sp = (np.concatenate([x[0] for x in srecs]), np.concatenate([x[1] for x in srecs]),
+              np.concatenate([x[2] for x in srecs]))
+        lines = (lines + (sp,)) if isinstance(lines, tuple) else (lines, sp)
     return lines, dig_start, dig_end, start
 
 
-def decode_time_sharded(ctx, push, n_bytes: int, d: int, halo_m: int = 1 << 18, info=False, bursts=False):
+def decode_time_sharded(ctx, push, n_bytes: int, d: int, halo_m: int = 1 << 18, info=False, bursts=False,
+                        spectrum=False):
     """All ranks: decode one capture in time chunks, exact by construction (see module docstring).
     Returns (my_lines, rounds); info=True / bursts=True: my_lines carries the records / burst pieces as in
     decode_time_chunk."""
@@ -180,7 +266,8 @@ def decode_time_sharded(ctx, push, n_bytes: int, d: int, halo_m: int = 1 << 18, 
     while True:
         rounds += 1
         if redo:
-            lines, ds, de, start = decode_time_chunk(ctx, push, n_bytes, d, rank, world, halo_m, info=info, bursts=bursts)
+            lines, ds, de, start = decode_time_chunk(ctx, push, n_bytes, d, rank, world, halo_m, info=info, bursts=bursts,
+                                                        spectrum=spectrum)
         mine = torch.zeros(65, dtype=torch.uint8)
         mine[:32] = torch.frombuffer(bytearray(ds or bytes(32)), dtype=torch.uint8)
         mine[32:64] = torch.frombuffer(bytearray(de), dtype=torch.uint8)
