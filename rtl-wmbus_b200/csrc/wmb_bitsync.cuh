@@ -4,8 +4,9 @@
  * a float recurrence, a branchy integer state machine and event output shared one loop.)
  *
  *   K2a  k2a_lane      float-only lanes: [DC block] -> slicer bit, x^2 -> 3 biquads ->
- *                      clock sign -> lock stencil.  Writes two bit-packed streams per
- *                      decimated sample: dbits (data bit) and sbits (time2 strobe).
+ *                      clock sign -> lock stencil.  Writes bit-packed streams per
+ *                      decimated sample: sbits (time2 strobe) and, with -o, dbits (data
+ *                      bit; without the DC block the demod kernel K1 slices them).
  *                      Speculative warm-up + state verification (rtl_wmbus.c:497-515,
  *                      :1059, :1089-1111; iir.h:59-74).
  *   K2t  k2t_*         time2 bit stream: strobed data bits -> shift register -> access
@@ -29,7 +30,8 @@ struct K2aParams {
     const float *dphi;          /* index 0 = batch sample 0; [-hist, M) readable              */
     int64_t  M, hist;
     uint32_t C, W, lanes;       /* all multiples of 32                                        */
-    uint32_t *dbits, *sbits;    /* word w covers samples 32w..32w+31 (bit i = sample 32w+i)   */
+    uint32_t *dbits, *sbits;    /* word w covers samples 32w..32w+31 (bit i = sample 32w+i); dbits written with -o only:
+                                   without the DC block the demod kernel slices them                */
     uint32_t *cbits;            /* optional stage tap: the clock signs (null unless the context was made with taps) */
     IirState *st_start, *st_end;
     const IirState *carry;
@@ -249,7 +251,7 @@ WMB_D void k2a_lane_t(const K2aParams &p, uint32_t lane)
         r.clk3 = lock_history<LK>(r.clk3, cword, n, p.lock);
         if (m >= s0) {
             const uint32_t keep = (n == 32) ? 0xFFFFFFFFu : ((1u << n) - 1u);
-            p.dbits[m >> 5] = dword & keep;
+            if (DC) p.dbits[m >> 5] = dword & keep;
             p.sbits[m >> 5] = sword & keep;
             if (p.cbits) p.cbits[m >> 5] = cword & keep;
         }
@@ -328,8 +330,8 @@ __device__ __forceinline__ void k2a2_step(K2a2Thread &t, const float xs, const i
     const float out = wmb_fadd(wmb_fadd(h0, wmb_fmul(t.b1, t.h1)), wmb_fmul(t.b2, t.h2));
     t.h2 = t.h1; t.h1 = h0; t.o = out;
     if (OUT) {
-        const float z = t.r0 ? xs : wmb_fmul(out, gain);          /* data bit (rtl_wmbus.c:1059) / clock sign */
-        if (z >= 0.0f) t.R |= 1u << i;
+        /* clock sign (only the last section's bits are kept; the data bits come from the demod kernel) */
+        if (wmb_fmul(out, gain) >= 0.0f) t.R |= 1u << i;
     }
 }
 
@@ -412,7 +414,6 @@ __global__ void __launch_bounds__(K2A2_THREADS) k2a2_lanes_kernel(const K2aParam
         }
         if (valid && jb >= jw && jb < je) {
             const int64_t w = (m0 >> 5) + jb;                               /* word of the batch (m0 is a multiple of 32) */
-            if (t.r0) p.dbits[w] = A;
             if (t.r2) { p.sbits[w] = sword; if (p.cbits) p.cbits[w] = A; }
         }
         if (at_start || at_end) {

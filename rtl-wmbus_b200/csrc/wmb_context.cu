@@ -136,12 +136,16 @@ struct wmb_ctx {
     /* Streams: k1s runs the demod kernels of consecutive batches back to back; as[set] the clock-recovery lanes of
      * a batch (they only need its demod output, so they overlap the next batch's demod and each other); cs everything
      * that is sequential from batch to batch (lane verification, bit streams, gather, framer, result copies), with ts
-     * (time2) and s2 (S1 run-length lanes) forked from and joined to it; xs the H2D copies. */
+     * (time2) and s2 (S1 run-length lanes) forked from and joined to it; xs the H2D copies.  When the demod kernel
+     * slices the data bits, the run-length path starts behind it instead, beside the clock lanes: T1/C1 on rs, S1 on
+     * s2, both forked from cs at the start of the batch (run_batch). */
     cudaStream_t cs = nullptr, xs = nullptr, k1s = nullptr, as[2] = {nullptr, nullptr}, as2[2] = {nullptr, nullptr};
     cudaStream_t ts = nullptr;
     cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
     cudaStream_t s2 = nullptr;
     cudaEvent_t ev_fork2 = nullptr, ev_join2 = nullptr;
+    cudaStream_t rs = nullptr;
+    cudaEvent_t ev_join_rs = nullptr;
     cudaEvent_t ev_h2d[2] = {nullptr, nullptr}, ev_k1done[2] = {nullptr, nullptr};
     cudaEvent_t ev_k1[2] = {nullptr, nullptr}, ev_k2a[2] = {nullptr, nullptr}, ev_k2a2[2] = {nullptr, nullptr}, ev_chain[2] = {nullptr, nullptr};
     bool chain_recorded[2] = {false, false};
@@ -267,6 +271,14 @@ static uint32_t *gd_field(wmb_ctx *c, size_t off) { return (uint32_t *)((uint8_t
 
 #ifdef WMB_HOSTSIM
 #include "hostsim_launch.inl"
+/* the CPU build runs every launch when it is enqueued, in the order of the calls: the stream is not needed */
+static int launch_k2p1(wmb_ctx *c, const K2p1Params &p, cudaStream_t) { return launch_k2p1(c, p); }
+static int launch_k2p_rest(wmb_ctx *c, const K2pcParams &pc, const K2p2Params &p2, cudaStream_t) { return launch_k2p_rest(c, pc, p2); }
+static int launch_k2p_fold(wmb_ctx *c, const P1State *p1_end_last, RlState *p2_out, RlState *carry, const K2pDev *pd,
+                           const RlState *mono_end, cudaStream_t)
+{
+    return launch_k2p_fold(c, p1_end_last, p2_out, carry, pd, mono_end);
+}
 #else
 static int g_k1_ctas = 0;                /* WMBUS_B200_K1_CTAS: resident demod blocks per SM (0: as many as fit) */
 
@@ -365,13 +377,13 @@ static int launch_k2m(wmb_ctx *c, int chain, const K2mParams &p, cudaStream_t st
     return WMB_OK;
 }
 
-static int launch_k2p1(wmb_ctx *c, const K2p1Params &p)
+static int launch_k2p1(wmb_ctx *c, const K2p1Params &p, cudaStream_t st)
 {
     uint32_t *nf = c->d_nfail + 4;
-    k2p1_lanes_kernel<<<(p.lanes + 127) / 128, 128, 0, c->cs>>>(p);
-    k2p1_verify_kernel<<<(p.lanes + 255) / 256, 256, 0, c->cs>>>(p, nf);
-    if (g_fixseg & 4) k2p1_fixseg_kernel<<<(p.lanes + FIX_SEG - 1) / FIX_SEG, FIX_SEG, 0, c->cs>>>(p, nf, GD_FIELD(c, lanes_rerun));
-    k2p1_fixup_kernel<<<1, FIX_THREADS, 0, c->cs>>>(p, nf, GD_FIELD(c, lanes_rerun), c->d_errors);
+    k2p1_lanes_kernel<<<(p.lanes + 127) / 128, 128, 0, st>>>(p);
+    k2p1_verify_kernel<<<(p.lanes + 255) / 256, 256, 0, st>>>(p, nf);
+    if (g_fixseg & 4) k2p1_fixseg_kernel<<<(p.lanes + FIX_SEG - 1) / FIX_SEG, FIX_SEG, 0, st>>>(p, nf, GD_FIELD(c, lanes_rerun));
+    k2p1_fixup_kernel<<<1, FIX_THREADS, 0, st>>>(p, nf, GD_FIELD(c, lanes_rerun), c->d_errors);
     CUDA_TRY(cudaGetLastError());
     c->st.kernel_launches += 4;
     return WMB_OK;
@@ -393,23 +405,23 @@ static void launch_cscan(wmb_ctx *c, const uint32_t *cnt, uint64_t *base, uint32
 }
 
 /* two-phase run-length path after phase 1: records -> phase 2 -> ring (the carried state is folded later) */
-static int launch_k2p_rest(wmb_ctx *c, const K2pcParams &pc, K2p2Params p2)
+static int launch_k2p_rest(wmb_ctx *c, const K2pcParams &pc, K2p2Params p2, cudaStream_t st)
 {
-    launch_cscan(c, pc.cnt, pc.base, pc.lanes, pc.agg, &pc.pd->n_rec, nullptr, &pc.pd->fallback, 1);
-    k2pc_compact_kernel<<<pc.lanes, 128, 0, c->cs>>>(pc);
-    k2p2_count_kernel<<<(p2.lanes + g_p2_block - 1) / g_p2_block, g_p2_block, 0, c->cs>>>(p2);
-    k2p2_sum_kernel<<<p2.lanes, K2P2W_THREADS, 0, c->cs>>>(p2);
-    launch_cscan(c, p2.cnt, p2.base, p2.lanes, p2.agg, &p2.sd->total, &p2.pd->fallback);
-    k2p2_write_kernel<<<p2.lanes, K2P2W_THREADS, 0, c->cs>>>(p2);
+    launch_cscan(c, pc.cnt, pc.base, pc.lanes, pc.agg, &pc.pd->n_rec, nullptr, &pc.pd->fallback, 1, st);
+    k2pc_compact_kernel<<<pc.lanes, 128, 0, st>>>(pc);
+    k2p2_count_kernel<<<(p2.lanes + g_p2_block - 1) / g_p2_block, g_p2_block, 0, st>>>(p2);
+    k2p2_sum_kernel<<<p2.lanes, K2P2W_THREADS, 0, st>>>(p2);
+    launch_cscan(c, p2.cnt, p2.base, p2.lanes, p2.agg, &p2.sd->total, &p2.pd->fallback, nullptr, 0, st);
+    k2p2_write_kernel<<<p2.lanes, K2P2W_THREADS, 0, st>>>(p2);
     CUDA_TRY(cudaGetLastError());
     c->st.kernel_launches += 4;
     return WMB_OK;
 }
 
 static int launch_k2p_fold(wmb_ctx *c, const P1State *p1_end_last, RlState *p2_out, RlState *carry, const K2pDev *pd,
-                           const RlState *mono_end)
+                           const RlState *mono_end, cudaStream_t st)
 {
-    k2p_fold_kernel<<<1, 32, 0, c->cs>>>(p1_end_last, p2_out, carry, pd, mono_end, GD_FIELD(c, rl_fallbacks));
+    k2p_fold_kernel<<<1, 32, 0, st>>>(p1_end_last, p2_out, carry, pd, mono_end, GD_FIELD(c, rl_fallbacks));
     CUDA_TRY(cudaGetLastError());
     c->st.kernel_launches += 1;
     return WMB_OK;
@@ -1035,7 +1047,8 @@ extern "C" int wmb_create(const wmb_opts *o, int cuda_device, wmb_ctx **out)
         cudaStreamCreateWithFlags(&c->as2[0], cudaStreamNonBlocking) != cudaSuccess ||
         cudaStreamCreateWithFlags(&c->as2[1], cudaStreamNonBlocking) != cudaSuccess ||
         cudaStreamCreateWithFlags(&c->ts, cudaStreamNonBlocking) != cudaSuccess ||
-        cudaStreamCreateWithFlags(&c->s2, cudaStreamNonBlocking) != cudaSuccess) {
+        cudaStreamCreateWithFlags(&c->s2, cudaStreamNonBlocking) != cudaSuccess ||
+        cudaStreamCreateWithFlags(&c->rs, cudaStreamNonBlocking) != cudaSuccess) {
         delete c;
         return set_err(WMB_E_CUDA, "cannot create CUDA streams");
     }
@@ -1055,6 +1068,7 @@ extern "C" int wmb_create(const wmb_opts *o, int cuda_device, wmb_ctx **out)
     cudaEventCreate(&c->ev_join);
     cudaEventCreate(&c->ev_fork2);
     cudaEventCreate(&c->ev_join2);
+    cudaEventCreateWithFlags(&c->ev_join_rs, cudaEventDisableTiming);
     *out = c;
     return WMB_OK;
 }
@@ -1067,7 +1081,7 @@ extern "C" void wmb_destroy(wmb_ctx *c)
     if (c->xs) cudaStreamSynchronize(c->xs);
     for (void *p : c->dev_allocs) cudaFree(p);
     for (void *p : c->host_allocs) cudaFreeHost(p);
-    for (cudaStream_t st : { c->k1s, c->as[0], c->as[1], c->as2[0], c->as2[1], c->ts, c->s2 }) if (st) cudaStreamSynchronize(st);
+    for (cudaStream_t st : { c->k1s, c->as[0], c->as[1], c->as2[0], c->as2[1], c->ts, c->s2, c->rs }) if (st) cudaStreamSynchronize(st);
     for (int i = 0; i < 2; i++) {
         for (cudaEvent_t e : { c->ev_h2d[i], c->ev_k1done[i], c->ev_k1[i], c->ev_k2a[i], c->ev_k2a2[i], c->ev_chain[i] }) if (e) cudaEventDestroy(e);
         if (c->as[i]) cudaStreamDestroy(c->as[i]);
@@ -1088,6 +1102,8 @@ extern "C" void wmb_destroy(wmb_ctx *c)
     if (c->ev_fork2) cudaEventDestroy(c->ev_fork2);
     if (c->ev_join2) cudaEventDestroy(c->ev_join2);
     if (c->s2) cudaStreamDestroy(c->s2);
+    if (c->ev_join_rs) cudaEventDestroy(c->ev_join_rs);
+    if (c->rs) cudaStreamDestroy(c->rs);
     if (c->cs) cudaStreamDestroy(c->cs);
     if (c->xs) cudaStreamDestroy(c->xs);
     delete c;
@@ -1241,6 +1257,9 @@ static int run_batch(wmb_ctx *c, const uint8_t *src, size_t nbytes, cudaEvent_t 
         for (cudaStream_t st : { c->k1s, c->as[0], c->as[1], c->as2[0], c->as2[1] }) CUDA_TRY(cudaStreamWaitEvent(st, c->ev_reset, 0));
         c->reset_pending = false;
     }
+    const bool any_sync = c->o.rla_enabled || c->o.t2_enabled;
+    /* the demod kernel slices the data bits unless the DC block (-o) sits between its FIR and the slicer */
+    const bool k1_bits = any_sync && !c->o.remove_dc;
     /* ================= stage 1 (k1s): history prefix of this set, demod ================= */
     if (c->chain_recorded[set]) CUDA_TRY(cudaStreamWaitEvent(sk, c->ev_chain[set], 0));    /* batch i-2 is done with the set */
     if (input_ready) CUDA_TRY(cudaStreamWaitEvent(sk, input_ready, 0));
@@ -1250,6 +1269,9 @@ static int run_batch(wmb_ctx *c, const uint8_t *src, size_t nbytes, cudaEvent_t 
             ChainBuf &b = c->cb[ch];
             TRY(copy_history(b.set[set].dphi, b.set[pset].dphi, 4, c->W, c->prev_M, sk));
             TRY(copy_history(b.set[set].rssi, b.set[pset].rssi, 1, c->W, c->prev_M, sk));
+            /* bit history for the run-length warm-ups: the previous batch's last W samples */
+            if (k1_bits && c->prev_M % 32 == 0)          /* only a final (flush) batch can be ragged */
+                TRY(copy_history(b.set[set].dbits, b.set[pset].dbits, 4, c->W / 32, c->prev_M / 32, sk));
         }
     CUDA_TRY(cudaEventRecord(evt[0], sk));
     if (!c->push_started) { CUDA_TRY(cudaEventRecord(c->ev_push_start, sk)); c->push_started = true; }
@@ -1274,6 +1296,7 @@ static int run_batch(wmb_ctx *c, const uint8_t *src, size_t nbytes, cudaEvent_t 
     for (int ch = 0; ch < WMB_N_CHAINS; ch++) {
         k1.dphi[ch] = c->cb[ch].set[set].dphi ? c->cb[ch].set[set].dphi + c->W : nullptr;
         k1.rssi[ch] = c->cb[ch].set[set].rssi ? c->cb[ch].set[set].rssi + c->W : nullptr;
+        k1.dbits[ch] = k1_bits && c->cb[ch].set[set].dbits ? c->cb[ch].set[set].dbits + c->W / 32 : nullptr;
     }
     TRY(launch_k1(c, k1, sk));
     CUDA_TRY(cudaEventRecord(evt[1], sk));
@@ -1298,13 +1321,112 @@ static int run_batch(wmb_ctx *c, const uint8_t *src, size_t nbytes, cudaEvent_t 
     const uint32_t C = pick_chunk(c, M, alone);
     const uint32_t lanes = (uint32_t)((M + C - 1) / C);
     if (lanes > c->lanes_max) return set_err(WMB_E_INVAL, "internal: %u lanes > %u", lanes, c->lanes_max);
-    const bool any_sync = c->o.rla_enabled || c->o.t2_enabled;
     const int64_t wofs = c->W / 32;                       /* word offset of batch sample 0 */
 
+    /* ---- run-length bit sync: T1/C1 on st0, S1 on st1 ---- */
+    auto enqueue_run_length = [&](cudaStream_t st0, cudaStream_t st1) -> int {
+        const bool two = (c->chains & 1u) && c->two_phase;
+        /* chains that take the monolithic lanes unconditionally: S1 always, T1/C1 when forced (tests) */
+        const uint32_t mono = (c->chains & 2u) | (((c->chains & 1u) && !two) ? 1u : 0u);
+        K2mParams km[WMB_N_CHAINS];
+        auto setup_mono = [&](int ch, const uint32_t *run_if) -> int {
+            ChainBuf &b = c->cb[ch];
+            SetBuf &sb = b.set[set];
+            K2mParams &p = km[ch];
+            memset(&p, 0, sizeof(p));
+            p.dbits = sb.dbits + wofs; p.rssi = sb.rssi + c->W; p.M = M; p.hist = c->hist_m;
+            p.C = C; p.W = c->W_m[ch]; p.lanes = lanes;
+            p.cap = C / 4 + K2_EDGE_EMIT_CAP + 8;
+            if ((uint64_t)lanes * p.cap > c->cap_words_rl) return set_err(WMB_E_INVAL, "internal: event buffers too small for C=%u", C);
+            p.ev = b.s[WMB_ALGO_RLA].ev; p.cnt = b.s[WMB_ALGO_RLA].cnt;
+            p.st_start = b.rl_start; p.st_end = b.rl_end; p.carry = b.rl_carry; p.rerun = b.rerun;
+            p.errors = c->d_errors; p.lane_err = b.lane_err;
+            p.mode = 0; p.run_if = run_if; p.ac_err = c->ac_err[ch];
+            if (!run_if) c->st.lanes_run += lanes;
+            return WMB_OK;
+        };
+        auto compact_mono = [&](int ch, cudaStream_t st, const uint32_t *run_if) -> int {       /* lane events -> ring */
+            ChainBuf &b = c->cb[ch];
+            Stream &s = b.s[WMB_ALGO_RLA];
+            K2cParams q;
+            memset(&q, 0, sizeof(q));
+            q.ev = s.ev; q.cnt = s.cnt; q.base = s.base; q.lanes = lanes; q.cap = km[ch].cap; q.C = C;
+            q.m_base = (int64_t)c->m_consumed;
+            q.ring = s.ring; q.ring_mask = s.ring_cap - 1; q.sd = s.sd; q.cand = s.cand; q.cand_cap = c->cand_cap;
+            q.agg = s.agg; q.rssi = b.set[set].rssi + c->W; q.run_if = run_if;
+            q.lane_err = b.lane_err; q.errors = c->d_errors;
+            return launch_k2c(c, q, st);
+        };
+        for (int ch = 0; ch < WMB_N_CHAINS; ch++) {
+            if (!(mono & (1u << ch))) continue;
+            cudaStream_t st = ch == 0 ? st0 : st1;
+            TRY(setup_mono(ch, nullptr));
+            TRY(launch_k2m(c, ch, km[ch], st));
+            TRY(launch_k2m_carry(c, c->cb[ch].rl_end + (lanes - 1), c->cb[ch].rl_carry, nullptr, st));
+            TRY(compact_mono(ch, st, nullptr));
+        }
+        if (two) {
+            /* T1/C1: phase 1 (per-sample, verified) -> records -> phase 2 (per-run) */
+            ChainBuf &b = c->cb[0];
+            Stream &s = b.s[WMB_ALGO_RLA];
+            K2p1Params p1;
+            memset(&p1, 0, sizeof(p1));
+            p1.dbits = b.set[set].dbits + wofs; p1.M = M; p1.hist = c->hist_m;
+            p1.C = K2P1_CHUNK; p1.W = K2P1_WARM; p1.lanes = (uint32_t)((M + K2P1_CHUNK - 1) / K2P1_CHUNK);
+            p1.cap = K2P1_CAP; p1.rec = b.p1_rec; p1.cnt = b.p1_cnt;
+            p1.st_start = b.p1_start; p1.st_end = b.p1_end; p1.carry = b.rl_carry; p1.rerun = b.p1_rerun;
+            p1.mode = 0;
+            if (p1.lanes > c->p1_lanes_max) return set_err(WMB_E_INVAL, "internal: phase-1 lanes");
+            c->st.lanes_run += p1.lanes;
+            TRY(launch_k2p1(c, p1, st0));
+            K2pcParams pc;
+            memset(&pc, 0, sizeof(pc));
+            pc.rec = b.p1_rec; pc.cnt = b.p1_cnt; pc.base = b.p1_base; pc.lanes = p1.lanes; pc.cap = p1.cap; pc.C = p1.C;
+            pc.rec_m = b.rec_m; pc.rec_v = b.rec_v; pc.agg = s.agg; pc.pd = b.pd;
+            K2p2Params p2;
+            memset(&p2, 0, sizeof(p2));
+            p2.rec_m = b.rec_m; p2.rec_v = b.rec_v; p2.rec_n = b.rec_n; p2.pd = b.pd; p2.R = K2P2_RECORDS;
+            p2.lanes = (uint32_t)(((uint64_t)M / 5 + 2 * (uint64_t)p1.lanes) / K2P2_RECORDS + 2);
+            if (p2.lanes > c->p2_lanes_max) return set_err(WMB_E_INVAL, "internal: phase-2 lanes");
+            p2.cnt = b.p2_cnt; p2.base = b.p2_base; p2.rssi = b.set[set].rssi + c->W; p2.m_base = (int64_t)c->m_consumed;
+            p2.ring = s.ring; p2.ring_mask = s.ring_cap - 1; p2.sd = s.sd; p2.cand = s.cand; p2.cand_cap = c->cand_cap;
+            p2.carry = b.rl_carry; p2.p2_out = b.p2_out; p2.agg = s.agg; p2.ac_err = c->ac_err[0];
+            TRY(launch_k2p_rest(c, pc, p2, st0));
+            /* the second reset rule (rtl_wmbus.c:756-762) fired somewhere in this batch (pd->fallback, set by phase
+             * 2, which then wrote nothing): redo T1/C1 with the exact monolithic lanes.  The kernels are always
+             * enqueued; without the flag every thread returns at once. */
+            const uint32_t *flag = &b.pd->fallback;
+            TRY(setup_mono(0, flag));
+            TRY(launch_k2m(c, 0, km[0], st0));
+            TRY(compact_mono(0, st0, flag));
+            TRY(launch_k2p_fold(c, b.p1_end + (p1.lanes - 1), b.p2_out, b.rl_carry, b.pd, b.rl_end + (lanes - 1), st0));
+        }
+        return WMB_OK;
+    };
+
     if (any_sync) {
+        const bool coop = c->o.t2_enabled && !c->o.remove_dc && M % 32 == 0;
+        /* The run-length path reads only the data bits and the rssi, both from the demod kernel here: it starts right
+         * behind that kernel, T1/C1 on rs and S1 on s2, and runs beside the clock lanes (one warp per scheduler,
+         * mostly idle SMs), instead of after their verification.  Both streams also wait for what cs held before this
+         * batch -- the previous gather reads the rings and candidate lists these kernels append to, wmb_reset's
+         * kernel sets their carries -- and cs waits for them before the gather (ev_chain[set] thus covers them too).
+         * -o (the clock lanes slice), a ragged final batch and a batch without time2 keep the order below. */
+        const bool early = coop && c->o.rla_enabled;
+        if (early) {
+            CUDA_TRY(cudaEventRecord(c->ev_fork2, c->cs));
+            for (cudaStream_t st : { c->rs, c->s2 }) {
+                CUDA_TRY(cudaStreamWaitEvent(st, c->ev_fork2, 0));
+                CUDA_TRY(cudaStreamWaitEvent(st, c->ev_k1[set], 0));
+            }
+            TRY(enqueue_run_length(c->rs, c->s2));
+            CUDA_TRY(cudaEventRecord(c->ev_join_rs, c->rs));
+            CUDA_TRY(cudaEventRecord(c->ev_join2, c->s2));
+            tr("p1+p2");
+        }
+
         /* ================= stage 2 (as[set]): clock-recovery lanes, every lane speculative ================= */
         K2aParams ka[WMB_N_CHAINS];
-        const bool coop = c->o.t2_enabled && !c->o.remove_dc && M % 32 == 0;
         const uint32_t Ca = coop ? pick_chunk_coop(c, M) : C;
         const uint32_t lanes_a = (uint32_t)((M + Ca - 1) / Ca);
         /* the two chains' lanes side by side when three threads share a lane: one such warp leaves its scheduler half
@@ -1346,27 +1468,16 @@ static int run_batch(wmb_ctx *c, const uint8_t *src, size_t nbytes, cudaEvent_t 
             ChainBuf &b = c->cb[ch];
             TRY(launch_k2a_verify(c, ch, ka[ch]));
             CUDA_TRY(cudaMemcpyAsync(b.ia_carry, b.set[set].ia_end + (ka[ch].lanes - 1), sizeof(IirState), cudaMemcpyDeviceToDevice, c->cs));
-            /* bit history for the run-length warm-ups: the previous batch's last W samples (exact since its fix-up) */
+            /* the bit history of the run-length warm-ups: the previous batch's last W samples (exact since its fix-up);
+             * without -o the demod stream copied the data bits */
             if (!first && c->prev_M % 32 == 0) {         /* only a final (flush) batch can be ragged */
-                TRY(copy_history(b.set[set].dbits, b.set[pset].dbits, 4, c->W / 32, c->prev_M / 32, c->cs));
+                if (!k1_bits) TRY(copy_history(b.set[set].dbits, b.set[pset].dbits, 4, c->W / 32, c->prev_M / 32, c->cs));
                 TRY(copy_history(b.set[set].sbits, b.set[pset].sbits, 4, c->W / 32, c->prev_M / 32, c->cs));
             }
         }
 
-        /* chain 1's run-length lanes run on their own stream (forked after whatever cs holds, joined at the end) */
-        auto fork2 = [&]() -> int {
-            CUDA_TRY(cudaEventRecord(c->ev_fork2, c->cs));
-            CUDA_TRY(cudaStreamWaitEvent(c->s2, c->ev_fork2, 0));
-            return WMB_OK;
-        };
-        auto join2 = [&]() -> int {
-            CUDA_TRY(cudaEventRecord(c->ev_join2, c->s2));
-            CUDA_TRY(cudaStreamWaitEvent(c->cs, c->ev_join2, 0));
-            return WMB_OK;
-        };
-
         /* ---- K2t: time2 bit streams straight into the rings (own stream: independent of the
-         *      run-length kernels below, and both leave most of the GPU idle on their own) ---- */
+         *      run-length kernels, and both leave most of the GPU idle on their own) ---- */
         if (c->o.t2_enabled) {
             CUDA_TRY(cudaEventRecord(c->ev_fork, c->cs));
             CUDA_TRY(cudaStreamWaitEvent(c->ts, c->ev_fork, 0));
@@ -1392,88 +1503,22 @@ static int run_batch(wmb_ctx *c, const uint8_t *src, size_t nbytes, cudaEvent_t 
             CUDA_TRY(cudaEventRecord(c->ev_join, c->ts));
         }
 
-        /* ---- run-length bit sync ---- */
-        if (c->o.rla_enabled) {
-            const bool two = (c->chains & 1u) && c->two_phase;
-            /* chains that take the monolithic lanes unconditionally: S1 always, T1/C1 when forced (tests) */
-            const uint32_t mono = (c->chains & 2u) | (((c->chains & 1u) && !two) ? 1u : 0u);
-            K2mParams km[WMB_N_CHAINS];
-            auto setup_mono = [&](int ch, const uint32_t *run_if) -> int {
-                ChainBuf &b = c->cb[ch];
-                SetBuf &sb = b.set[set];
-                K2mParams &p = km[ch];
-                memset(&p, 0, sizeof(p));
-                p.dbits = sb.dbits + wofs; p.rssi = sb.rssi + c->W; p.M = M; p.hist = c->hist_m;
-                p.C = C; p.W = c->W_m[ch]; p.lanes = lanes;
-                p.cap = C / 4 + K2_EDGE_EMIT_CAP + 8;
-                if ((uint64_t)lanes * p.cap > c->cap_words_rl) return set_err(WMB_E_INVAL, "internal: event buffers too small for C=%u", C);
-                p.ev = b.s[WMB_ALGO_RLA].ev; p.cnt = b.s[WMB_ALGO_RLA].cnt;
-                p.st_start = b.rl_start; p.st_end = b.rl_end; p.carry = b.rl_carry; p.rerun = b.rerun;
-                p.errors = c->d_errors; p.lane_err = b.lane_err;
-                p.mode = 0; p.run_if = run_if; p.ac_err = c->ac_err[ch];
-                if (!run_if) c->st.lanes_run += lanes;
-                return WMB_OK;
-            };
-            auto compact_mono = [&](int ch, cudaStream_t st, const uint32_t *run_if) -> int {       /* lane events -> ring */
-                ChainBuf &b = c->cb[ch];
-                Stream &s = b.s[WMB_ALGO_RLA];
-                K2cParams q;
-                memset(&q, 0, sizeof(q));
-                q.ev = s.ev; q.cnt = s.cnt; q.base = s.base; q.lanes = lanes; q.cap = km[ch].cap; q.C = C;
-                q.m_base = (int64_t)c->m_consumed;
-                q.ring = s.ring; q.ring_mask = s.ring_cap - 1; q.sd = s.sd; q.cand = s.cand; q.cand_cap = c->cand_cap;
-                q.agg = s.agg; q.rssi = b.set[set].rssi + c->W; q.run_if = run_if;
-                q.lane_err = b.lane_err; q.errors = c->d_errors;
-                return launch_k2c(c, q, st);
-            };
-            /* S1 (and a forced T1/C1) beside the two-phase path of T1/C1 */
-            const bool s1_beside = two && (mono & 2u);
-            if (s1_beside) TRY(fork2());
-            for (int ch = 0; ch < WMB_N_CHAINS; ch++) {
-                if (!(mono & (1u << ch))) continue;
-                cudaStream_t st = (s1_beside && ch == 1) ? c->s2 : c->cs;
-                TRY(setup_mono(ch, nullptr));
-                TRY(launch_k2m(c, ch, km[ch], st));
-                TRY(launch_k2m_carry(c, c->cb[ch].rl_end + (lanes - 1), c->cb[ch].rl_carry, nullptr, st));
-                TRY(compact_mono(ch, st, nullptr));
+        if (early) {
+            CUDA_TRY(cudaStreamWaitEvent(c->cs, c->ev_join_rs, 0));
+            CUDA_TRY(cudaStreamWaitEvent(c->cs, c->ev_join2, 0));
+        } else if (c->o.rla_enabled) {
+            /* on cs, behind the verification; S1 beside the two-phase path of T1/C1 on s2 (forked after whatever cs
+             * holds, joined at the end) */
+            const bool s1_beside = (c->chains & 1u) && c->two_phase && (c->chains & 2u);
+            if (s1_beside) {
+                CUDA_TRY(cudaEventRecord(c->ev_fork2, c->cs));
+                CUDA_TRY(cudaStreamWaitEvent(c->s2, c->ev_fork2, 0));
             }
-            if (two) {
-                /* T1/C1: phase 1 (per-sample, verified) -> records -> phase 2 (per-run) */
-                ChainBuf &b = c->cb[0];
-                Stream &s = b.s[WMB_ALGO_RLA];
-                K2p1Params p1;
-                memset(&p1, 0, sizeof(p1));
-                p1.dbits = b.set[set].dbits + wofs; p1.M = M; p1.hist = c->hist_m;
-                p1.C = K2P1_CHUNK; p1.W = K2P1_WARM; p1.lanes = (uint32_t)((M + K2P1_CHUNK - 1) / K2P1_CHUNK);
-                p1.cap = K2P1_CAP; p1.rec = b.p1_rec; p1.cnt = b.p1_cnt;
-                p1.st_start = b.p1_start; p1.st_end = b.p1_end; p1.carry = b.rl_carry; p1.rerun = b.p1_rerun;
-                p1.mode = 0;
-                if (p1.lanes > c->p1_lanes_max) return set_err(WMB_E_INVAL, "internal: phase-1 lanes");
-                c->st.lanes_run += p1.lanes;
-                TRY(launch_k2p1(c, p1));
-                K2pcParams pc;
-                memset(&pc, 0, sizeof(pc));
-                pc.rec = b.p1_rec; pc.cnt = b.p1_cnt; pc.base = b.p1_base; pc.lanes = p1.lanes; pc.cap = p1.cap; pc.C = p1.C;
-                pc.rec_m = b.rec_m; pc.rec_v = b.rec_v; pc.agg = s.agg; pc.pd = b.pd;
-                K2p2Params p2;
-                memset(&p2, 0, sizeof(p2));
-                p2.rec_m = b.rec_m; p2.rec_v = b.rec_v; p2.rec_n = b.rec_n; p2.pd = b.pd; p2.R = K2P2_RECORDS;
-                p2.lanes = (uint32_t)(((uint64_t)M / 5 + 2 * (uint64_t)p1.lanes) / K2P2_RECORDS + 2);
-                if (p2.lanes > c->p2_lanes_max) return set_err(WMB_E_INVAL, "internal: phase-2 lanes");
-                p2.cnt = b.p2_cnt; p2.base = b.p2_base; p2.rssi = b.set[set].rssi + c->W; p2.m_base = (int64_t)c->m_consumed;
-                p2.ring = s.ring; p2.ring_mask = s.ring_cap - 1; p2.sd = s.sd; p2.cand = s.cand; p2.cand_cap = c->cand_cap;
-                p2.carry = b.rl_carry; p2.p2_out = b.p2_out; p2.agg = s.agg; p2.ac_err = c->ac_err[0];
-                TRY(launch_k2p_rest(c, pc, p2));
-                /* the second reset rule (rtl_wmbus.c:756-762) fired somewhere in this batch (pd->fallback, set by phase
-                 * 2, which then wrote nothing): redo T1/C1 with the exact monolithic lanes.  The kernels are always
-                 * enqueued; without the flag every thread returns at once. */
-                const uint32_t *flag = &b.pd->fallback;
-                TRY(setup_mono(0, flag));
-                TRY(launch_k2m(c, 0, km[0], c->cs));
-                TRY(compact_mono(0, c->cs, flag));
-                TRY(launch_k2p_fold(c, b.p1_end + (p1.lanes - 1), b.p2_out, b.rl_carry, b.pd, b.rl_end + (lanes - 1)));
+            TRY(enqueue_run_length(c->cs, s1_beside ? c->s2 : c->cs));
+            if (s1_beside) {
+                CUDA_TRY(cudaEventRecord(c->ev_join2, c->s2));
+                CUDA_TRY(cudaStreamWaitEvent(c->cs, c->ev_join2, 0));
             }
-            if (s1_beside) TRY(join2());
             tr("k2t+p1+p2");
         }
         if (c->o.t2_enabled) CUDA_TRY(cudaStreamWaitEvent(c->cs, c->ev_join, 0));
@@ -2282,7 +2327,7 @@ extern "C" int wmb_reset(wmb_ctx *c)
     if (!c) return set_err(WMB_E_INVAL, "null argument");
     CUDA_TRY(cudaSetDevice(c->device));
     /* whatever was enqueued is abandoned: let it finish (a completed push has left the streams idle) */
-    for (cudaStream_t st : { c->cs, c->xs, c->k1s, c->as[0], c->as[1], c->as2[0], c->as2[1], c->ts, c->s2 })
+    for (cudaStream_t st : { c->cs, c->xs, c->k1s, c->as[0], c->as[1], c->as2[0], c->as2[1], c->ts, c->s2, c->rs })
         if (st && cudaStreamQuery(st) != cudaSuccess) CUDA_TRY(cudaStreamSynchronize(st));
     c->iq_consumed = 0; c->m_consumed = 0; c->hist_m = 0; c->hist_iq = 0;
     c->remainder.clear(); c->lines.clear(); c->held.clear(); c->held_prev.clear();
