@@ -10,9 +10,9 @@
  *                      Speculative warm-up + state verification (rtl_wmbus.c:497-515,
  *                      :1059, :1089-1111; iir.h:59-74).
  *   K2t  k2t_*         time2 bit stream: strobed data bits -> shift register -> access
- *                      code.  Exact without speculation: each lane reports its strobe
- *                      count and its last 24 strobed bits, a scan folds them into every
- *                      lane's start register (rtl_wmbus.c:806-852).
+ *                      code.  Exact without speculation: each tile of words reports its
+ *                      strobe count and its last 24 strobed bits, a scan folds them into
+ *                      every tile's start register (rtl_wmbus.c:806-852).
  *   K2m  k2m_lane      run-length bit sync, integer-only lanes reading dbits
  *                      (rtl_wmbus.c:617-803).  Speculative warm-up + verification.
  */
@@ -477,18 +477,43 @@ struct StreamDev {                  /* device-resident bookkeeping of one (chain
     uint32_t pad;
 };
 
+/* ---- geometry of the time2 pass ---------------------------------------------------------------
+ * Five kernels per chain: k2t_count (one block per tile of T2_TILE_WORDS words: strobe count and last strobed bits of
+ * the tile), the three-kernel scan t2scan_a/b/c over the tiles (their start ordinals and shift registers; the tiles
+ * are its "lanes") and k2t_write (one block per tile again: the events into the ring).  In a tile, thread t loads
+ * words 4t..4t+3 with 128-bit loads; for the events, "warp" w (T2_WARP consecutive threads) owns the tile's words
+ * [w * T2_WARP * T2_WPT, +T2_WARP * T2_WPT) and handles them in T2_WPT rounds of T2_WARP consecutive words, lane l
+ * taking the round's word l, so that a round's events are consecutive ordinals.  The CPU build uses tiny tiles and
+ * "warps" so that its tests cross every boundary. */
+#ifdef WMB_HOSTSIM
+#define T2_THREADS 8
+#define T2_WARP 4
+#else
+#define T2_THREADS 256
+#define T2_WARP 32
+#endif
+#define T2_WPT 4                                /* words per thread (one 128-bit load each of sbits and dbits)     */
+#define T2_TILE_WORDS (T2_THREADS * T2_WPT)
+#define T2_WARPS (T2_THREADS / T2_WARP)
+/* Staging holds one round of a warp, sized for the densest strobes the lock stencil allows: a strobe at m needs the
+ * clock low at m-L-1 and high at m-L..m (lock_strobes), so strobes are at least L+2 >= 3 samples apart and a 32-sample
+ * word holds at most 11 of them for every threshold 1..WMB_LOCK_MAX. */
+#define T2_MIN_GAP 3
+#define T2_MAX_PER_WORD 11
+static_assert(T2_MAX_PER_WORD >= (32 + T2_MIN_GAP - 1) / T2_MIN_GAP, "time2 staging smaller than a dense round");
+#define T2_STAGE (T2_WARP * T2_MAX_PER_WORD)
+
 struct K2tParams {
-    const uint32_t *dbits, *sbits;
+    const uint32_t *dbits, *sbits;  /* 16-byte aligned                                      */
     const uint8_t *rssi;            /* index 0 = batch sample 0                             */
     int64_t  M;
-    uint32_t Cw;                    /* words per lane                                       */
-    uint32_t lanes;
-    uint32_t *cnt;                  /* [lanes] strobes per lane                             */
+    uint32_t lanes;                 /* tiles of T2_TILE_WORDS words, one block each         */
+    uint32_t *cnt;                  /* [lanes] strobes per tile                             */
     uint32_t *tail;                 /* [lanes] last <=24 strobed bits, chronological        */
     uint32_t *tail_len;             /* [lanes]                                              */
-    uint64_t *base;                 /* [lanes] ordinal of each lane's first event           */
-    uint32_t *sr_start;             /* [lanes] shift register at the lane's first sample    */
-    uint64_t *agg_cnt; uint32_t *agg_tail, *agg_len;   /* [SCAN_THREADS] scan scratch          */
+    uint64_t *base;                 /* [lanes] ordinal of each tile's first event           */
+    uint32_t *sr_start;             /* [lanes] shift register at the tile's first sample    */
+    uint64_t *agg_cnt; uint32_t *agg_tail, *agg_len;   /* [scan tiles] scan scratch             */
     int64_t  m_base;
     uint64_t *ring; uint64_t ring_mask;
     StreamDev *sd;
@@ -497,31 +522,15 @@ struct K2tParams {
 };
 
 WMB_HD uint32_t k2t_words(const K2tParams &p) { return (uint32_t)((p.M + 31) >> 5); }
+WMB_HD uint32_t k2t_tiles(int64_t M) { return (uint32_t)(((M + 31) >> 5) + T2_TILE_WORDS - 1) / T2_TILE_WORDS; }
 
-/* pass 1: per lane, strobe count and the last strobed bits */
-template <class CH>
-WMB_D void k2t_count(const K2tParams &p, uint32_t lane)
-{
-    if (lane >= p.lanes) return;
-    const uint32_t nw = k2t_words(p);
-    const uint32_t w0 = lane * p.Cw, w1 = (w0 + p.Cw < nw) ? w0 + p.Cw : nw;
-    const int NB = (CH::ID == 0) ? 16 : 24;
-    uint32_t cnt = 0;
-    for (uint32_t w = w0; w < w1; w++) cnt += (uint32_t)wmb_popc(p.sbits[w]);
-    uint32_t tail = 0; int len = 0;
-    for (uint32_t w = w1; w > w0 && len < NB;) {
-        w--;
-        uint32_t s = p.sbits[w];
-        const uint32_t d = p.dbits[w];
-        while (s && len < NB) {
-            const int i = 31 - wmb_clz(s);
-            s &= ~(1u << i);
-            tail |= ((d >> i) & 1u) << len;
-            len++;
-        }
-    }
-    p.cnt[lane] = cnt; p.tail[lane] = tail; p.tail_len[lane] = (uint32_t)len;
-}
+/* per tile: the strobe and data words of every tile word, and each word's first ordinal (relative to the tile's) and
+ * shift register; the staged events of every warp's current round */
+struct K2tSmem {
+    uint32_t s[T2_TILE_WORDS], d[T2_TILE_WORDS];
+    uint32_t ord[T2_TILE_WORDS], sr[T2_TILE_WORDS];
+    uint64_t stage[T2_WARPS][T2_STAGE];
+};
 
 /* ---- device-wide exclusive scans over lanes -------------------------------------------------
  * Three small kernels: (A) every block of SCAN_BLOCK threads reduces a tile of SCAN_TILE lanes
@@ -663,60 +672,126 @@ WMB_D void t2scan_c_write(const K2tParams &p, uint32_t tile, uint32_t tid, const
     }
 }
 
-/* pass 2: write the events straight into the stream ring.  Four words (128 samples) at a time:
- * their strobe/data words and the 128 rssi bytes they may need are requested together. */
+
 template <class CH>
-WMB_D void k2t_write(const K2tParams &p, uint32_t lane)
+WMB_D T2Fold t2_fold(T2Fold a, const T2Fold &b) { t2_append<CH>(a, b.cnt, b.tail, b.len); return a; }
+
+/* one word: its strobed data bits, oldest first (the newest in bit 0) */
+template <class CH>
+WMB_D T2Fold t2_word(uint32_t s, uint32_t d)
 {
-    if (lane >= p.lanes) return;
-    const uint32_t nw = k2t_words(p);
-    const uint32_t w0 = lane * p.Cw, w1 = (w0 + p.Cw < nw) ? w0 + p.Cw : nw;
-    uint32_t sr = p.sr_start[lane];
-    uint64_t ord = p.base[lane];
-    for (uint32_t wb = w0; wb < w1; wb += 4) {
-        uint32_t s4[4], d4[4];
-        u32x4 rs[8];
-        if (wb + 4 <= w1) {
-            const u32x4 sv = *(const u32x4 *)(p.sbits + wb), dv = *(const u32x4 *)(p.dbits + wb);
-            s4[0] = sv.x; s4[1] = sv.y; s4[2] = sv.z; s4[3] = sv.w;
-            d4[0] = dv.x; d4[1] = dv.y; d4[2] = dv.z; d4[3] = dv.w;
-        } else {
-#pragma unroll
-            for (int q = 0; q < 4; q++) { s4[q] = (wb + q < w1) ? p.sbits[wb + q] : 0u; d4[q] = (wb + q < w1) ? p.dbits[wb + q] : 0u; }
-        }
-        if ((s4[0] | s4[1] | s4[2] | s4[3]) == 0u) continue;
-        const u32x4 *r4 = (const u32x4 *)(p.rssi + (int64_t)wb * 32);   /* 32-byte aligned; slack behind M */
-#pragma unroll
-        for (int q = 0; q < 8; q++) rs[q] = r4[q];
-#pragma unroll
-        for (int q = 0; q < 4; q++) {
-            uint32_t s = s4[q];
-            const uint32_t d = d4[q];
-            while (s) {
-                const int i = wmb_ffs(s) - 1;
-                s &= s - 1;
-                const uint32_t bit = (d >> i) & 1u;
-                sr = ((sr << 1) | bit) & CH::CODE_MASK;              /* rtl_wmbus.c:820 */
-                const uint32_t sync = ac_match<CH>(sr, p.ac_err);    /* rtl_wmbus.c:822 */
-                const int64_t m = (int64_t)(wb + q) * 32 + i;
-                const u32x4 rq = rs[2 * q + (i >> 4)];
-                const uint32_t rw = ((i >> 2) & 3) == 0 ? rq.x : ((i >> 2) & 3) == 1 ? rq.y : ((i >> 2) & 3) == 2 ? rq.z : rq.w;
-                const uint32_t rssi = (rw >> (8 * (i & 3))) & 0xFFu;
-                const uint64_t g = ((uint64_t)(p.m_base + m) << 24) | ((uint64_t)rssi << 16) | (sync << 1) | bit;
-                p.ring[ord & p.ring_mask] = g;
-                if (sync) {
-#ifdef WMB_HOSTSIM
-                    const uint32_t slot = p.sd->n_cand++;
-#else
-                    const uint32_t slot = atomicAdd(&p.sd->n_cand, 1u);
-#endif
-                    if (slot < p.cand_cap) p.cand[slot] = ord;
-                    else p.sd->cand_overflow = 1;
-                }
-                ord++;
-            }
-        }
+    constexpr uint32_t NB = (CH::ID == 0) ? 16 : 24;
+    T2Fold f = { (uint64_t)wmb_popc(s), 0u, 0u };
+    while (s) {
+        const int i = wmb_ffs(s) - 1;
+        s &= s - 1;
+        f.tail = (f.tail << 1) | ((d >> i) & 1u);
     }
+    f.tail &= CH::CODE_MASK;
+    f.len = f.cnt > NB ? NB : (uint32_t)f.cnt;
+    return f;
+}
+
+/* k2t_count / k2t_write, phase 1: thread `tid` loads its four words of the tile (zero past the batch), keeps them in
+ * `sm` when given, and returns their fold */
+template <class CH>
+WMB_D T2Fold k2t_load(const K2tParams &p, uint32_t tile, uint32_t tid, K2tSmem *sm)
+{
+    const uint32_t nw = k2t_words(p), w = tile * T2_TILE_WORDS + tid * T2_WPT;
+    uint32_t s4[T2_WPT], d4[T2_WPT];
+    if (w + T2_WPT <= nw) {
+        const u32x4 sv = *(const u32x4 *)(p.sbits + w), dv = *(const u32x4 *)(p.dbits + w);
+        s4[0] = sv.x; s4[1] = sv.y; s4[2] = sv.z; s4[3] = sv.w;
+        d4[0] = dv.x; d4[1] = dv.y; d4[2] = dv.z; d4[3] = dv.w;
+    } else {
+#pragma unroll
+        for (int q = 0; q < T2_WPT; q++) { s4[q] = (w + q < nw) ? p.sbits[w + q] : 0u; d4[q] = (w + q < nw) ? p.dbits[w + q] : 0u; }
+    }
+    T2Fold f = { 0, 0, 0 };
+#pragma unroll
+    for (int q = 0; q < T2_WPT; q++) {
+        f = t2_fold<CH>(f, t2_word<CH>(s4[q], d4[q]));
+        if (sm) { sm->s[tid * T2_WPT + q] = s4[q]; sm->d[tid * T2_WPT + q] = d4[q]; }
+    }
+    return f;
+}
+
+/* k2t_count, last phase: the tile's aggregate (the scan's inclusive total from the identity) */
+WMB_D void k2t_count_store(const K2tParams &p, uint32_t tile, const T2Fold &total)
+{
+    p.cnt[tile] = (uint32_t)total.cnt; p.tail[tile] = total.tail; p.tail_len[tile] = total.len;
+}
+
+/* k2t_write: the carry into the tile's scan -- ordinals relative to the tile's first event, and its start register */
+template <class CH>
+WMB_D T2Fold k2t_carry(const K2tParams &p, uint32_t tile)
+{
+    constexpr uint32_t NB = (CH::ID == 0) ? 16 : 24;
+    const T2Fold c = { 0, p.sr_start[tile], NB };
+    return c;
+}
+/* k2t_write, after the scan: thread `tid` spreads its exclusive prefix over its four words */
+template <class CH>
+WMB_D void k2t_spread(uint32_t tid, T2Fold acc, K2tSmem &sm)
+{
+#pragma unroll
+    for (int q = 0; q < T2_WPT; q++) {
+        const uint32_t w = tid * T2_WPT + q;
+        sm.ord[w] = (uint32_t)acc.cnt; sm.sr[w] = acc.tail;
+        acc = t2_fold<CH>(acc, t2_word<CH>(sm.s[w], sm.d[w]));
+    }
+}
+
+/* k2t_write, round r: lane l of warp w produces the events of the round's word l into the warp's staging (at their
+ * ordinal's offset from the round's first), and appends its access-code matches to the candidate list */
+WMB_HD uint32_t k2t_round_word(uint32_t tid, uint32_t r)
+{
+    return (tid / T2_WARP) * (T2_WARP * T2_WPT) + r * T2_WARP + tid % T2_WARP;
+}
+template <class CH>
+WMB_D void k2t_emit(const K2tParams &p, uint32_t tile, uint32_t tid, uint32_t r, K2tSmem &sm)
+{
+    const uint32_t w = k2t_round_word(tid, r);
+    uint32_t s = sm.s[w];
+    if (!s) return;
+    const uint32_t d = sm.d[w];
+    uint64_t *stage = sm.stage[tid / T2_WARP] + (sm.ord[w] - sm.ord[k2t_round_word(tid - tid % T2_WARP, r)]);
+    uint64_t ord = p.base[tile] + sm.ord[w];
+    uint32_t sr = sm.sr[w];
+    const int64_t word = (int64_t)tile * T2_TILE_WORDS + w;
+    const u32x4 *r4 = (const u32x4 *)(p.rssi + word * 32);           /* 32-byte aligned */
+    const u32x4 rs[2] = { r4[0], r4[1] };
+    while (s) {
+        const int i = wmb_ffs(s) - 1;
+        s &= s - 1;
+        const uint32_t bit = (d >> i) & 1u;
+        sr = ((sr << 1) | bit) & CH::CODE_MASK;                      /* rtl_wmbus.c:820 */
+        const uint32_t sync = ac_match<CH>(sr, p.ac_err);            /* rtl_wmbus.c:822 */
+        const u32x4 rq = rs[i >> 4];
+        const uint32_t rw = ((i >> 2) & 3) == 0 ? rq.x : ((i >> 2) & 3) == 1 ? rq.y : ((i >> 2) & 3) == 2 ? rq.z : rq.w;
+        const uint32_t rssi = (rw >> (8 * (i & 3))) & 0xFFu;
+        *stage++ = ((uint64_t)(p.m_base + word * 32 + i) << 24) | ((uint64_t)rssi << 16) | (sync << 1) | bit;
+        if (sync) {
+#ifdef WMB_HOSTSIM
+            const uint32_t slot = p.sd->n_cand++;
+#else
+            const uint32_t slot = atomicAdd(&p.sd->n_cand, 1u);
+#endif
+            if (slot < p.cand_cap) p.cand[slot] = ord;
+            else p.sd->cand_overflow = 1;
+        }
+        ord++;
+    }
+}
+/* k2t_write, round r after the warp's emits: its lanes copy the staged events to the ring in ordinal order, so that a
+ * warp's stores cover consecutive slots (split only where the ring wraps) */
+WMB_D void k2t_flush(const K2tParams &p, uint32_t tile, uint32_t tid, uint32_t r, const K2tSmem &sm)
+{
+    const uint32_t l = tid % T2_WARP, first = k2t_round_word(tid - l, r), last = first + T2_WARP - 1;
+    const uint32_t n = sm.ord[last] + (uint32_t)wmb_popc(sm.s[last]) - sm.ord[first];
+    const uint64_t ord0 = p.base[tile] + sm.ord[first];
+    const uint64_t *stage = sm.stage[tid / T2_WARP];
+    for (uint32_t i = l; i < n; i += T2_WARP) p.ring[(ord0 + i) & p.ring_mask] = stage[i];
 }
 
 /* ------------------------------------------------------------------------------------- */

@@ -69,8 +69,8 @@ static int set_err(int code, const char *fmt, ...)
 
 struct Stream {                     /* one (chain, algo) bit stream */
     uint32_t *ev = nullptr;         /* run-length: lane-local events              */
-    uint32_t *cnt = nullptr;        /* per-lane counts                            */
-    uint64_t *base = nullptr;       /* per-lane ordinal base                      */
+    uint32_t *cnt = nullptr;        /* per-lane (time2: per-tile) counts          */
+    uint64_t *base = nullptr;       /* per-lane (time2: per-tile) ordinal base    */
     uint64_t *ring = nullptr;       /* global event ring                          */
     uint64_t ring_cap = 0;          /* power of two                               */
     StreamDev *sd = nullptr;        /* device bookkeeping                         */
@@ -108,7 +108,7 @@ struct ChainBuf {
     uint32_t *rec_m = nullptr, *rec_v = nullptr; uint16_t *rec_n = nullptr;
     uint32_t *p2_cnt = nullptr; uint64_t *p2_base = nullptr;
     K2pDev *pd = nullptr; RlState *p2_out = nullptr;
-    /* time2 lanes */
+    /* time2 tiles */
     uint32_t *t2_tail = nullptr, *t2_len = nullptr, *t2_sr = nullptr, *t2_agg_tail = nullptr, *t2_agg_len = nullptr;
     Stream s[WMB_N_ALGOS];
 };
@@ -165,7 +165,7 @@ struct wmb_ctx {
     uint32_t W_m[WMB_N_CHAINS] = {32768, 8192};    /* warm-up of the run-length lanes  */
     uint32_t C_fixed = 0;
     uint32_t lanes_max = 0;
-    uint32_t t2_lanes_max = 0;
+    uint32_t t2_tiles_max = 0;
     uint32_t p1_lanes_max = 0, p2_lanes_max = 0;
     size_t rec_max = 0;
     bool two_phase = true;
@@ -437,19 +437,19 @@ static int launch_k2m_carry(wmb_ctx *c, const RlState *end, RlState *carry, cons
 
 static int launch_k2t(wmb_ctx *c, int chain, const K2tParams &p)
 {
-    const unsigned grid = (p.lanes + 127) / 128, tiles = scan_tiles(p.lanes);
+    const unsigned tiles = scan_tiles(p.lanes);
     if (chain == 0) {
-        k2t_count_kernel<ChainT1C1><<<grid, 128, 0, c->ts>>>(p);
+        k2t_count_kernel<ChainT1C1><<<p.lanes, T2_THREADS, 0, c->ts>>>(p);
         t2scan_a_kernel<ChainT1C1><<<tiles, SCAN_BLOCK, 0, c->ts>>>(p);
         t2scan_b_kernel<ChainT1C1><<<1, 32, 0, c->ts>>>(p);
         t2scan_c_kernel<ChainT1C1><<<tiles, SCAN_BLOCK, 0, c->ts>>>(p);
-        k2t_write_kernel<ChainT1C1><<<grid, 128, 0, c->ts>>>(p);
+        k2t_write_kernel<ChainT1C1><<<p.lanes, T2_THREADS, 0, c->ts>>>(p);
     } else {
-        k2t_count_kernel<ChainS1><<<grid, 128, 0, c->ts>>>(p);
+        k2t_count_kernel<ChainS1><<<p.lanes, T2_THREADS, 0, c->ts>>>(p);
         t2scan_a_kernel<ChainS1><<<tiles, SCAN_BLOCK, 0, c->ts>>>(p);
         t2scan_b_kernel<ChainS1><<<1, 32, 0, c->ts>>>(p);
         t2scan_c_kernel<ChainS1><<<tiles, SCAN_BLOCK, 0, c->ts>>>(p);
-        k2t_write_kernel<ChainS1><<<grid, 128, 0, c->ts>>>(p);
+        k2t_write_kernel<ChainS1><<<p.lanes, T2_THREADS, 0, c->ts>>>(p);
     }
     CUDA_TRY(cudaGetLastError());
     c->st.kernel_launches += 5;
@@ -663,11 +663,9 @@ static int host_alloc(wmb_ctx *c, T **p, size_t count)
 
 #define TRY(expr) do { int _rc = (expr); if (_rc) return _rc; } while (0)
 
-/* lane geometry of the bit-sync kernels; WMBUS_B200_TUNE="t2words:p1chunk:p2records" overrides it for experiments */
-static uint32_t g_t2_words = 128u;       /* time2 lane = 32 * this many decimated samples */
+/* lane geometry of the run-length kernels; WMBUS_B200_TUNE="t2words:p1chunk:p2records" overrides it for experiments */
 static uint32_t g_p1_chunk = 2048u;      /* decimated samples per phase-1 run-length lane */
 static uint32_t g_p2_records = 512u;     /* records per phase-2 lane (nominal) */
-#define K2T_WORDS_PER_LANE g_t2_words
 #define K2P1_CHUNK g_p1_chunk
 #define K2P1_WARM  256u
 #define K2P1_CAP   (K2P1_CHUNK / 5 + 2)
@@ -704,10 +702,11 @@ static void read_tuning()
 #endif
     if (const char *b = getenv("WMBUS_B200_PIPE_MIB")) { const unsigned long v = strtoul(b, nullptr, 10); if (v >= 1 && v <= 4096) g_pipe_bytes = (size_t)v << 20; }
     if (const char *b = getenv("WMBUS_B200_P2BLK")) { const unsigned v = (unsigned)atoi(b); if (v == 32 || v == 64 || v == 128) g_p2_block = v; }
+    /* the first field (formerly the time2 lane length) is parsed and ignored: the time2 kernels work on fixed tiles
+     * (T2_TILE_WORDS), and tools/tune_sweep*.py keep the three-field format */
     const char *e = getenv("WMBUS_B200_TUNE");
     unsigned a = 0, b = 0, r = 0;
     if (!e || sscanf(e, "%u:%u:%u", &a, &b, &r) != 3) return;
-    if (a >= 4 && a <= 4096 && a % 4 == 0) g_t2_words = a;
     if (b >= 512 && b <= 65536 && b % 32 == 0) g_p1_chunk = b;
     if (r >= 32 && r <= K2P2W_THREADS * K2P2W_ITEMS) g_p2_records = r;
 }
@@ -719,7 +718,7 @@ static int ctx_alloc(wmb_ctx *c)
     c->M_max = (int64_t)(c->max_batch_bytes / (2 * (size_t)d));
     const uint32_t C_min = c->C_fixed ? c->C_fixed : 8192;
     c->lanes_max = (uint32_t)(c->M_max / C_min + 2);
-    c->t2_lanes_max = (uint32_t)(c->M_max / (32 * K2T_WORDS_PER_LANE) + 2);
+    c->t2_tiles_max = k2t_tiles(c->M_max);
     const size_t words_rl = (size_t)c->M_max / 4 + (size_t)c->lanes_max * (K2_EDGE_EMIT_CAP + 8) + 1024;
     c->cap_words_rl = (uint32_t)std::min<size_t>(words_rl, 0xFFFFFFFFu);
     c->ring_events = next_pow2((size_t)c->M_max / 4 + 65536 + WMB_MAXBITS);
@@ -816,10 +815,10 @@ static int ctx_alloc(wmb_ctx *c)
             TRY(dev_alloc(c, &b.pd, 1, true));
             TRY(dev_alloc(c, &b.p2_out, 1, true));
         }
-        TRY(dev_alloc(c, &b.t2_tail, c->t2_lanes_max));
-        TRY(dev_alloc(c, &b.t2_len, c->t2_lanes_max));
-        TRY(dev_alloc(c, &b.t2_sr, c->t2_lanes_max));
-        uint32_t scan_lanes = c->lanes_max > c->t2_lanes_max ? c->lanes_max : c->t2_lanes_max;
+        TRY(dev_alloc(c, &b.t2_tail, c->t2_tiles_max));
+        TRY(dev_alloc(c, &b.t2_len, c->t2_tiles_max));
+        TRY(dev_alloc(c, &b.t2_sr, c->t2_tiles_max));
+        uint32_t scan_lanes = c->lanes_max > c->t2_tiles_max ? c->lanes_max : c->t2_tiles_max;
         if (c->p1_lanes_max > scan_lanes) scan_lanes = c->p1_lanes_max;
         if (c->p2_lanes_max > scan_lanes) scan_lanes = c->p2_lanes_max;
         const size_t n_agg = scan_tiles(scan_lanes) + 1;
@@ -833,7 +832,7 @@ static int ctx_alloc(wmb_ctx *c)
         CUDA_TRY(cudaMemcpy(b.rl_carry, &rl, sizeof(rl), cudaMemcpyHostToDevice));
         for (int a = 0; a < WMB_N_ALGOS; a++) {
             Stream &s = b.s[a];
-            const uint32_t nl = a == WMB_ALGO_T2A ? c->t2_lanes_max : c->lanes_max;
+            const uint32_t nl = a == WMB_ALGO_T2A ? c->t2_tiles_max : c->lanes_max;
             if (a == WMB_ALGO_RLA) TRY(dev_alloc(c, &s.ev, c->cap_words_rl));
             TRY(dev_alloc(c, &s.cnt, nl, true));
             TRY(dev_alloc(c, &s.base, nl));
@@ -1489,10 +1488,8 @@ static int run_batch(wmb_ctx *c, const uint8_t *src, size_t nbytes, cudaEvent_t 
                 K2tParams p;
                 memset(&p, 0, sizeof(p));
                 p.dbits = sb.dbits + wofs; p.sbits = sb.sbits + wofs; p.rssi = sb.rssi + c->W;
-                p.M = M; p.Cw = K2T_WORDS_PER_LANE;
-                const uint32_t nw = (uint32_t)((M + 31) / 32);
-                p.lanes = (nw + p.Cw - 1) / p.Cw;
-                if (p.lanes > c->t2_lanes_max) return set_err(WMB_E_INVAL, "internal: time2 lanes");
+                p.M = M; p.lanes = k2t_tiles(M);
+                if (p.lanes > c->t2_tiles_max) return set_err(WMB_E_INVAL, "internal: time2 tiles");
                 p.cnt = s.cnt; p.tail = b.t2_tail; p.tail_len = b.t2_len; p.base = s.base; p.sr_start = b.t2_sr;
                 p.agg_cnt = s.agg; p.agg_tail = b.t2_agg_tail; p.agg_len = b.t2_agg_len;
                 p.m_base = (int64_t)c->m_consumed;

@@ -1525,6 +1525,43 @@ WMB_D void wmb_reset_device(const ResetParams &p)
     *p.gd = g;
     for (int i = 0; i < 16; i++) p.errors[i] = 0;
 }
+#ifdef WMB_HOSTSIM
+/* ---- time2 blocks in the CPU build ----
+ * The CPU launch runs a time2 kernel as one call per tile (k2t_count / k2t_write, the tile being the scans' lane): the
+ * block's barrier-separated phases one after another over its threads, in the order hs_for picks.  Only the block scan
+ * differs from the device's: serial over the threads' parts instead of warp shuffles. */
+template <class F> static void hs_for(uint32_t n, F f);
+
+/* exclusive scan, in place, of part[0..n) on top of `acc`; returns the inclusive total */
+template <class CH>
+static T2Fold t2_scan_serial(T2Fold *part, uint32_t n, T2Fold acc)
+{
+    for (uint32_t t = 0; t < n; t++) { const T2Fold f = part[t]; part[t] = acc; acc = t2_fold<CH>(acc, f); }
+    return acc;
+}
+template <class CH>
+static void k2t_count(const K2tParams &p, uint32_t tile)
+{
+    static T2Fold part[T2_THREADS];
+    hs_for(T2_THREADS, [&](uint32_t t) { part[t] = k2t_load<CH>(p, tile, t, nullptr); });
+    const T2Fold zero = { 0, 0, 0 };
+    k2t_count_store(p, tile, t2_scan_serial<CH>(part, T2_THREADS, zero));
+}
+template <class CH>
+static void k2t_write(const K2tParams &p, uint32_t tile)
+{
+    static T2Fold part[T2_THREADS];
+    static K2tSmem sm;
+    memset(&sm, 0xA5, sizeof(sm));                                     /* garbage-filled like real smem */
+    hs_for(T2_THREADS, [&](uint32_t t) { part[t] = k2t_load<CH>(p, tile, t, &sm); });
+    t2_scan_serial<CH>(part, T2_THREADS, k2t_carry<CH>(p, tile));
+    hs_for(T2_THREADS, [&](uint32_t t) { k2t_spread<CH>(t, part[t], sm); });
+    for (uint32_t r = 0; r < T2_WPT; r++) {
+        hs_for(T2_THREADS, [&](uint32_t t) { k2t_emit<CH>(p, tile, t, r, sm); });
+        hs_for(T2_THREADS, [&](uint32_t t) { k2t_flush(p, tile, t, r, sm); });
+    }
+}
+#endif
 #ifndef WMB_HOSTSIM
 /* ---- __global__ wrappers ---- */
 __global__ void __launch_bounds__(SCAN_BLOCK) cscan_a_kernel(const CountScan p)
@@ -1543,6 +1580,41 @@ __global__ void __launch_bounds__(SCAN_BLOCK) cscan_c_kernel(const CountScan p)
     if (threadIdx.x == 0) cscan_c_block(p, blockIdx.x, part);
     __syncthreads();
     cscan_c_write(p, blockIdx.x, threadIdx.x, part);
+}
+/* time2: exclusive scan of one T2Fold per thread, in thread order, on top of `carry` (the CPU build's k2t_count /
+ * k2t_write below run it serially): a shuffle scan in every warp, the warps' totals through shared memory.  The inclusive total is the last
+ * thread's result folded with its own value. */
+template <class CH, int NT>
+__device__ T2Fold t2_block_scan(const T2Fold v, const T2Fold carry, T2Fold (&wtot)[NT / 32])
+{
+    const uint32_t lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    T2Fold inc = v;
+#pragma unroll
+    for (uint32_t o = 1; o < 32; o <<= 1) {
+        T2Fold u;
+        u.cnt = __shfl_up_sync(0xFFFFFFFFu, inc.cnt, o);
+        u.tail = __shfl_up_sync(0xFFFFFFFFu, inc.tail, o);
+        u.len = __shfl_up_sync(0xFFFFFFFFu, inc.len, o);
+        if (lane >= o) inc = t2_fold<CH>(u, inc);
+    }
+    if (lane == 31) wtot[w] = inc;
+    T2Fold ex;
+    ex.cnt = __shfl_up_sync(0xFFFFFFFFu, inc.cnt, 1);
+    ex.tail = __shfl_up_sync(0xFFFFFFFFu, inc.tail, 1);
+    ex.len = __shfl_up_sync(0xFFFFFFFFu, inc.len, 1);
+    __syncthreads();
+    T2Fold acc = carry;
+    for (uint32_t i = 0; i < w; i++) acc = t2_fold<CH>(acc, wtot[i]);
+    return lane ? t2_fold<CH>(acc, ex) : acc;
+}
+template <class CH>
+__global__ void __launch_bounds__(T2_THREADS) k2t_count_kernel(const K2tParams p)
+{
+    __shared__ T2Fold wtot[T2_THREADS / 32];
+    const T2Fold f = k2t_load<CH>(p, blockIdx.x, threadIdx.x, nullptr);
+    const T2Fold zero = { 0, 0, 0 };
+    const T2Fold ex = t2_block_scan<CH, T2_THREADS>(f, zero, wtot);
+    if (threadIdx.x == T2_THREADS - 1) k2t_count_store(p, blockIdx.x, t2_fold<CH>(ex, f));
 }
 template <class CH>
 __global__ void __launch_bounds__(SCAN_BLOCK) t2scan_a_kernel(const K2tParams p)
@@ -1565,6 +1637,22 @@ __global__ void __launch_bounds__(SCAN_BLOCK) t2scan_c_kernel(const K2tParams p)
     t2scan_c_write<CH>(p, blockIdx.x, threadIdx.x, part);
 }
 template <class CH>
+__global__ void __launch_bounds__(T2_THREADS) k2t_write_kernel(const K2tParams p)
+{
+    __shared__ K2tSmem sm;
+    __shared__ T2Fold wtot[T2_THREADS / 32];
+    const T2Fold f = k2t_load<CH>(p, blockIdx.x, threadIdx.x, &sm);
+    const T2Fold ex = t2_block_scan<CH, T2_THREADS>(f, k2t_carry<CH>(p, blockIdx.x), wtot);
+    k2t_spread<CH>(threadIdx.x, ex, sm);
+    __syncthreads();
+    for (uint32_t r = 0; r < T2_WPT; r++) {
+        k2t_emit<CH>(p, blockIdx.x, threadIdx.x, r, sm);
+        __syncwarp();
+        k2t_flush(p, blockIdx.x, threadIdx.x, r, sm);
+        __syncwarp();                                             /* the next round reuses the staging */
+    }
+}
+template <class CH>
 __global__ void __launch_bounds__(K2_THREADS) k2a_lanes_kernel(const K2aParams p)
 {
     k2a_lane<CH>(p, blockIdx.x * blockDim.x + threadIdx.x);
@@ -1573,10 +1661,6 @@ __global__ void k2a_verify_kernel(const K2aParams p, uint32_t *n_fail)
 {
     k2a_verify_lane(p, blockIdx.x * blockDim.x + threadIdx.x, n_fail);
 }
-template <class CH>
-__global__ void k2t_count_kernel(const K2tParams p) { k2t_count<CH>(p, blockIdx.x * blockDim.x + threadIdx.x); }
-template <class CH>
-__global__ void k2t_write_kernel(const K2tParams p) { k2t_write<CH>(p, blockIdx.x * blockDim.x + threadIdx.x); }
 template <class CH>
 __global__ void __launch_bounds__(K2_THREADS) k2m_lanes_kernel(const K2mParams p)
 {
