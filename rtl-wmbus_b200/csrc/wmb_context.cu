@@ -79,7 +79,7 @@ struct Stream {                     /* one (chain, algo) bit stream */
     OfsAcc *pend_ofs = nullptr;     /* device: their carrier-offset sums          */
     uint64_t *agg = nullptr;        /* scan scratch [tiles]                       */
     uint64_t total = 0;             /* host mirror of sd->total at the last read  */
-    uint64_t total_prev = 0;        /* ... before the last batch (stage tap)      */
+    uint64_t total_prev = 0;        /* ... before the last batch read (stage tap) */
     /* host framer bookkeeping */
     int64_t busy_until = -1;        /* last ordinal consumed by an accepted packet */
 };
@@ -1249,9 +1249,6 @@ static int run_batch(wmb_ctx *c, const uint8_t *src, size_t nbytes, cudaEvent_t 
      * clock lanes go on cs too, which saves the cross-stream hand-overs (a few microseconds each) */
     const bool solo = alone && c->inflight.empty();
     cudaStream_t sk = solo ? c->cs : c->k1s, sa = solo ? c->cs : c->as[set];
-    for (int ch = 0; ch < WMB_N_CHAINS; ch++)
-        for (int a = 0; a < WMB_N_ALGOS; a++) c->cb[ch].s[a].total_prev = c->cb[ch].s[a].total;   /* stage tap: events of this batch */
-
     if (c->reset_pending) {                            /* the streams that do not follow cs wait for wmb_reset's kernel */
         for (cudaStream_t st : { c->k1s, c->as[0], c->as[1], c->as2[0], c->as2[1] }) CUDA_TRY(cudaStreamWaitEvent(st, c->ev_reset, 0));
         c->reset_pending = false;
@@ -1793,6 +1790,10 @@ static int consume_oldest(wmb_ctx *c)
         for (int a = 0; a < WMB_N_ALGOS; a++) {
             const int k = ch * WMB_N_ALGOS + a;
             c->st.candidates[ch][a] = r.n_cand_total[k];
+            /* stage tap: the events of the batch this gather closes (has_timers).  Records are read in batch order, so
+             * the total before it is the one the record before read -- not s.total when the batch was enqueued, which
+             * lags by the batches still in flight then */
+            if (f.has_timers) c->cb[ch].s[a].total_prev = c->cb[ch].s[a].total;
             c->cb[ch].s[a].total = r.total[k];
         }
     if (r.n > c->slot_cap) return set_err(WMB_E_STATE, "internal: batch record beyond its slot");
