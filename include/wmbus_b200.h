@@ -262,6 +262,66 @@ int wmb_set_bursts(wmb_ctx *c, int chain, uint32_t level);
  * taken stay queued. */
 int wmb_take_bursts(wmb_ctx *c, wmb_burst *out, size_t cap, size_t *n);
 
+/* ---- signal quality: FSK deviation, eye SNR and chip rate of each line and burst --------------------------------
+ * Off by default; wmb_set_line_quality(ctx, 1) turns it on.  Over the carrier-offset window [lo, hi) of a line
+ * (wmb_line_info: T1/C1 [s-384, s-128), S1 [s-1367, s-586), clipped) or of a burst (wmb_burst: [start + g0,
+ * min(end, start + g0 + w))), n samples, x[q] = rint(dphi[q] * 2^24), sum = sum of x:
+ *   1. Class: sample q is high iff x[q] n >= sum (the window mean, in int64, no division), else low.  A sample q in
+ *      [lo + 1, hi - 1) counts iff q - 1, q and q + 1 are all of the same class: the FIR's chip transitions are left
+ *      out of the tone estimates.
+ *   2. Per class k in {hi, lo}, over its counting samples: n_k, s1_k = sum of x, s2_k = sum of x^2 -- integers, exact
+ *      in any order (|x| < 2^26, n <= 781: s2_k < 2^63).  Zero with -a (the cross-product discriminator is not a
+ *      frequency).
+ *   3. On the host, in double: m_k = s1_k / n_k;
+ *        deviation_hz = (m_hi - m_lo) / 2 / 2^24 * 400 kHz / G (G the chain's FIR DC gain, as for offset_hz);
+ *        var = (s2_hi - n_hi m_hi^2 + s2_lo - n_lo m_lo^2) / (n_hi + n_lo - 2);
+ *        eye_snr_db = 10 log10(((m_hi - m_lo) / 2)^2 / var).
+ *      valid = 0 (both NaN) with -a, when a class has fewer than 2 counting samples, when var <= 0, when the report is
+ *      off, and for lines of frames handed to wmb_decode_frames.
+ *   4. Lines only: chip_rate_hz = 800 kHz (bits - 1) / (end_sample - sync_sample), bits = the bit events the framer
+ *      consumed from the access-code bit through the telegram's last bit -- decoded chips per second (T1/C1 chips, S1
+ *      Manchester chips).  It does not need the report (NaN when bits < 2), and holds for wmb_decode_frames' lines too.
+ * Valid before the first push or right after wmb_reset / wmb_seek (else WMB_E_STATE); on is 0 or 1 (else
+ * WMB_E_INVAL).  The setting survives wmb_reset and wmb_seek.  Cost: one more pass over each window already read, and
+ * 40 bytes of device-to-host traffic per candidate and per burst. */
+typedef struct wmb_line_quality {
+    uint64_t sync_sample;     /* as in wmb_line_info                                                         */
+    uint64_t end_sample;
+    uint32_t n_hi, n_lo;      /* counting samples per class                                                  */
+    int64_t  s1_hi, s1_lo;    /* their sum of x                                                              */
+    uint64_t s2_hi, s2_lo;    /* their sum of x^2                                                            */
+    uint32_t bits;            /* bit events consumed, access-code bit through the last bit                   */
+    uint8_t  chain;           /* WMB_CHAIN_*                                                                 */
+    uint8_t  algo;            /* WMB_ALGO_*                                                                  */
+    uint8_t  crc_ok;
+    uint8_t  valid;           /* deviation_hz and eye_snr_db                                                 */
+    double   deviation_hz;
+    double   eye_snr_db;
+    double   chip_rate_hz;
+} wmb_line_quality;
+
+typedef struct wmb_burst_quality {
+    uint64_t start_sample;    /* as in wmb_burst                                                             */
+    uint32_t n_hi, n_lo;
+    int64_t  s1_hi, s1_lo;
+    uint64_t s2_hi, s2_lo;
+    double   deviation_hz;
+    double   eye_snr_db;
+    uint8_t  chain;
+    uint8_t  valid;
+    uint8_t  pad[6];
+} wmb_burst_quality;
+
+int wmb_set_line_quality(wmb_ctx *c, int on);
+
+/* wmb_take_lines_info that also fills qual[i] for the i-th line taken (info and qual may each be NULL); with either it
+ * takes at most rec_cap lines. */
+size_t wmb_take_lines_quality(wmb_ctx *c, char *buf, size_t cap, size_t *n_lines, int timestamp_mode,
+                              wmb_line_info *info, wmb_line_quality *qual, size_t rec_cap);
+
+/* wmb_take_bursts that also fills qual[i] for out[i] (qual may be NULL: wmb_take_bursts is this call). */
+int wmb_take_bursts_quality(wmb_ctx *c, wmb_burst *out, wmb_burst_quality *qual, size_t cap, size_t *n);
+
 /* ---- band survey: a power spectrum of the whole captured band, to find the carriers to decode --------------------
  * Off by default.  wmb_set_spectrum(ctx, N, B) with N bins (256, 512, 1024 or 2048) and B blocks per record (1 .. 2^20)
  * turns it on.  It works on the raw cu8 input, before any mixer, prefilter or decimation, so it does not depend on -s,

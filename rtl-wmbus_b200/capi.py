@@ -52,6 +52,26 @@ def burst_dtype():
     return np.dtype(BURST_FIELDS)
 
 
+# numpy mirrors of wmb_line_quality and wmb_burst_quality (see include/wmbus_b200.h)
+LINE_QUALITY_FIELDS = [("sync_sample", "<u8"), ("end_sample", "<u8"), ("n_hi", "<u4"), ("n_lo", "<u4"),
+                       ("s1_hi", "<i8"), ("s1_lo", "<i8"), ("s2_hi", "<u8"), ("s2_lo", "<u8"), ("bits", "<u4"),
+                       ("chain", "u1"), ("algo", "u1"), ("crc_ok", "u1"), ("valid", "u1"), ("deviation_hz", "<f8"),
+                       ("eye_snr_db", "<f8"), ("chip_rate_hz", "<f8")]
+BURST_QUALITY_FIELDS = [("start_sample", "<u8"), ("n_hi", "<u4"), ("n_lo", "<u4"), ("s1_hi", "<i8"), ("s1_lo", "<i8"),
+                        ("s2_hi", "<u8"), ("s2_lo", "<u8"), ("deviation_hz", "<f8"), ("eye_snr_db", "<f8"),
+                        ("chain", "u1"), ("valid", "u1"), ("pad", "V6")]
+
+
+def line_quality_dtype():
+    import numpy as np
+    return np.dtype(LINE_QUALITY_FIELDS)
+
+
+def burst_quality_dtype():
+    import numpy as np
+    return np.dtype(BURST_QUALITY_FIELDS)
+
+
 # numpy mirror of wmb_spectrum_row (one record of the band survey; see include/wmbus_b200.h)
 SPECTRUM_FIELDS = [("record", "<u8"), ("start_iq", "<u8"), ("blocks", "<u4"), ("bins", "<u4"), ("hz_low", "<f8"),
                    ("hz_step", "<f8")]
@@ -120,6 +140,11 @@ def _bind(lib):
     lib.wmb_set_receiver.argtypes = [C.c_void_p, C.c_int, C.c_uint32, C.c_uint32]
     lib.wmb_set_bursts.argtypes = [C.c_void_p, C.c_int, C.c_uint32]
     lib.wmb_take_bursts.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
+    lib.wmb_set_line_quality.argtypes = [C.c_void_p, C.c_int]
+    lib.wmb_take_lines_quality.argtypes = [C.c_void_p, C.c_char_p, C.c_size_t, C.POINTER(C.c_size_t), C.c_int,
+                                           C.c_void_p, C.c_void_p, C.c_size_t]
+    lib.wmb_take_lines_quality.restype = C.c_size_t
+    lib.wmb_take_bursts_quality.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
     lib.wmb_set_spectrum.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32]
     lib.wmb_take_spectrum.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
     lib.wmb_debug_spectrum_tables.argtypes = [C.c_uint32, C.c_void_p, C.c_void_p]
@@ -135,7 +160,7 @@ EXPORTS = ["wmb_reset", "wmb_host_alloc", "wmb_host_free", "wmb_default_opts", "
            "wmb_process", "wmb_process_device", "wmb_get_stats", "wmb_debug_copy_stage", "wmb_debug_copy_bits", "wmb_debug_copy_events", "wmb_debug_arith",
            "wmb_seek", "wmb_set_line_window", "wmb_boundary_state", "wmb_pending_before", "wmb_set_receiver",
            "wmb_take_lines_info", "wmb_set_bursts", "wmb_take_bursts", "wmb_set_spectrum", "wmb_take_spectrum",
-           "wmb_debug_spectrum_tables"]
+           "wmb_debug_spectrum_tables", "wmb_set_line_quality", "wmb_take_lines_quality", "wmb_take_bursts_quality"]
 
 
 def load_library(path: str | None = None):
@@ -183,10 +208,12 @@ class WmbusB200:
     burst_level=(t1c1, s1): the burst report's level per chain, see wmb_set_bursts() (0: off, the default); it survives
     reset() and seek() too.  take_bursts() hands out the closed pieces.
     spectrum=(bins, blocks_per_record): the band survey, see wmb_set_spectrum() (None: off, the default); it survives
-    reset() and seek().  take_spectrum() hands out the closed records."""
+    reset() and seek().  take_spectrum() hands out the closed records.
+    quality=True: the signal-quality report, see wmb_set_line_quality() (off by default); it survives reset() and
+    seek().  take_lines(quality=True) and take_bursts(quality=True) hand out its records."""
 
     def __init__(self, flags: str = "", device: int = 0, lib=None, clock_lock=None, access_code_errors=None,
-                 burst_level=None, spectrum=None, **tuning):
+                 burst_level=None, spectrum=None, quality=False, **tuning):
         self.lib = lib or load_library()
         self.opts = opts_from_flags(self.lib, flags, **tuning)
         self._ctx = C.c_void_p()
@@ -213,6 +240,12 @@ class WmbusB200:
         if spectrum is not None:
             try:
                 self.set_spectrum(*spectrum)
+            except Exception:
+                self.close()
+                raise
+        if quality:
+            try:
+                self.set_line_quality(True)
             except Exception:
                 self.close()
                 raise
@@ -313,10 +346,29 @@ class WmbusB200:
     def decode_frames(self, arr, n):
         self._check(self.lib.wmb_decode_frames(self._ctx, arr, n))
 
-    def take_lines(self, timestamp_mode=1, info=False):
-        """info=True: (lines, records), records a numpy structured array of wmb_line_info, one per line"""
+    def take_lines(self, timestamp_mode=1, info=False, quality=False):
+        """info=True: (lines, records), records a numpy structured array of wmb_line_info, one per line.
+        quality=True: (lines, quality) with a numpy structured array of wmb_line_quality (line_quality_dtype()), one per
+        line; with both: (lines, records, quality)"""
         nl = C.c_size_t(0)
         out = []
+        if quality:
+            import numpy as np
+            cap = 1 << 14
+            infos, quals = [], []
+            while True:
+                r = np.zeros(cap, line_info_dtype())
+                q = np.zeros(cap, line_quality_dtype())
+                n = self.lib.wmb_take_lines_quality(self._ctx, self._out, len(self._out), C.byref(nl), timestamp_mode,
+                                                    r.ctypes.data, q.ctypes.data, cap)
+                if not nl.value:
+                    break
+                out += self._lines(n)
+                infos.append(r[:nl.value])
+                quals.append(q[:nl.value])
+            infos = np.concatenate(infos) if infos else np.zeros(0, line_info_dtype())
+            quals = np.concatenate(quals) if quals else np.zeros(0, line_quality_dtype())
+            return (out, infos, quals) if info else (out, quals)
         if not info:
             while True:
                 n = self.lib.wmb_take_lines(self._ctx, self._out, len(self._out), C.byref(nl), timestamp_mode)
@@ -352,21 +404,32 @@ class WmbusB200:
         """burst report level of one chain, 0 = off (before the first push, or after reset/seek)"""
         self._check(self.lib.wmb_set_bursts(self._ctx, chain, level))
 
-    def take_bursts(self):
+    def take_bursts(self, quality=False):
         """the closed burst pieces not taken yet, ordered by (start_sample, chain): a numpy structured array of
-        wmb_burst (burst_dtype())"""
+        wmb_burst (burst_dtype()); quality=True: (bursts, quality), quality the wmb_burst_quality records
+        (burst_quality_dtype()), one per burst"""
         import numpy as np
         cap = 1 << 14
-        parts = []
+        parts, qparts = [], []
         while True:
             r = np.zeros(cap, burst_dtype())
+            q = np.zeros(cap if quality else 0, burst_quality_dtype())
             n = C.c_size_t(0)
-            self._check(self.lib.wmb_take_bursts(self._ctx, r.ctypes.data, cap, C.byref(n)))
+            self._check(self.lib.wmb_take_bursts_quality(self._ctx, r.ctypes.data, q.ctypes.data if quality else None,
+                                                         cap, C.byref(n)))
             if n.value:
                 parts.append(r[:n.value])
+                qparts.append(q[:n.value])
             if n.value < cap:
                 break
-        return np.concatenate(parts) if parts else np.zeros(0, burst_dtype())
+        b = np.concatenate(parts) if parts else np.zeros(0, burst_dtype())
+        if not quality:
+            return b
+        return b, (np.concatenate(qparts) if qparts else np.zeros(0, burst_quality_dtype()))
+
+    def set_line_quality(self, on: bool):
+        """signal-quality report on / off (before the first push, or after reset/seek)"""
+        self._check(self.lib.wmb_set_line_quality(self._ctx, 1 if on else 0))
 
     def set_spectrum(self, bins: int, blocks_per_record: int):
         """band survey: bins 256 .. 2048 (0 = off), blocks per record (before the first push, or after reset/seek)"""

@@ -33,6 +33,12 @@
  *   WMBUS_B200_SPECTRUM_BINS=<n>    bins N: 256, 512, 1024 (default) or 2048
  *   WMBUS_B200_SPECTRUM_BLOCKS=<n>  blocks of N IQ samples per record, 1 .. 2^20 (default 16384: 10.5 s at 1.6 MS/s)
  *   A path that cannot be opened or a bad value is an error at start-up.  stdout does not change.
+ *   WMBUS_B200_LINE_QUALITY=<path>  write one record per stdout line, in the same order and flushed with it:
+ *                              ALGO;MODE;CRC_OK;LINK_LAYER_IDENT_NO;SYNC_SAMPLE;DEVIATION_HZ;EYE_SNR_DB;CHIP_RATE_HZ
+ *                              (wmb_line_quality; nan where not valid).
+ *   WMBUS_B200_BURST_QUALITY=<path> (with WMBUS_B200_BURSTS) write one record per burst piece, in the burst file's
+ *                              order: CHAIN;START_SAMPLE;DEVIATION_HZ;EYE_SNR_DB (wmb_burst_quality; nan where not valid).
+ *   Either turns the quality report on (wmb_set_line_quality).  A path that cannot be opened is an error at start-up.
  */
 #define _GNU_SOURCE
 #include <errno.h>
@@ -112,12 +118,22 @@ static int parse_pair(const char *e, unsigned long v[2])
     return *end == 0 && v[0] <= 0xFFFFFFFFul && v[1] <= 0xFFFFFFFFul;
 }
 
-/* WMBUS_B200_LINE_INFO: one record per stdout line, in the same order */
-static FILE *g_info_file = NULL;
+/* WMBUS_B200_LINE_INFO / WMBUS_B200_LINE_QUALITY: one record per stdout line, in the same order */
+static FILE *g_info_file = NULL, *g_qual_file = NULL;
 #define INFO_CAP 4096
 static wmb_line_info g_info[INFO_CAP];
+static wmb_line_quality g_qual[INFO_CAP];
 
-/* ALGO;MODE;CRC_OK;LINK_LAYER_IDENT_NO;SYNC_SAMPLE;CARRIER_HZ;OFFSET_HZ of each line of out[0..n) */
+/* "%.<prec>f" of v, or nan */
+static const char *fmt_or_nan(char *s, size_t cap, int valid, int prec, double v)
+{
+    if (valid && v == v) snprintf(s, cap, "%.*f", prec, v);
+    else snprintf(s, cap, "nan");
+    return s;
+}
+
+/* ALGO;MODE;CRC_OK;LINK_LAYER_IDENT_NO;SYNC_SAMPLE;CARRIER_HZ;OFFSET_HZ of each line of out[0..n) to the info file, and
+ * ALGO;MODE;CRC_OK;LINK_LAYER_IDENT_NO;SYNC_SAMPLE;DEVIATION_HZ;EYE_SNR_DB;CHIP_RATE_HZ to the quality file */
 static void write_info(const char *out, size_t n, size_t nl, int show_algorithm)
 {
     const char *l = out;
@@ -135,14 +151,22 @@ static void write_info(const char *out, size_t n, size_t nl, int show_algorithm)
             if (!q) break;
             p = q + 1;
         }
-        const wmb_line_info *r = &g_info[i];
-        char off[32];
-        if (r->valid) snprintf(off, sizeof(off), "%.0f", r->offset_hz);
-        else snprintf(off, sizeof(off), "nan");
-        if (nf >= 8)
+        if (nf >= 8 && g_info_file) {
+            const wmb_line_info *r = &g_info[i];
+            char off[32];
             fprintf(g_info_file, "%s;%.*s;%u;%.*s;%llu;%.0f;%s\n", r->algo == WMB_ALGO_RLA ? "rla" : "t2a",
                     (int)(f[1] - f[0] - 1), f[0], (unsigned)r->crc_ok, (int)(f[7] - f[6] - 1), f[6],
-                    (unsigned long long)r->sync_sample, r->carrier_hz, off);
+                    (unsigned long long)r->sync_sample, r->carrier_hz, fmt_or_nan(off, sizeof(off), r->valid, 0, r->offset_hz));
+        }
+        if (nf >= 8 && g_qual_file) {
+            const wmb_line_quality *r = &g_qual[i];
+            char dev[32], snr[32], rate[32];
+            fprintf(g_qual_file, "%s;%.*s;%u;%.*s;%llu;%s;%s;%s\n", r->algo == WMB_ALGO_RLA ? "rla" : "t2a",
+                    (int)(f[1] - f[0] - 1), f[0], (unsigned)r->crc_ok, (int)(f[7] - f[6] - 1), f[6],
+                    (unsigned long long)r->sync_sample, fmt_or_nan(dev, sizeof(dev), r->valid, 0, r->deviation_hz),
+                    fmt_or_nan(snr, sizeof(snr), r->valid, 2, r->eye_snr_db),
+                    fmt_or_nan(rate, sizeof(rate), 1, 1, r->chip_rate_hz));
+        }
         l = e + 1;
     }
 }
@@ -154,13 +178,17 @@ static void write_info(const char *out, size_t n, size_t nl, int show_algorithm)
 static FILE *g_burst_file = NULL;
 #define BURST_CAP 1024
 static wmb_burst g_bursts[BURST_CAP];
+/* WMBUS_B200_BURST_QUALITY: one record per burst piece, in the burst file's order: CHAIN;START_SAMPLE;DEVIATION_HZ;
+ * EYE_SNR_DB */
+static FILE *g_bqual_file = NULL;
+static wmb_burst_quality g_bqual[BURST_CAP];
 
 static void emit_bursts(wmb_ctx *ctx)
 {
     if (!g_burst_file) return;
     for (;;) {
         size_t n = 0;
-        if (wmb_take_bursts(ctx, g_bursts, BURST_CAP, &n) != WMB_OK || !n) break;
+        if (wmb_take_bursts_quality(ctx, g_bursts, g_bqual_file ? g_bqual : NULL, BURST_CAP, &n) != WMB_OK || !n) break;
         for (size_t i = 0; i < n; i++) {
             const wmb_burst *b = &g_bursts[i];
             char off[32];
@@ -169,10 +197,18 @@ static void emit_bursts(wmb_ctx *ctx)
             fprintf(g_burst_file, "%s;%llu;%llu;%u;%.1f;%.0f;%s;%u\n", b->chain == WMB_CHAIN_T1C1 ? "T1C1" : "S1",
                     (unsigned long long)b->start_sample, (unsigned long long)b->end_sample, (unsigned)b->peak,
                     (double)b->rssi_sum / (double)(b->end_sample - b->start_sample), b->carrier_hz, off, (unsigned)b->flags);
+            if (g_bqual_file) {
+                const wmb_burst_quality *q = &g_bqual[i];
+                char dev[32], snr[32];
+                fprintf(g_bqual_file, "%s;%llu;%s;%s\n", q->chain == WMB_CHAIN_T1C1 ? "T1C1" : "S1",
+                        (unsigned long long)q->start_sample, fmt_or_nan(dev, sizeof(dev), q->valid, 0, q->deviation_hz),
+                        fmt_or_nan(snr, sizeof(snr), q->valid, 2, q->eye_snr_db));
+            }
         }
         if (n < BURST_CAP) break;
     }
     fflush(g_burst_file);
+    if (g_bqual_file) fflush(g_bqual_file);
 }
 
 /* WMBUS_B200_SPECTRUM: a mean line and a peak line per closed record of the band survey */
@@ -212,14 +248,16 @@ static int emit_lines(wmb_ctx *ctx, char *out, size_t outcap, int show_algorithm
     emit_spectrum(ctx);
     for (;;) {
         size_t nl = 0;
-        const size_t n = g_info_file ? wmb_take_lines_info(ctx, out, outcap, &nl, 0, g_info, INFO_CAP)
-                                     : wmb_take_lines(ctx, out, outcap, &nl, 0);
+        const size_t n = g_info_file || g_qual_file
+            ? wmb_take_lines_quality(ctx, out, outcap, &nl, 0, g_info_file ? g_info : NULL, g_qual_file ? g_qual : NULL, INFO_CAP)
+            : wmb_take_lines(ctx, out, outcap, &nl, 0);
         if (!nl) return 0;
         fwrite(out, 1, n, stdout);
         fflush(stdout);                                 /* t1_c1_packet_decoder.h:698-699 */
-        if (g_info_file) {
+        if (g_info_file || g_qual_file) {
             write_info(out, n, nl, show_algorithm);
-            fflush(g_info_file);
+            if (g_info_file) fflush(g_info_file);
+            if (g_qual_file) fflush(g_qual_file);
         }
     }
 }
@@ -334,6 +372,20 @@ int main(int argc, char *argv[])
         fprintf(stderr, "rtl_wmbus_b200: WMBUS_B200_LINE_INFO=%s: %s\n", e, strerror(errno));
         return EXIT_FAILURE;
     }
+    if ((e = getenv("WMBUS_B200_LINE_QUALITY")) != NULL && (g_qual_file = fopen(e, "w")) == NULL) {
+        fprintf(stderr, "rtl_wmbus_b200: WMBUS_B200_LINE_QUALITY=%s: %s\n", e, strerror(errno));
+        return EXIT_FAILURE;
+    }
+    if ((e = getenv("WMBUS_B200_BURST_QUALITY")) != NULL) {
+        if (!g_burst_file) {
+            fprintf(stderr, "rtl_wmbus_b200: WMBUS_B200_BURST_QUALITY needs WMBUS_B200_BURSTS\n");
+            return EXIT_FAILURE;
+        }
+        if ((g_bqual_file = fopen(e, "w")) == NULL) {
+            fprintf(stderr, "rtl_wmbus_b200: WMBUS_B200_BURST_QUALITY=%s: %s\n", e, strerror(errno));
+            return EXIT_FAILURE;
+        }
+    }
 
     wmb_ctx *ctx = NULL;
     if (wmb_create(&o, device, &ctx) != WMB_OK) {
@@ -351,6 +403,10 @@ int main(int argc, char *argv[])
                 fprintf(stderr, "rtl_wmbus_b200: %s\n", wmb_last_error());
                 return EXIT_FAILURE;
             }
+    if ((g_qual_file || g_bqual_file) && wmb_set_line_quality(ctx, 1) != WMB_OK) {
+        fprintf(stderr, "rtl_wmbus_b200: %s\n", wmb_last_error());
+        return EXIT_FAILURE;
+    }
     if (g_spec_file && wmb_set_spectrum(ctx, (uint32_t)spec_bins, (uint32_t)spec_blocks) != WMB_OK) {
         fprintf(stderr, "rtl_wmbus_b200: WMBUS_B200_SPECTRUM: %s\n", wmb_last_error());
         return EXIT_FAILURE;
@@ -434,6 +490,14 @@ int main(int argc, char *argv[])
     }
     if (g_info_file && fclose(g_info_file) != 0 && rc == WMB_OK) {
         fprintf(stderr, "rtl_wmbus_b200: WMBUS_B200_LINE_INFO: %s\n", strerror(errno));
+        return EXIT_FAILURE;
+    }
+    if (g_qual_file && fclose(g_qual_file) != 0 && rc == WMB_OK) {
+        fprintf(stderr, "rtl_wmbus_b200: WMBUS_B200_LINE_QUALITY: %s\n", strerror(errno));
+        return EXIT_FAILURE;
+    }
+    if (g_bqual_file && fclose(g_bqual_file) != 0 && rc == WMB_OK) {
+        fprintf(stderr, "rtl_wmbus_b200: WMBUS_B200_BURST_QUALITY: %s\n", strerror(errno));
         return EXIT_FAILURE;
     }
     return rc == WMB_OK ? EXIT_SUCCESS : EXIT_FAILURE;

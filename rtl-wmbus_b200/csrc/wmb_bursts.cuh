@@ -40,6 +40,8 @@ struct BurstDev {                   /* carried from batch to batch, one per chai
     uint32_t open, flags;           /* a run is in progress; the open piece's flags                               */
     uint64_t n_ev;                  /* events of the current batch (the count scan's total)                       */
     uint32_t n_items, pad;
+    QualAcc  q;                     /* quality: the open piece's class sums, once its window is whole (qdone)     */
+    uint32_t qdone, pad2;
 };
 
 struct BurstItem {                  /* one piece for kb_reduce, batch-relative sample indices */
@@ -48,7 +50,12 @@ struct BurstItem {                  /* one piece for kb_reduce, batch-relative s
     uint64_t rsum; int64_t wsum;    /* sums before a (the open piece of the last batch)                           */
     uint32_t peak, wn;
     uint32_t flags; int32_t out;    /* out: record index, -1: the piece still open (sums go to BurstDev)          */
+    QualAcc  q;                     /* quality sums taken in an earlier batch (qdone)                             */
+    uint32_t qdone, pad;
 };
+
+/* what kb_reduce's quality pass does for one item: the window [lo, hi) with its sum and n, run = take the sums now */
+struct BurstQPlan { int64_t lo, hi, sum, n; uint32_t run, pad; };
 
 struct BurstRec {                   /* device -> host, one per reported piece */
     uint64_t start, end;
@@ -79,6 +86,8 @@ struct BurstParams {
     BurstItem *items;
     BurstRec *out;                  /* this slot's records of the chain                                           */
     BurstSlot *slot;
+    QualAcc  *qout;                 /* quality (null: off): the records' class sums, parallel to out              */
+    uint32_t qual_skip, pad;        /* 1 (-a): zero sums                                                          */
 };
 
 WMB_D int burst_msb(uint32_t v)
@@ -154,6 +163,7 @@ struct BurstRunCtx {                /* what every thread of kb_runs reads before
     uint64_t rsum; int64_t wsum; uint32_t peak, wn, flags0;
     uint32_t open_in, n_runs;
     uint64_t n_ev;
+    QualAcc q; uint32_t qdone;
 };
 
 WMB_D void kb_run_ctx(const BurstParams &p, BurstRunCtx &r)
@@ -163,6 +173,7 @@ WMB_D void kb_run_ctx(const BurstParams &p, BurstRunCtx &r)
     r.n_ev = p.final_ ? 0 : bd.n_ev;
     r.s0 = bd.s - p.m_first; r.ps0 = bd.ps - p.m_first; r.la0 = bd.la - p.m_first;
     r.rsum = bd.rsum; r.wsum = bd.wsum; r.peak = bd.peak; r.wn = bd.wn; r.flags0 = bd.flags;
+    r.q = bd.q; r.qdone = bd.qdone;
     /* the last above sample so far: an open run has one within the last G samples */
     r.la = r.open_in ? r.la0 : -((int64_t)1 << 40);
     const int64_t G = burst_G(p.chain);
@@ -223,6 +234,8 @@ WMB_D uint32_t kb_run(const BurstParams &p, const BurstRunCtx &r, uint32_t i, bo
                 const bool carried = cur == ps && r.open_in && i == 0;
                 it.rsum = carried ? rsum : 0; it.wsum = carried ? wsum : 0;
                 it.peak = carried ? peak : 0; it.wn = carried ? wn : 0;
+                if (carried) it.q = r.q; else qual_zero(it.q);
+                it.qdone = carried ? r.qdone : 0u; it.pad = 0;
                 it.flags = f; it.out = item_open ? -1 : (int32_t)(at + n);
                 p.items[at + n] = it;
             }
@@ -289,17 +302,14 @@ WMB_D void kb_reduce_part(const BurstParams &p, uint32_t it, uint32_t t, uint32_
     const int64_t wlo = wlo0 > x.a ? wlo0 : x.a;
     const int64_t whi = whi0 < x.b ? whi0 : x.b;
     int64_t wsum = 0;
-    for (int64_t m = wlo + t; m < whi; m += nt) {
-#ifdef WMB_HOSTSIM
-        wsum += (int64_t)llrintf(p.dphi[m] * WMB_OFS_SCALE);
-#else
-        wsum += __float2ll_rn(p.dphi[m] * WMB_OFS_SCALE);
-#endif
-    }
+    for (int64_t m = wlo + t; m < whi; m += nt) wsum += wmb_ofs_x(p.dphi[m]);
     part[t].rsum = rsum; part[t].wsum = wsum; part[t].peak = peak; part[t].pad = 0;
 }
 
-WMB_D void kb_reduce_finish(const BurstParams &p, uint32_t it, const BurstPart *part, uint32_t nt)
+/* qp (quality on): the item's quality pass.  The window [ps + g0, min(pe, ps + g0 + w)) is whole once its end is known:
+ * a closed piece's always, the open piece's when ps + g0 + w <= b (its end lies at or after b).  The sums are taken in
+ * that batch; the window reaches back at most G + w + 1 samples before it, inside the set's history prefix */
+WMB_D void kb_reduce_finish(const BurstParams &p, uint32_t it, const BurstPart *part, uint32_t nt, BurstQPlan *qp)
 {
     const BurstItem &x = p.items[it];
     uint64_t rsum = x.rsum;
@@ -310,6 +320,11 @@ WMB_D void kb_reduce_finish(const BurstParams &p, uint32_t it, const BurstPart *
     const int64_t wlo = wlo0 > x.a ? wlo0 : x.a;
     const int64_t whi = whi0 < x.b ? whi0 : x.b;
     const uint32_t wn = x.wn + (uint32_t)(whi > wlo ? whi - wlo : 0);
+    if (qp) {
+        const int64_t qhi = x.out < 0 ? whi0 : (whi0 < x.pe ? whi0 : x.pe);
+        qp->lo = wlo0; qp->hi = qhi; qp->sum = wsum; qp->n = wn; qp->pad = 0;
+        qp->run = (!x.qdone && !p.qual_skip && (x.out >= 0 || whi0 <= x.b)) ? 1u : 0u;
+    }
     if (x.out < 0) {
         BurstDev &bd = *p.bd;
         bd.rsum = rsum; bd.wsum = wsum; bd.peak = peak; bd.wn = wn;
@@ -320,6 +335,27 @@ WMB_D void kb_reduce_finish(const BurstParams &p, uint32_t it, const BurstPart *
     r.rssi_sum = rsum; r.sum = wsum; r.n = wn;
     r.peak = (uint8_t)peak; r.chain = (uint8_t)p.chain; r.flags = (uint8_t)x.flags; r.pad = 0;
     p.out[x.out] = r;
+}
+
+/* the quality pass (quality on, after kb_reduce_finish): thread t of nt */
+WMB_D void kb_qual_part(const BurstParams &p, const BurstQPlan &qp, uint32_t t, uint32_t nt, QualAcc *part)
+{
+    if (qp.run) qual_part(p.dphi, qp.lo, qp.hi, qp.sum, qp.n, t, nt, part[t]);
+    else qual_zero(part[t]);
+}
+
+/* ... and its result: the record's sums, or the open piece's (kept in BurstDev until its record is written) */
+WMB_D void kb_qual_finish(const BurstParams &p, uint32_t it, const BurstQPlan &qp, const QualAcc *part, uint32_t nt)
+{
+    const BurstItem &x = p.items[it];
+    QualAcc q = x.q;
+    if (qp.run) {
+        qual_zero(q);
+        for (uint32_t t = 0; t < nt; t++) qual_add(q, part[t]);
+    }
+    if (x.out >= 0) { p.qout[x.out] = q; return; }
+    BurstDev &bd = *p.bd;
+    bd.q = q; bd.qdone = (x.qdone || qp.run) ? 1u : 0u;
 }
 
 #ifndef WMB_HOSTSIM
@@ -359,12 +395,20 @@ __global__ void __launch_bounds__(WMB_BURST_BLOCK) kb_runs_kernel(const BurstPar
 __global__ void __launch_bounds__(WMB_BURST_BLOCK) kb_reduce_kernel(const BurstParams p)
 {
     __shared__ BurstPart part[WMB_BURST_BLOCK];
+    __shared__ QualAcc qpart[WMB_BURST_BLOCK];
+    __shared__ BurstQPlan qp;
     const uint32_t n = p.bd->n_items;
     for (uint32_t it = blockIdx.x; it < n; it += gridDim.x) {
         kb_reduce_part(p, it, threadIdx.x, WMB_BURST_BLOCK, part);
         __syncthreads();
-        if (threadIdx.x == 0) kb_reduce_finish(p, it, part, WMB_BURST_BLOCK);
+        if (threadIdx.x == 0) kb_reduce_finish(p, it, part, WMB_BURST_BLOCK, p.qout ? &qp : nullptr);
         __syncthreads();
+        if (p.qout) {                                   /* the launch's parameter: the whole block takes this branch */
+            kb_qual_part(p, qp, threadIdx.x, WMB_BURST_BLOCK, qpart);
+            __syncthreads();
+            if (threadIdx.x == 0) kb_qual_finish(p, it, qp, qpart, WMB_BURST_BLOCK);
+            __syncthreads();
+        }
     }
 }
 #endif

@@ -77,6 +77,7 @@ struct Stream {                     /* one (chain, algo) bit stream */
     uint64_t *cand = nullptr;       /* device: new access-code matches (ordinals, unordered) */
     uint64_t *pend = nullptr;       /* device: candidates waiting for more bits   */
     OfsAcc *pend_ofs = nullptr;     /* device: their carrier-offset sums          */
+    QualAcc *pend_qual = nullptr;   /* device: their quality sums (quality on)    */
     uint64_t *agg = nullptr;        /* scan scratch [tiles]                       */
     uint64_t total = 0;             /* host mirror of sd->total at the last read  */
     uint64_t total_prev = 0;        /* ... before the last batch read (stage tap) */
@@ -126,6 +127,13 @@ struct QueuedLine {
     uint64_t sync_sample;           /* access-code match */
     int64_t ofs_sum;                /* carrier-offset window (FrameHdr) */
     uint32_t ofs_n;
+    QualAcc qual;                   /* quality class sums (zero when the report is off or the frame came from the caller) */
+};
+
+/* a closed burst piece and its quality sums (wmb_take_bursts_quality) */
+struct QueuedBurst {
+    wmb_burst b;
+    QualAcc q;
 };
 
 struct wmb_ctx {
@@ -196,7 +204,8 @@ struct wmb_ctx {
     uint32_t *d_cut_n = nullptr;
     uint64_t *d_k3_agg = nullptr;
     uint32_t spec_n = 0, spec_pool = 0;              /* entries / bytes copied before their counts are known */
-    struct InFlight { int slot; bool final; bool has_timers; uint64_t m_end; bool bursts; uint32_t burst_spec; bool spec; };
+    struct InFlight { int slot; bool final; bool has_timers; uint64_t m_end; bool bursts; uint32_t burst_spec; bool spec;
+                      bool quality, bquality; };
     std::vector<InFlight> inflight;                  /* gathered batches whose results the host has not read yet */
     uint64_t stat_rerun_seen = 0, stat_fallback_seen = 0;
     double acc_demod_ms = 0, acc_bitsync_ms = 0, acc_pass_ms = 0;    /* timers of the current push */
@@ -228,8 +237,14 @@ struct wmb_ctx {
     uint32_t burst_spec = 64;                        /* records copied per slot and chain before their count is known */
     BurstRec *d_brec = nullptr, *h_brec = nullptr;   /* [WMB_NSLOT][chain][burst_cap] */
     BurstSlot *d_bslot = nullptr, *h_bslot = nullptr;
-    std::vector<wmb_burst> bursts;                   /* closed pieces not taken yet */
+    std::vector<QueuedBurst> bursts;                 /* closed pieces not taken yet */
     uint64_t burst_frontier = 0;                     /* no piece still to come starts before this sample */
+
+    /* signal quality (wmb_set_line_quality; survives wmb_reset).  Off: nothing is allocated, launched or copied */
+    bool quality = false;
+    bool qual_allocated = false;
+    QualAcc *d_qual = nullptr, *h_qual = nullptr;    /* [WMB_NSLOT * slot_cap], parallel to d_hdr / h_hdr */
+    QualAcc *d_bqual = nullptr, *h_bqual = nullptr;  /* [WMB_NSLOT][chain][burst_cap], parallel to d_brec / h_brec */
 
     /* band survey (wmb_set_spectrum; the setting survives wmb_reset).  Bins 0: off, nothing is allocated or launched */
     uint32_t spec_bins = 0, spec_B = 0;
@@ -522,9 +537,15 @@ static int launch_bursts(wmb_ctx *c, const BurstParams &p, uint64_t *agg)
     }
     {
         static BurstPart part[WMB_BURST_BLOCK];
+        static QualAcc qpart[WMB_BURST_BLOCK];
         hs_for(p.bd->n_items, [&](uint32_t it) {
+            BurstQPlan qp;
             hs_for(WMB_BURST_BLOCK, [&](uint32_t t) { kb_reduce_part(p, it, t, WMB_BURST_BLOCK, part); });
-            kb_reduce_finish(p, it, part, WMB_BURST_BLOCK);
+            kb_reduce_finish(p, it, part, WMB_BURST_BLOCK, p.qout ? &qp : nullptr);
+            if (p.qout) {
+                hs_for(WMB_BURST_BLOCK, [&](uint32_t t) { kb_qual_part(p, qp, t, WMB_BURST_BLOCK, qpart); });
+                kb_qual_finish(p, it, qp, qpart, WMB_BURST_BLOCK);
+            }
         });
     }
     c->st.kernel_launches += 2;
@@ -886,6 +907,25 @@ static int burst_alloc(wmb_ctx *c)
     c->burst_spec = std::min<uint32_t>(64, c->burst_cap);
     CUDA_TRY(cudaDeviceSynchronize());
     c->burst_allocated = true;
+    return WMB_OK;
+}
+
+/* the quality report's buffers, at the first gather that needs them: beside the candidate log and the carried
+ * candidates, and (when the burst report is on, so its tables exist) beside the burst records */
+static int qual_alloc(wmb_ctx *c)
+{
+    if (!c->qual_allocated) {
+        TRY(dev_alloc(c, &c->d_qual, (size_t)WMB_NSLOT * c->slot_cap));
+        TRY(host_alloc(c, &c->h_qual, (size_t)WMB_NSLOT * c->slot_cap));
+        for (int ch = 0; ch < WMB_N_CHAINS; ch++)
+            for (int a = 0; a < WMB_N_ALGOS; a++)
+                if (c->cb[ch].s[a].pend) TRY(dev_alloc(c, &c->cb[ch].s[a].pend_qual, c->pend_cap));
+        c->qual_allocated = true;
+    }
+    if (c->burst_allocated && !c->d_bqual) {
+        TRY(dev_alloc(c, &c->d_bqual, (size_t)WMB_NSLOT * WMB_N_CHAINS * c->burst_cap));
+        TRY(host_alloc(c, &c->h_bqual, (size_t)WMB_NSLOT * WMB_N_CHAINS * c->burst_cap));
+    }
     return WMB_OK;
 }
 
@@ -1546,7 +1586,7 @@ static double chain_carrier_hz(const wmb_ctx *c, int chain)
 }
 
 /* one slot's burst records -> the queue; the frontier: where the next piece of any chain may start */
-static int book_bursts(wmb_ctx *c, int slot, uint64_t m_end, uint32_t spec)
+static int book_bursts(wmb_ctx *c, int slot, uint64_t m_end, uint32_t spec, bool quality)
 {
     const BurstSlot bs = c->h_bslot[slot];
     uint64_t frontier = m_end;
@@ -1559,21 +1599,27 @@ static int book_bursts(wmb_ctx *c, int slot, uint64_t m_end, uint32_t spec)
         if (n > spec) {
             CUDA_TRY(cudaMemcpyAsync(c->h_brec + at + spec, c->d_brec + at + spec, (size_t)(n - spec) * sizeof(BurstRec),
                                      cudaMemcpyDeviceToHost, c->xs));
+            if (quality)
+                CUDA_TRY(cudaMemcpyAsync(c->h_bqual + at + spec, c->d_bqual + at + spec, (size_t)(n - spec) * sizeof(QualAcc),
+                                         cudaMemcpyDeviceToHost, c->xs));
             CUDA_TRY(cudaStreamSynchronize(c->xs));
         }
         c->st.d2h_bytes += (uint64_t)std::max(n, spec) * sizeof(BurstRec);
+        if (quality) c->st.d2h_bytes += (uint64_t)std::max(n, spec) * sizeof(QualAcc);
         most = std::max(most, n);
         for (uint32_t i = 0; i < n; i++) {
             const BurstRec &r = c->h_brec[at + i];
-            wmb_burst b;
+            QueuedBurst qb;
+            wmb_burst &b = qb.b;
             memset(&b, 0, sizeof(b));
+            if (quality) qb.q = c->h_bqual[at + i]; else qual_zero(qb.q);
             b.start_sample = r.start; b.end_sample = r.end; b.rssi_sum = r.rssi_sum; b.sum = r.sum; b.n = r.n;
             b.chain = r.chain; b.peak = r.peak; b.flags = r.flags;
             /* -a: the cross-product discriminator is not a frequency */
             b.valid = (uint8_t)(r.n > 0 && c->o.accurate_atan ? 1 : 0);
             b.carrier_hz = chain_carrier_hz(c, ch);
             b.offset_hz = b.valid ? (double)r.sum / (double)r.n / (double)WMB_OFS_SCALE * 400e3 / c->fir_gain[ch] : NAN;
-            c->bursts.push_back(b);
+            c->bursts.push_back(qb);
         }
         if (bs.open[ch] && (uint64_t)bs.ps[ch] < frontier) frontier = (uint64_t)bs.ps[ch];
     }
@@ -1594,6 +1640,10 @@ static int enqueue_gather(wmb_ctx *c, bool final, bool after_batch)
     if (c->inflight.size() >= WMB_NSLOT) TRY(consume_oldest(c));          /* the slot's host mirror must be free */
     const int slot = (int)(c->gather_no % WMB_NSLOT);
     const size_t lb = (size_t)slot * c->slot_cap, pb = (size_t)slot * c->slot_pool;
+    const bool quality = c->quality && !c->manual;  /* (a caller's frames carry no sums: manual mode takes none) */
+    const bool bursts = bursts_on(c) && (after_batch || final);
+    if (bursts) TRY(burst_alloc(c));
+    if (quality) TRY(qual_alloc(c));
     if (any_sync) {
         K3Params p;
         memset(&p, 0, sizeof(p));
@@ -1605,6 +1655,7 @@ static int enqueue_gather(wmb_ctx *c, bool final, bool after_batch)
                 const int k = ch * WMB_N_ALGOS + a;
                 p.ring[k] = s.ring; p.ring_mask[k] = s.ring_cap - 1; p.sd[k] = s.sd; p.cand[k] = s.cand; p.pend[k] = s.pend;
                 p.pend_ofs[k] = s.pend_ofs;
+                if (quality) p.pend_qual[k] = s.pend_qual;
             }
             p.dphi[ch] = c->cb[ch].set[c->last_set].dphi;
         }
@@ -1618,6 +1669,7 @@ static int enqueue_gather(wmb_ctx *c, bool final, bool after_batch)
         p.words = c->d_words; p.words_cap = c->frame_words_cap;
         p.cut_n = c->d_cut_n; p.agg = c->d_k3_agg; p.errors = c->d_errors;
         p.final = final ? 1u : 0u;
+        if (quality) { p.qual_log = c->d_qual; p.qual_skip = c->o.accurate_atan ? 0u : 1u; }
         K4Params q;
         memset(&q, 0, sizeof(q));
         q.hdr = c->d_hdr; q.words = c->d_words; q.dec = c->d_dec;
@@ -1627,22 +1679,25 @@ static int enqueue_gather(wmb_ctx *c, bool final, bool after_batch)
          * produces more, is fetched when the record has been read) */
         CUDA_TRY(cudaMemcpyAsync(c->h_rec + slot, c->d_rec + slot, sizeof(BatchRec), cudaMemcpyDeviceToHost, c->cs));
         CUDA_TRY(cudaMemcpyAsync(c->h_hdr + lb, c->d_hdr + lb, (size_t)c->spec_n * sizeof(FrameHdr), cudaMemcpyDeviceToHost, c->cs));
+        if (quality)
+            CUDA_TRY(cudaMemcpyAsync(c->h_qual + lb, c->d_qual + lb, (size_t)c->spec_n * sizeof(QualAcc), cudaMemcpyDeviceToHost, c->cs));
         if (!c->manual) {
             CUDA_TRY(cudaMemcpyAsync(c->h_dec + lb, c->d_dec + lb, (size_t)c->spec_n * sizeof(DecHdr), cudaMemcpyDeviceToHost, c->cs));
             CUDA_TRY(cudaMemcpyAsync(c->h_pool + pb, c->d_pool + pb, c->spec_pool, cudaMemcpyDeviceToHost, c->cs));
         }
     }
     /* the burst report: behind the demod kernel of the batch (cs waited for it), before ev_chain[set] releases the set */
-    const bool bursts = bursts_on(c) && (after_batch || final);
+    const bool bqual = bursts && c->quality;
     if (bursts) {
-        TRY(burst_alloc(c));
         for (int ch = 0; ch < WMB_N_CHAINS; ch++) {
             if (!c->burst_level[ch] || !(c->chains & (1u << ch))) continue;
             const wmb_ctx::BurstBuf &b = c->bb[ch];
             BurstParams p;
             memset(&p, 0, sizeof(p));
             const SetBuf &sb = c->cb[ch].set[c->last_set];
-            p.rssi = sb.rssi + c->W; p.dphi = sb.dphi + c->W;
+            /* batch sample 0 = decimated sample m_first; the end-of-input gather (M = 0) comes after the last batch, whose
+             * set ends at m_first: the quality pass may read the window of a piece closed there out of that set */
+            p.rssi = sb.rssi + c->W; p.dphi = sb.dphi + c->W + (after_batch ? 0 : c->last_M);
             p.M = after_batch ? c->last_M : 0;
             p.clip = c->last_hist;
             p.m_first = (int64_t)(c->m_consumed - (uint64_t)p.M);
@@ -1651,6 +1706,10 @@ static int enqueue_gather(wmb_ctx *c, bool final, bool after_batch)
             p.mask = b.mask; p.cnt = b.cnt; p.base = b.base; p.ev = b.ev; p.bd = b.bd; p.items = b.items;
             p.out = c->d_brec + ((size_t)slot * WMB_N_CHAINS + ch) * c->burst_cap;
             p.slot = c->d_bslot + slot;
+            if (bqual) {
+                p.qout = c->d_bqual + ((size_t)slot * WMB_N_CHAINS + ch) * c->burst_cap;
+                p.qual_skip = c->o.accurate_atan ? 0u : 1u;
+            }
             TRY(launch_bursts(c, p, b.agg));
         }
         CUDA_TRY(cudaMemcpyAsync(c->h_bslot + slot, c->d_bslot + slot, sizeof(BurstSlot), cudaMemcpyDeviceToHost, c->cs));
@@ -1658,6 +1717,8 @@ static int enqueue_gather(wmb_ctx *c, bool final, bool after_batch)
             if (!c->burst_level[ch] || !(c->chains & (1u << ch))) continue;
             const size_t at = ((size_t)slot * WMB_N_CHAINS + ch) * c->burst_cap;
             CUDA_TRY(cudaMemcpyAsync(c->h_brec + at, c->d_brec + at, (size_t)c->burst_spec * sizeof(BurstRec), cudaMemcpyDeviceToHost, c->cs));
+            if (bqual)
+                CUDA_TRY(cudaMemcpyAsync(c->h_bqual + at, c->d_bqual + at, (size_t)c->burst_spec * sizeof(QualAcc), cudaMemcpyDeviceToHost, c->cs));
         }
     }
     /* the band survey: the rows the batch closed (its kernels ran on the demod stream), or at the end of input the
@@ -1711,12 +1772,14 @@ static int enqueue_gather(wmb_ctx *c, bool final, bool after_batch)
     f.slot = slot; f.final = final; f.has_timers = after_batch; f.m_end = c->m_consumed; f.bursts = bursts;
     f.burst_spec = c->burst_spec;                    /* records the copies above fetched (burst_spec may grow before they are read) */
     f.spec = spec;
+    f.quality = quality && any_sync; f.bquality = bqual;
     c->inflight.push_back(f);
     c->gather_no++;
     return WMB_OK;
 }
 
-static int book_device_frames(wmb_ctx *c, const FrameHdr *hdr, const DecHdr *dec, const uint8_t *pool, size_t n, bool final);
+static int book_device_frames(wmb_ctx *c, const FrameHdr *hdr, const DecHdr *dec, const QualAcc *qual, const uint8_t *pool,
+                              size_t n, bool final);
 
 /* Wait for the oldest gathered batch's results (an event, not a stream: later batches keep running), fetch what the
  * prefix copy did not cover, and run the stream-order bookkeeping over it. */
@@ -1740,7 +1803,7 @@ static int consume_oldest(wmb_ctx *c)
         /* the whole per-sample pass of the push so far: first demod kernel -> this batch's last bit-sync kernel */
         if (cudaEventElapsedTime(&ms, c->ev_push_start, evt[3]) == cudaSuccess) c->acc_pass_ms = ms;
     }
-    if (f.bursts) TRY(book_bursts(c, f.slot, f.m_end, f.burst_spec));
+    if (f.bursts) TRY(book_bursts(c, f.slot, f.m_end, f.burst_spec, f.bquality));
     if (f.spec) {                                    /* the slot's survey rows -> the queue */
         const std::vector<wmb_spectrum_row> &rows = c->spec_slot_rows[f.slot];
         const size_t at = (size_t)f.slot * c->spec_cap, n = rows.size() * (size_t)c->spec_bins;
@@ -1765,6 +1828,7 @@ static int consume_oldest(wmb_ctx *c)
     if (r.n > c->spec_n) {
         CUDA_TRY(cudaMemcpyAsync(c->h_hdr + lb + c->spec_n, c->d_hdr + lb + c->spec_n, (size_t)(r.n - c->spec_n) * sizeof(FrameHdr), cudaMemcpyDeviceToHost, c->xs));
         if (dev_decode) CUDA_TRY(cudaMemcpyAsync(c->h_dec + lb + c->spec_n, c->d_dec + lb + c->spec_n, (size_t)(r.n - c->spec_n) * sizeof(DecHdr), cudaMemcpyDeviceToHost, c->xs));
+        if (f.quality) CUDA_TRY(cudaMemcpyAsync(c->h_qual + lb + c->spec_n, c->d_qual + lb + c->spec_n, (size_t)(r.n - c->spec_n) * sizeof(QualAcc), cudaMemcpyDeviceToHost, c->xs));
         more = true;
     }
     if (dev_decode && r.pool_n > c->spec_pool) {
@@ -1781,6 +1845,7 @@ static int consume_oldest(wmb_ctx *c)
     if (r.n > c->spec_n) c->spec_n = std::min<uint32_t>(c->slot_cap, r.n + r.n / 4 + 256);
     if (r.pool_n > c->spec_pool) c->spec_pool = std::min<uint32_t>(c->slot_pool, r.pool_n + r.pool_n / 4 + 4096);
     c->st.d2h_bytes += sizeof(BatchRec) + (size_t)r.n * sizeof(FrameHdr) + (dev_decode ? (size_t)r.n * sizeof(DecHdr) + r.pool_n : 0);
+    if (f.quality) c->st.d2h_bytes += (size_t)r.n * sizeof(QualAcc);
     /* statistics kept on the device */
     c->st.lanes_rerun += r.lanes_rerun - c->stat_rerun_seen; c->st.lanes_run += r.lanes_rerun - c->stat_rerun_seen;
     c->stat_rerun_seen = r.lanes_rerun;
@@ -1802,7 +1867,7 @@ static int consume_oldest(wmb_ctx *c)
      * congruent to it that is not beyond the samples produced when the batch was gathered */
     for (uint32_t i = 0; i < r.n; i++) hdr[i].sync_sample = f.m_end - ((f.m_end - hdr[i].sync_sample) & EVG_M_MASK);
     int rc = WMB_OK;
-    if (dev_decode) rc = book_device_frames(c, hdr, c->h_dec + lb, c->h_pool + pb, r.n, f.final);
+    if (dev_decode) rc = book_device_frames(c, hdr, c->h_dec + lb, f.quality ? c->h_qual + lb : nullptr, c->h_pool + pb, r.n, f.final);
     else {
         /* manual mode: keep the frames (newest version of a re-delivered partial one wins) for wmb_poll */
         for (uint32_t i = 0; i < r.n; i++) {
@@ -2042,7 +2107,8 @@ extern "C" int wmb_poll(wmb_ctx *c, wmb_frame *out, size_t cap, size_t *n, int f
  * that is receiving ignores further access-code matches (t1_c1_packet_decoder.h:272-278 honours the
  * flag only in idle), so a candidate inside the telegram of an earlier one is dropped; the rest
  * become lines, queued in the order the reference prints them. */
-struct FrameMeta { uint8_t chain, algo, partial, truncated, ofs_valid; uint64_t ordinal, sync_sample; int64_t ofs_sum; uint32_t ofs_n; };
+struct FrameMeta { uint8_t chain, algo, partial, truncated, ofs_valid; uint64_t ordinal, sync_sample; int64_t ofs_sum; uint32_t ofs_n;
+                   const QualAcc *qual; /* null: no quality sums */ };
 struct DecLite { int status; uint32_t consumed; uint64_t end_sample; uint8_t crc_ok; };
 
 template <class Meta, class Lite, class Fill>
@@ -2107,13 +2173,15 @@ static int book_frames(wmb_ctx *c, size_t n, Meta meta, Lite lite, Fill fill)
         const FrameMeta m = meta(fresh[i].fi);
         q.chain = m.chain; q.sync_sample = m.sync_sample;
         q.ofs_valid = m.ofs_valid; q.ofs_sum = m.ofs_sum; q.ofs_n = m.ofs_n;
+        if (m.qual) q.qual = *m.qual; else qual_zero(q.qual);
         fill(fresh[i].fi, q.d);
     }
     return WMB_OK;
 }
 
 /* candidates of one gathered batch, decoded by K4 (already in stream order) */
-static int book_device_frames(wmb_ctx *c, const FrameHdr *hdr, const DecHdr *dec, const uint8_t *pool, size_t n, bool final)
+static int book_device_frames(wmb_ctx *c, const FrameHdr *hdr, const DecHdr *dec, const QualAcc *qual, const uint8_t *pool,
+                              size_t n, bool final)
 {
     static const char modes[3][3] = { "T1", "C1", "S1" };
     /* frames without any bit (candidate at the very end of the stream) are not decoded at all */
@@ -2126,6 +2194,7 @@ static int book_device_frames(wmb_ctx *c, const FrameHdr *hdr, const DecHdr *dec
             FrameMeta m;
             m.chain = h.chain; m.algo = h.algo; m.ordinal = h.ordinal; m.sync_sample = h.sync_sample;
             m.ofs_valid = 1; m.ofs_sum = h.ofs_sum; m.ofs_n = h.ofs_n;
+            m.qual = qual ? qual + idx[k] : nullptr;
             m.partial = (uint8_t)((!h.complete && !final) ? 1 : 0);
             m.truncated = (uint8_t)((h.complete && !h.cut) ? 0 : 1);
             return m;
@@ -2230,6 +2299,7 @@ extern "C" int wmb_decode_frames(wmb_ctx *c, const wmb_frame *frames, size_t n)
             m.chain = v[i]->chain; m.algo = v[i]->algo; m.ordinal = v[i]->ordinal; m.sync_sample = v[i]->sync_sample;
             m.partial = v[i]->reserved; m.truncated = v[i]->truncated;
             m.ofs_valid = 0; m.ofs_sum = 0; m.ofs_n = 0;                   /* a caller's frame carries no sum */
+            m.qual = nullptr;
             return m;
         },
         [&](size_t i) {
@@ -2240,15 +2310,30 @@ extern "C" int wmb_decode_frames(wmb_ctx *c, const wmb_frame *frames, size_t n)
         [&](size_t i, wmb_decoded &o) { o = dec[i]; });
 }
 
-extern "C" size_t wmb_take_lines_info(wmb_ctx *c, char *buf, size_t cap, size_t *n_lines, int timestamp_mode,
-                                      wmb_line_info *info, size_t info_cap)
+/* deviation and eye SNR from the class sums (wmb_line_quality); returns valid */
+static uint8_t qual_derive(const QualAcc &q, bool ok, double fir_gain, double *deviation_hz, double *eye_snr_db)
+{
+    *deviation_hz = NAN; *eye_snr_db = NAN;
+    if (!ok || q.n_hi < 2 || q.n_lo < 2) return 0;
+    const double nh = (double)q.n_hi, nl = (double)q.n_lo;
+    const double mh = (double)q.s1_hi / nh, ml = (double)q.s1_lo / nl;
+    const double var = ((double)q.s2_hi - nh * mh * mh + (double)q.s2_lo - nl * ml * ml) / (nh + nl - 2.0);
+    if (!(var > 0.0)) return 0;
+    const double half = (mh - ml) / 2.0;
+    *deviation_hz = half / (double)WMB_OFS_SCALE * 400e3 / fir_gain;
+    *eye_snr_db = 10.0 * log10(half * half / var);
+    return 1;
+}
+
+extern "C" size_t wmb_take_lines_quality(wmb_ctx *c, char *buf, size_t cap, size_t *n_lines, int timestamp_mode,
+                                         wmb_line_info *info, wmb_line_quality *qual, size_t rec_cap)
 {
     size_t len = 0, taken = 0;
     if (n_lines) *n_lines = 0;
     if (!c || !buf) return 0;
     char ts[64];
     for (; taken < c->lines.size(); taken++) {
-        if (info && taken >= info_cap) break;
+        if ((info || qual) && taken >= rec_cap) break;
         const QueuedLine &q = c->lines[taken];
         if (timestamp_mode == 1) snprintf(ts, sizeof(ts), "TS");
         else if (timestamp_mode == 2) snprintf(ts, sizeof(ts), "@%014llu.%d", (unsigned long long)q.end_sample, q.prio);
@@ -2270,11 +2355,31 @@ extern "C" size_t wmb_take_lines_info(wmb_ctx *c, char *buf, size_t cap, size_t 
             r.carrier_hz = chain_carrier_hz(c, q.chain);
             r.offset_hz = r.valid ? (double)q.ofs_sum / (double)q.ofs_n / (double)WMB_OFS_SCALE * 400e3 / c->fir_gain[q.chain] : NAN;
         }
+        if (qual) {
+            wmb_line_quality &r = qual[taken];
+            memset(&r, 0, sizeof(r));
+            r.sync_sample = q.sync_sample; r.end_sample = q.end_sample;
+            r.chain = q.chain; r.algo = q.algo; r.crc_ok = q.d.crc_ok;
+            r.n_hi = q.qual.n_hi; r.n_lo = q.qual.n_lo; r.s1_hi = q.qual.s1_hi; r.s1_lo = q.qual.s1_lo;
+            r.s2_hi = q.qual.s2_hi; r.s2_lo = q.qual.s2_lo;
+            r.bits = q.d.consumed;
+            /* -a: the cross-product discriminator is not a frequency; a caller's frame carries no sums */
+            r.valid = qual_derive(q.qual, q.ofs_valid && c->o.accurate_atan, c->fir_gain[q.chain], &r.deviation_hz,
+                                  &r.eye_snr_db);
+            r.chip_rate_hz = (r.bits >= 2 && q.end_sample > q.sync_sample)
+                ? 800e3 * (double)(r.bits - 1) / (double)(q.end_sample - q.sync_sample) : NAN;
+        }
     }
     if (len < cap) buf[len] = 0;
     c->lines.erase(c->lines.begin(), c->lines.begin() + (long)taken);
     if (n_lines) *n_lines = taken;
     return len;
+}
+
+extern "C" size_t wmb_take_lines_info(wmb_ctx *c, char *buf, size_t cap, size_t *n_lines, int timestamp_mode,
+                                      wmb_line_info *info, size_t info_cap)
+{
+    return wmb_take_lines_quality(c, buf, cap, n_lines, timestamp_mode, info, nullptr, info_cap);
 }
 
 extern "C" size_t wmb_take_lines(wmb_ctx *c, char *buf, size_t cap, size_t *n_lines, int timestamp_mode)
@@ -2406,19 +2511,44 @@ extern "C" int wmb_set_bursts(wmb_ctx *c, int chain, uint32_t level)
     return WMB_OK;
 }
 
-extern "C" int wmb_take_bursts(wmb_ctx *c, wmb_burst *out, size_t cap, size_t *n)
+extern "C" int wmb_take_bursts_quality(wmb_ctx *c, wmb_burst *out, wmb_burst_quality *qual, size_t cap, size_t *n)
 {
     if (!c || !n || (!out && cap)) return set_err(WMB_E_INVAL, "null argument");
     /* per chain the queue is in start order (pieces of a chain are disjoint and close in order); across chains a
      * piece closed later may start earlier */
-    std::stable_sort(c->bursts.begin(), c->bursts.end(), [](const wmb_burst &a, const wmb_burst &b) {
-        return a.start_sample != b.start_sample ? a.start_sample < b.start_sample : a.chain < b.chain;
+    std::stable_sort(c->bursts.begin(), c->bursts.end(), [](const QueuedBurst &a, const QueuedBurst &b) {
+        return a.b.start_sample != b.b.start_sample ? a.b.start_sample < b.b.start_sample : a.b.chain < b.b.chain;
     });
     size_t k = 0;
-    while (k < cap && k < c->bursts.size() && c->bursts[k].start_sample < c->burst_frontier) k++;
-    if (k) memcpy(out, c->bursts.data(), k * sizeof(wmb_burst));
+    while (k < cap && k < c->bursts.size() && c->bursts[k].b.start_sample < c->burst_frontier) k++;
+    for (size_t i = 0; i < k; i++) {
+        const QueuedBurst &qb = c->bursts[i];
+        out[i] = qb.b;
+        if (!qual) continue;
+        wmb_burst_quality &r = qual[i];
+        memset(&r, 0, sizeof(r));
+        r.start_sample = qb.b.start_sample; r.chain = qb.b.chain;
+        r.n_hi = qb.q.n_hi; r.n_lo = qb.q.n_lo; r.s1_hi = qb.q.s1_hi; r.s1_lo = qb.q.s1_lo;
+        r.s2_hi = qb.q.s2_hi; r.s2_lo = qb.q.s2_lo;
+        r.valid = qual_derive(qb.q, c->o.accurate_atan != 0, c->fir_gain[qb.b.chain], &r.deviation_hz, &r.eye_snr_db);
+    }
     c->bursts.erase(c->bursts.begin(), c->bursts.begin() + (long)k);
     *n = k;
+    return WMB_OK;
+}
+
+extern "C" int wmb_take_bursts(wmb_ctx *c, wmb_burst *out, size_t cap, size_t *n)
+{
+    return wmb_take_bursts_quality(c, out, nullptr, cap, n);
+}
+
+extern "C" int wmb_set_line_quality(wmb_ctx *c, int on)
+{
+    if (!c) return set_err(WMB_E_INVAL, "null argument");
+    if (on != 0 && on != 1) return set_err(WMB_E_INVAL, "line quality %d: 0 (off) or 1 (on)", on);
+    if (c->batch_no != 0 || !c->remainder.empty())
+        return set_err(WMB_E_STATE, "wmb_set_line_quality after samples were pushed (call it before the first push or after wmb_reset / wmb_seek)");
+    c->quality = on != 0;
     return WMB_OK;
 }
 

@@ -892,6 +892,46 @@ struct OfsAcc {                     /* a carried candidate's sum (beside its ord
     uint32_t pad;
 };
 
+WMB_D int64_t wmb_ofs_x(float d)    /* one term of the offset sum: rint(dphi * 2^24) */
+{
+#ifdef WMB_HOSTSIM
+    return (int64_t)llrintf(d * WMB_OFS_SCALE);
+#else
+    return __float2ll_rn(d * WMB_OFS_SCALE);            /* 64-bit: -a's cross products reach 2^15 before scaling */
+#endif
+}
+
+/* Signal quality of an offset window (DESIGN §8, wmb_line_quality): sample q is high iff x[q] n >= sum (the window
+ * mean, no division); q in [lo + 1, hi - 1) counts iff q - 1, q, q + 1 share its class.  Per class: the counting
+ * samples, their sum and their sum of squares -- integers, exact in any order (|x| < 2^26, n <= 781: s2 < 2^63) */
+struct QualAcc {
+    uint32_t n_hi, n_lo;
+    int64_t  s1_hi, s1_lo;
+    uint64_t s2_hi, s2_lo;
+};
+
+WMB_HD void qual_zero(QualAcc &a) { a.n_hi = a.n_lo = 0; a.s1_hi = a.s1_lo = 0; a.s2_hi = a.s2_lo = 0; }
+WMB_HD void qual_add(QualAcc &a, const QualAcc &b)
+{
+    a.n_hi += b.n_hi; a.n_lo += b.n_lo; a.s1_hi += b.s1_hi; a.s1_lo += b.s1_lo; a.s2_hi += b.s2_hi; a.s2_lo += b.s2_lo;
+}
+
+/* thread t of nt: its share of the class sums over the window [lo, hi) of dphi (its n samples add up to sum).  Reads
+ * stay inside [lo, hi).  k3_fill and kb_reduce both take their sums here. */
+WMB_D void qual_part(const float *dphi, int64_t lo, int64_t hi, int64_t sum, int64_t n, uint32_t t, uint32_t nt,
+                     QualAcc &a)
+{
+    qual_zero(a);
+    for (int64_t q = lo + 1 + (int64_t)t; q < hi - 1; q += nt) {
+        const int64_t x0 = wmb_ofs_x(dphi[q - 1]), x = wmb_ofs_x(dphi[q]), x2 = wmb_ofs_x(dphi[q + 1]);
+        const bool c0 = x0 * n >= sum, c = x * n >= sum, c2 = x2 * n >= sum;
+        if (c0 != c || c2 != c) continue;                 /* a chip transition: the FIR's ramp between the tones */
+        const uint64_t sq = (uint64_t)(x * x);
+        if (c) { a.n_hi++; a.s1_hi += x; a.s2_hi += sq; }
+        else { a.n_lo++; a.s1_lo += x; a.s2_lo += sq; }
+    }
+}
+
 struct FrameHdr {                   /* one per candidate, device -> host                   */
     uint64_t ordinal;
     uint64_t sync_sample;
@@ -935,6 +975,10 @@ struct K3Params {
     const uint64_t *cand[WMB_N_STREAMS];   /* new matches, unordered                        */
     uint64_t *pend[WMB_N_STREAMS];  /* carried candidates, ordered                          */
     OfsAcc *pend_ofs[WMB_N_STREAMS];/* their carrier-offset sums, same slots                */
+    /* line quality (wmb_set_line_quality): null when off -- nothing below reads or writes them then */
+    QualAcc *pend_qual[WMB_N_STREAMS];   /* carried candidates' class sums, same slots as pend   */
+    QualAcc *qual_log;              /* one per candidate, parallel to hdr_log               */
+    uint32_t qual_skip;             /* 1 (-a): the records hold zero sums                   */
     uint32_t pend_cap, cand_cap;
     /* the carrier-offset windows of new matches are read from this batch's dphi set: [prefix | batch_m samples], batch
      * sample 0 = decimated sample m_first (40 bits); `clip` samples before it exist since the last reset / seek */
@@ -1041,20 +1085,31 @@ WMB_D void k3_fill(const K3Params &p, uint32_t i, uint32_t part, uint32_t nparts
     }
     const float *dphi = fresh ? p.dphi[chain] + p.prefix : nullptr;
     int64_t sum = 0;
-    for (int64_t q = lo + (int64_t)part; q < hi; q += nparts) {
-#ifdef WMB_HOSTSIM
-        sum += (int64_t)llrintf(dphi[q] * WMB_OFS_SCALE);
-#else
-        sum += __float2ll_rn(dphi[q] * WMB_OFS_SCALE);    /* 64-bit: -a's cross products reach 2^15 before scaling */
-#endif
-    }
+    for (int64_t q = lo + (int64_t)part; q < hi; q += nparts) sum += wmb_ofs_x(dphi[q]);
 #ifndef WMB_HOSTSIM
     for (uint32_t d = nparts >> 1; d > 0; d >>= 1) {
         rank += __shfl_xor_sync(0xFFFFFFFFu, rank, d);
         sum += __shfl_xor_sync(0xFFFFFFFFu, sum, d);
     }
 #endif
+    /* line quality: a second pass over the same window, classed against the mean the shuffles just gave every part */
+    QualAcc qa;
+    qual_zero(qa);
+    if (p.qual_log) {
+        if (!p.qual_skip) qual_part(dphi, lo, hi, sum, hi - lo, part, nparts, qa);
+#ifndef WMB_HOSTSIM
+        for (uint32_t d = nparts >> 1; d > 0; d >>= 1) {
+            qa.n_hi += __shfl_xor_sync(0xFFFFFFFFu, qa.n_hi, d);
+            qa.n_lo += __shfl_xor_sync(0xFFFFFFFFu, qa.n_lo, d);
+            qa.s1_hi += __shfl_xor_sync(0xFFFFFFFFu, qa.s1_hi, d);
+            qa.s1_lo += __shfl_xor_sync(0xFFFFFFFFu, qa.s1_lo, d);
+            qa.s2_hi += __shfl_xor_sync(0xFFFFFFFFu, (unsigned long long)qa.s2_hi, d);
+            qa.s2_lo += __shfl_xor_sync(0xFFFFFFFFu, (unsigned long long)qa.s2_lo, d);
+        }
+#endif
+    }
     if (!live || part != 0) return;
+    if (p.qual_log) p.qual_log[g.base + g.off[k] + rank] = fresh ? qa : p.pend_qual[k][j];
     FrameHdr h;
     h.ordinal = key; h.sync_sample = 0; h.nbits = 0; h.word_off = 0; h.complete = 0; h.overflow = 0; h.cut = 0;
     h.pad = 0;
@@ -1234,6 +1289,7 @@ WMB_D void k3_carry(const K3Params &p, uint32_t i)
         p.pend[k][slot] = h.ordinal;
         OfsAcc a; a.sum = h.ofs_sum; a.n = h.ofs_n; a.pad = 0;
         p.pend_ofs[k][slot] = a;
+        if (p.qual_log) p.pend_qual[k][slot] = p.qual_log[g.base + i];
     }
     else k3_flag(p.errors, 64u);
 }

@@ -62,21 +62,26 @@ def blank_position(line: str) -> str:
     return ";".join(f)
 
 
-def merge_lines(parts, infos=None):
+def merge_lines(parts, infos=None, quals=None):
     """Lines of several time chunks (each taken with timestamp_mode=2) -> the sequential run's print order, with the
     TIMESTAMP column blanked.  Within one chunk the order is already right; across chunks a telegram that started in
     chunk g may finish after one that started in chunk g+1, so the merge is by print position (stable).
     infos: the chunks' line records (numpy arrays of wmb_line_info, one per line): returns (lines, records) then, the
-    records in the same order."""
+    records in the same order.  quals: the chunks' wmb_line_quality records, likewise: (lines[, records], quality)."""
     flat = [l for part in parts for l in part]
     order = sorted(range(len(flat)), key=lambda i: line_key(flat[i]))
     lines = [blank_position(flat[i]) for i in order]
-    if infos is None:
+    if infos is None and quals is None:
         return lines
     import numpy as np
-    recs = np.concatenate(infos)
-    assert len(recs) == len(flat), "one record per line"
-    return lines, recs[np.asarray(order, np.int64)]
+    out = [lines]
+    for arrs in (infos, quals):
+        if arrs is None:
+            continue
+        recs = np.concatenate(arrs)
+        assert len(recs) == len(flat), "one record per line"
+        out.append(recs[np.asarray(order, np.int64)])
+    return tuple(out)
 
 
 def chunk_bounds(n_bytes: int, d: int, world: int):
@@ -86,12 +91,18 @@ def chunk_bounds(n_bytes: int, d: int, world: int):
     return [min(n_iq, (n_iq * g // world) // gran * gran) for g in range(world)] + [n_iq]
 
 
-def merge_bursts(parts):
+def merge_bursts(parts, quals=None):
     """Burst records (wmb_burst arrays) of several time chunks, each holding the pieces that start in its chunk ->
-    the sequential run's records, ordered by (start_sample, chain)."""
+    the sequential run's records, ordered by (start_sample, chain).  quals: the chunks' wmb_burst_quality records, one
+    per burst: returns (records, quality) then."""
     import numpy as np
     recs = np.concatenate(parts)
-    return recs[np.lexsort((recs["chain"], recs["start_sample"]))]
+    order = np.lexsort((recs["chain"], recs["start_sample"]))
+    if quals is None:
+        return recs[order]
+    q = np.concatenate(quals)
+    assert len(q) == len(recs), "one quality record per burst"
+    return recs[order], q[order]
 
 
 def merge_spectrum(parts):
@@ -164,7 +175,7 @@ def find_carriers(rows, sum, peak, fs: float, threshold_db: float = 15.0, bridge
 
 
 def decode_time_chunk(ctx, push, n_bytes: int, d: int, rank: int, world: int, halo_m: int = 1 << 18, info=False,
-                      bursts=False, spectrum=False):
+                      bursts=False, spectrum=False, quality=False):
     """Decode rank `rank`'s chunk of a capture of n_bytes cu8 bytes.  `push(byte_lo, byte_hi)` feeds that byte
     range of the capture to ctx (host or device memory: the caller's business).
     Returns (lines, digest_start, digest_end, halo_start_iq): digest_start is None for a chunk that starts at 0.
@@ -176,10 +187,15 @@ def decode_time_chunk(ctx, push, n_bytes: int, d: int, rank: int, world: int, ha
     (DESIGN.md §8), inside the left halo, and one that starts before hi is closed within as many samples after hi, inside
     the right halo, so they are the sequential run's pieces.
     spectrum=True (ctx made with spectrum=...): the band survey's records (rows, sum, peak) come last in lines.  The line
-    window counts the chunk's blocks only, so merge_spectrum() over the chunks gives the sequential records."""
+    window counts the chunk's blocks only, so merge_spectrum() over the chunks gives the sequential records.
+    quality=True (ctx made with quality=True): the lines' wmb_line_quality records follow the line records, and with
+    bursts=True the bursts' wmb_burst_quality records follow the bursts: (lines[, records], quality[, bursts,
+    burst_quality][, spectrum]).  Their windows are the offset windows, so they are the sequential run's as well."""
     import hashlib
     recs = []
+    qrecs = []
     brecs = []
+    bqrecs = []
     srecs = []
 
     def take_s():
@@ -187,10 +203,19 @@ def decode_time_chunk(ctx, push, n_bytes: int, d: int, rank: int, world: int, ha
             srecs.append(ctx.take_spectrum())
 
     def take_b():
-        if bursts:
+        if bursts and quality:
+            b, q = ctx.take_bursts(quality=True)
+            brecs.append(b)
+            bqrecs.append(q)
+        elif bursts:
             brecs.append(ctx.take_bursts())
 
     def take():
+        if quality:
+            got = ctx.take_lines(2, info=True, quality=True)
+            recs.append(got[1])
+            qrecs.append(got[2])
+            return got[0]
         if not info:
             return ctx.take_lines(2)
         got, r = ctx.take_lines(2, info=True)
@@ -235,26 +260,29 @@ def decode_time_chunk(ctx, push, n_bytes: int, d: int, rank: int, world: int, ha
     lines += take()
     take_b()
     take_s()
+    import numpy as np
+    out = [lines]
     if info:
-        import numpy as np
-        lines = (lines, np.concatenate(recs))
+        out.append(np.concatenate(recs))
+    if quality:
+        out.append(np.concatenate(qrecs))
     if bursts:
-        import numpy as np
         b = np.concatenate(brecs)
         m_lo, m_hi = lo // d, (hi // d if rank + 1 < world else 1 << 63)
-        b = b[(b["start_sample"] >= m_lo) & (b["start_sample"] < m_hi)]
-        lines = (lines + (b,)) if info else (lines, b)
+        keep = (b["start_sample"] >= m_lo) & (b["start_sample"] < m_hi)
+        out.append(b[keep])
+        if quality:
+            out.append(np.concatenate(bqrecs)[keep])
     if spectrum:
-        import numpy as np
         srecs = [x for x in srecs if len(x[0])] or srecs[:1]
-        sp = (np.concatenate([x[0] for x in srecs]), np.concatenate([x[1] for x in srecs]),
-              np.concatenate([x[2] for x in srecs]))
-        lines = (lines + (sp,)) if isinstance(lines, tuple) else (lines, sp)
+        out.append((np.concatenate([x[0] for x in srecs]), np.concatenate([x[1] for x in srecs]),
+                    np.concatenate([x[2] for x in srecs])))
+    lines = tuple(out) if len(out) > 1 else lines
     return lines, dig_start, dig_end, start
 
 
 def decode_time_sharded(ctx, push, n_bytes: int, d: int, halo_m: int = 1 << 18, info=False, bursts=False,
-                        spectrum=False):
+                        spectrum=False, quality=False):
     """All ranks: decode one capture in time chunks, exact by construction (see module docstring).
     Returns (my_lines, rounds); info=True / bursts=True: my_lines carries the records / burst pieces as in
     decode_time_chunk."""
@@ -267,7 +295,7 @@ def decode_time_sharded(ctx, push, n_bytes: int, d: int, halo_m: int = 1 << 18, 
         rounds += 1
         if redo:
             lines, ds, de, start = decode_time_chunk(ctx, push, n_bytes, d, rank, world, halo_m, info=info, bursts=bursts,
-                                                        spectrum=spectrum)
+                                                        spectrum=spectrum, quality=quality)
         mine = torch.zeros(65, dtype=torch.uint8)
         mine[:32] = torch.frombuffer(bytearray(ds or bytes(32)), dtype=torch.uint8)
         mine[32:64] = torch.frombuffer(bytearray(de), dtype=torch.uint8)
