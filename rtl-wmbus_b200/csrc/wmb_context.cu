@@ -116,6 +116,36 @@ struct ChainBuf {
 
 #define WMB_NSLOT 4                      /* batches whose results may be waiting for the host */
 
+/* One kind of per-batch result: a device array of WMB_NSLOT x parts x cap elements and its pinned host mirror.  The
+ * copy enqueued behind a gather fetches a prefix of each (slot, part), since the host cannot know yet how many elements
+ * the batch wrote.  Once the count has been read the host fetches the rest and grows the prefix so that later batches
+ * fit it.  Several gathers are in flight at once, so the rest of a slot starts at what that slot's own copy fetched
+ * (wmb_ctx::InFlight), never at the current prefix, which may have grown since. */
+template <typename T> struct SlotTable {
+    T *d = nullptr, *h = nullptr;
+    size_t cap = 0;                 /* elements per slot and part */
+    uint32_t parts = 1;
+    uint32_t prefix = 0;            /* elements the next prefix copy fetches */
+    uint32_t slack = 0;             /* growth beyond n + n / 4 */
+
+    size_t at(int slot, int part = 0) const { return ((size_t)slot * parts + part) * cap; }
+    int alloc(wmb_ctx *c, uint32_t n_parts, size_t n_cap, uint32_t first_prefix, uint32_t grow_slack);
+    int release(wmb_ctx *c);
+    /* elements [copied, n) of (slot, part) on st when n > copied; sets *issued (if given) when it copies */
+    int fetch(int slot, int part, uint32_t copied, uint32_t n, cudaStream_t st, bool *issued = nullptr) const
+    {
+        if (n <= copied) return WMB_OK;
+        if (n > cap) return set_err(WMB_E_STATE, "internal: batch results beyond their slot table");
+        const size_t i = at(slot, part) + copied;
+        CUDA_TRY(cudaMemcpyAsync(h + i, d + i, (size_t)(n - copied) * sizeof(T), cudaMemcpyDeviceToHost, st));
+        if (issued) *issued = true;
+        return WMB_OK;
+    }
+    /* the prefix copy of (slot, part) on st; *copied: the elements it fetches */
+    int enqueue(int slot, int part, cudaStream_t st, uint32_t *copied) const { *copied = prefix; return fetch(slot, part, 0, prefix, st); }
+    void grow(uint32_t n) { if (n > prefix) prefix = (uint32_t)std::min<size_t>(cap, (size_t)n + n / 4 + slack); }
+};
+
 static uint32_t g_p2_block = 128u;       /* threads per block of the phase-2 count pass (WMBUS_B200_P2BLK, experiments) */
 
 struct QueuedLine {
@@ -196,16 +226,16 @@ struct wmb_ctx {
     /* results: WMB_NSLOT slots, one per batch in flight, each with its part of the candidate / verdict arrays and of
      * the datagram pool; the host mirrors are pinned and filled by copies enqueued right behind the device framer */
     BatchRec *d_rec = nullptr, *h_rec = nullptr;
-    FrameHdr *d_hdr = nullptr, *h_hdr = nullptr;
-    DecHdr *d_dec = nullptr, *h_dec = nullptr;
-    uint8_t *d_pool = nullptr, *h_pool = nullptr;
-    uint32_t slot_cap = 0, slot_pool = 0, pend_cap = 0;
+    SlotTable<FrameHdr> hdr;
+    SlotTable<DecHdr> dec;
+    SlotTable<uint8_t> pool;
+    uint32_t pend_cap = 0;
     uint32_t *d_words = nullptr, *h_words = nullptr;
     uint32_t *d_cut_n = nullptr;
     uint64_t *d_k3_agg = nullptr;
-    uint32_t spec_n = 0, spec_pool = 0;              /* entries / bytes copied before their counts are known */
-    struct InFlight { int slot; bool final; bool has_timers; uint64_t m_end; bool bursts; uint32_t burst_spec; bool spec;
-                      bool quality, bquality; };
+    /* a gathered batch; per table, the elements its prefix copy fetched (0: the table was not copied) */
+    struct InFlight { int slot; bool final; bool has_timers; uint64_t m_end;
+                      uint32_t hdr, dec, qual, pool, brec, bqual, ssum, speak; };
     std::vector<InFlight> inflight;                  /* gathered batches whose results the host has not read yet */
     uint64_t stat_rerun_seen = 0, stat_fallback_seen = 0;
     double acc_demod_ms = 0, acc_bitsync_ms = 0, acc_pass_ms = 0;    /* timers of the current push */
@@ -233,27 +263,25 @@ struct wmb_ctx {
     struct BurstBuf { uint32_t *mask = nullptr, *cnt = nullptr; uint64_t *base = nullptr, *agg = nullptr; int64_t *ev = nullptr;
                       BurstDev *bd = nullptr; BurstItem *items = nullptr; } bb[WMB_N_CHAINS];
     bool burst_allocated = false;
-    uint32_t burst_cap = 0;                          /* records per slot and chain: pieces >= 256 samples of one batch */
-    uint32_t burst_spec = 64;                        /* records copied per slot and chain before their count is known */
-    BurstRec *d_brec = nullptr, *h_brec = nullptr;   /* [WMB_NSLOT][chain][burst_cap] */
+    SlotTable<BurstRec> brec;                        /* [WMB_NSLOT][chain][cap] */
     BurstSlot *d_bslot = nullptr, *h_bslot = nullptr;
     std::vector<QueuedBurst> bursts;                 /* closed pieces not taken yet */
     uint64_t burst_frontier = 0;                     /* no piece still to come starts before this sample */
 
     /* signal quality (wmb_set_line_quality; survives wmb_reset).  Off: nothing is allocated, launched or copied */
     bool quality = false;
-    bool qual_allocated = false;
-    QualAcc *d_qual = nullptr, *h_qual = nullptr;    /* [WMB_NSLOT * slot_cap], parallel to d_hdr / h_hdr */
-    QualAcc *d_bqual = nullptr, *h_bqual = nullptr;  /* [WMB_NSLOT][chain][burst_cap], parallel to d_brec / h_brec */
+    SlotTable<QualAcc> qual;                        /* parallel to hdr */
+    SlotTable<QualAcc> bqual;                        /* parallel to brec */
 
     /* band survey (wmb_set_spectrum; the setting survives wmb_reset).  Bins 0: off, nothing is allocated or launched */
     uint32_t spec_bins = 0, spec_B = 0;
     uint32_t spec_R = 0;                             /* ring rows = rows of a result slot: batch blocks / B + 2 */
-    size_t spec_cap = 0;                             /* bins the ring and each slot table hold as allocated */
     uint32_t spec_tab_n = 0;                         /* N of the tables on the device */
     float *d_spec_tab = nullptr;                     /* hann[N] | tw[N / 2][2] */
-    uint64_t *d_ssum_ring = nullptr, *d_ssum = nullptr, *h_ssum = nullptr;    /* ring [R][N]; slots [WMB_NSLOT][R][N] */
-    uint32_t *d_speak_ring = nullptr, *d_speak = nullptr, *h_speak = nullptr;
+    uint64_t *d_ssum_ring = nullptr;                 /* [R][N] */
+    uint32_t *d_speak_ring = nullptr;
+    SlotTable<uint64_t> ssum;                        /* [WMB_NSLOT][R][N] */
+    SlotTable<uint32_t> speak;
     cudaEvent_t ev_spec = nullptr;                   /* the batch's survey kernels are done (cs waits before its copies) */
     cudaEvent_t ev_spec_flush = nullptr;             /* the flush's close is done (the next batch's survey waits) */
     bool spec_flush_pending = false;
@@ -684,6 +712,33 @@ static int host_alloc(wmb_ctx *c, T **p, size_t count)
 
 #define TRY(expr) do { int _rc = (expr); if (_rc) return _rc; } while (0)
 
+static int mem_free(wmb_ctx *c, void *p, bool host)
+{
+    if (!p) return WMB_OK;
+    std::vector<void *> &v = host ? c->host_allocs : c->dev_allocs;
+    v.erase(std::remove(v.begin(), v.end(), p), v.end());
+    CUDA_TRY(host ? cudaFreeHost(p) : cudaFree(p));
+    return WMB_OK;
+}
+
+/* d and h are set only when both arrays exist */
+template <typename T>
+int SlotTable<T>::alloc(wmb_ctx *c, uint32_t n_parts, size_t n_cap, uint32_t first_prefix, uint32_t grow_slack)
+{
+    T *dd = nullptr, *hh = nullptr;
+    TRY(dev_alloc(c, &dd, (size_t)WMB_NSLOT * n_parts * n_cap));
+    TRY(host_alloc(c, &hh, (size_t)WMB_NSLOT * n_parts * n_cap));
+    d = dd; h = hh; parts = n_parts; cap = n_cap; slack = grow_slack; prefix = (uint32_t)std::min<size_t>(first_prefix, n_cap);
+    return WMB_OK;
+}
+
+template <typename T> int SlotTable<T>::release(wmb_ctx *c)
+{
+    TRY(mem_free(c, d, false)); TRY(mem_free(c, h, true));
+    d = h = nullptr; cap = 0;
+    return WMB_OK;
+}
+
 /* lane geometry of the run-length kernels; WMBUS_B200_TUNE="t2words:p1chunk:p2records" overrides it for experiments */
 static uint32_t g_p1_chunk = 2048u;      /* decimated samples per phase-1 run-length lane */
 static uint32_t g_p2_records = 512u;     /* records per phase-2 lane (nominal) */
@@ -767,23 +822,18 @@ static int ctx_alloc(wmb_ctx *c)
     TRY(dev_alloc(c, &c->d_errors, 16, true));
     c->d_nfail = c->d_errors + 4;
     TRY(dev_alloc(c, &c->d_gd, 1, true));
-    c->slot_cap = c->cand_cap;                   /* candidates of one batch */
     c->pend_cap = 1u << 16;                      /* candidates younger than one telegram at a batch end */
-    c->slot_pool = c->frame_words_cap / 8 + 4 * c->cand_cap;    /* a datagram byte takes >= 8 shipped bit words */
     TRY(dev_alloc(c, &c->d_rec, WMB_NSLOT, true));
-    TRY(dev_alloc(c, &c->d_hdr, (size_t)WMB_NSLOT * c->slot_cap));
-    TRY(dev_alloc(c, &c->d_dec, (size_t)WMB_NSLOT * c->slot_cap));
-    TRY(dev_alloc(c, &c->d_pool, (size_t)WMB_NSLOT * c->slot_pool));
     TRY(dev_alloc(c, &c->d_words, c->frame_words_cap));
     TRY(dev_alloc(c, &c->d_cut_n, c->cand_cap));
     TRY(dev_alloc(c, &c->d_k3_agg, SCAN_THREADS));
     TRY(host_alloc(c, &c->h_rec, WMB_NSLOT));
-    TRY(host_alloc(c, &c->h_hdr, (size_t)WMB_NSLOT * c->slot_cap));
-    TRY(host_alloc(c, &c->h_dec, (size_t)WMB_NSLOT * c->slot_cap));
-    TRY(host_alloc(c, &c->h_pool, (size_t)WMB_NSLOT * c->slot_pool));
     TRY(host_alloc(c, &c->h_words, c->frame_words_cap));
-    c->spec_n = std::min<uint32_t>(4096, c->slot_cap);          /* grows with what the batches actually produce (consume_oldest) */
-    c->spec_pool = std::min<uint32_t>(1u << 18, c->slot_pool);
+    /* a slot holds the candidates of one batch and their datagrams (a datagram byte takes >= 8 shipped bit words); the
+     * first prefix copies take 4096 candidates and 256 KiB of datagrams, and grow with what the batches produce */
+    TRY(c->hdr.alloc(c, 1, c->cand_cap, 4096, 256));
+    TRY(c->dec.alloc(c, 1, c->cand_cap, 4096, 256));
+    TRY(c->pool.alloc(c, 1, c->frame_words_cap / 8 + 4 * c->cand_cap, 1u << 18, 4096));
 
     /* mixer look-up tables, built with the host libm exactly like the reference
      * (setup_lookup_tables_for_frequency_translation, rtl_wmbus.c:974-993) */
@@ -886,7 +936,7 @@ static int burst_alloc(wmb_ctx *c)
     if (c->burst_allocated) return WMB_OK;
     const size_t M = (size_t)c->M_max;
     const size_t nw = M / 32 + 2, units = M / WMB_BURST_UNIT + 2;
-    c->burst_cap = (uint32_t)(M / 256 + 4);
+    const size_t cap = M / 256 + 4;             /* records per slot and chain: pieces >= 256 samples of one batch */
     for (int ch = 0; ch < WMB_N_CHAINS; ch++) {
         if (!(c->chains & (1u << ch))) continue;
         wmb_ctx::BurstBuf &b = c->bb[ch];
@@ -898,34 +948,28 @@ static int burst_alloc(wmb_ctx *c)
         TRY(dev_alloc(c, &b.agg, scan_tiles((uint32_t)units) + 1));
         TRY(dev_alloc(c, &b.ev, ev_cap));
         TRY(dev_alloc(c, &b.bd, 1, true));
-        TRY(dev_alloc(c, &b.items, (size_t)c->burst_cap + 1));
+        TRY(dev_alloc(c, &b.items, cap + 1));
     }
-    TRY(dev_alloc(c, &c->d_brec, (size_t)WMB_NSLOT * WMB_N_CHAINS * c->burst_cap));
-    TRY(host_alloc(c, &c->h_brec, (size_t)WMB_NSLOT * WMB_N_CHAINS * c->burst_cap));
+    TRY(c->brec.alloc(c, WMB_N_CHAINS, cap, 64, 64));
     TRY(dev_alloc(c, &c->d_bslot, WMB_NSLOT, true));
     TRY(host_alloc(c, &c->h_bslot, WMB_NSLOT));
-    c->burst_spec = std::min<uint32_t>(64, c->burst_cap);
     CUDA_TRY(cudaDeviceSynchronize());
     c->burst_allocated = true;
     return WMB_OK;
 }
 
 /* the quality report's buffers, at the first gather that needs them: beside the candidate log and the carried
- * candidates, and (when the burst report is on, so its tables exist) beside the burst records */
+ * candidates, and (when the burst report is on, so its tables exist) beside the burst records.  The sums are copied
+ * side by side with the headers / records, with the prefix those have grown to */
 static int qual_alloc(wmb_ctx *c)
 {
-    if (!c->qual_allocated) {
-        TRY(dev_alloc(c, &c->d_qual, (size_t)WMB_NSLOT * c->slot_cap));
-        TRY(host_alloc(c, &c->h_qual, (size_t)WMB_NSLOT * c->slot_cap));
+    if (!c->qual.d) {
         for (int ch = 0; ch < WMB_N_CHAINS; ch++)
             for (int a = 0; a < WMB_N_ALGOS; a++)
                 if (c->cb[ch].s[a].pend) TRY(dev_alloc(c, &c->cb[ch].s[a].pend_qual, c->pend_cap));
-        c->qual_allocated = true;
+        TRY(c->qual.alloc(c, 1, c->hdr.cap, c->hdr.prefix, 256));
     }
-    if (c->burst_allocated && !c->d_bqual) {
-        TRY(dev_alloc(c, &c->d_bqual, (size_t)WMB_NSLOT * WMB_N_CHAINS * c->burst_cap));
-        TRY(host_alloc(c, &c->h_bqual, (size_t)WMB_NSLOT * WMB_N_CHAINS * c->burst_cap));
-    }
+    if (c->burst_allocated && !c->bqual.d) TRY(c->bqual.alloc(c, WMB_N_CHAINS, c->brec.cap, c->brec.prefix, 64));
     return WMB_OK;
 }
 
@@ -947,34 +991,20 @@ static uint32_t spec_rows_for(const wmb_ctx *c, uint32_t N, uint32_t B)
     return (uint32_t)(c->max_batch_bytes / (2 * (size_t)N) / B + 2);
 }
 
-static int spec_free(wmb_ctx *c, void *p, bool host)
-{
-    if (!p) return WMB_OK;
-    std::vector<void *> &v = host ? c->host_allocs : c->dev_allocs;
-    v.erase(std::remove(v.begin(), v.end(), p), v.end());
-    CUDA_TRY(host ? cudaFreeHost(p) : cudaFree(p));
-    return WMB_OK;
-}
-
 /* the survey's buffers, at the first batch that needs them (again when a new setting needs larger tables) */
 static int spec_alloc(wmb_ctx *c)
 {
     const uint32_t N = c->spec_bins;
     c->spec_R = spec_rows_for(c, N, c->spec_B);
     const size_t need = (size_t)c->spec_R * N;
-    if (need > c->spec_cap) {
+    if (need > c->speak.cap) {                       /* speak comes last: its cap is that of the rings and of ssum */
         CUDA_TRY(cudaDeviceSynchronize());
-        TRY(spec_free(c, c->d_ssum_ring, false)); TRY(spec_free(c, c->d_speak_ring, false));
-        TRY(spec_free(c, c->d_ssum, false)); TRY(spec_free(c, c->d_speak, false));
-        TRY(spec_free(c, c->h_ssum, true)); TRY(spec_free(c, c->h_speak, true));
-        c->spec_cap = 0;
+        TRY(mem_free(c, c->d_ssum_ring, false)); TRY(mem_free(c, c->d_speak_ring, false));
+        TRY(c->ssum.release(c)); TRY(c->speak.release(c));
         TRY(dev_alloc(c, &c->d_ssum_ring, need, true));
         TRY(dev_alloc(c, &c->d_speak_ring, need, true));
-        TRY(dev_alloc(c, &c->d_ssum, need * WMB_NSLOT));
-        TRY(dev_alloc(c, &c->d_speak, need * WMB_NSLOT));
-        TRY(host_alloc(c, &c->h_ssum, need * WMB_NSLOT));
-        TRY(host_alloc(c, &c->h_speak, need * WMB_NSLOT));
-        c->spec_cap = need;
+        TRY(c->ssum.alloc(c, 1, need, 0, 0));         /* copied exactly: the host knows the rows a batch closed */
+        TRY(c->speak.alloc(c, 1, need, 0, 0));
     }
     if (!c->d_spec_tab) {
         TRY(dev_alloc(c, &c->d_spec_tab, 2 * (size_t)WMB_SPEC_MAXN));
@@ -1198,6 +1228,18 @@ static uint32_t pick_chunk_coop(const wmb_ctx *c, int64_t M)
     return (uint32_t)C;
 }
 
+/* a survey record's row: `blocks` of its blocks counted */
+static wmb_spectrum_row spec_row(const wmb_ctx *c, int64_t record, uint32_t blocks)
+{
+    const uint64_t N = c->spec_bins, B = c->spec_B;
+    const double fs = 0.8e6 * (double)c->d;
+    wmb_spectrum_row w;
+    memset(&w, 0, sizeof(w));
+    w.record = (uint64_t)record; w.start_iq = (uint64_t)record * B * N; w.blocks = blocks; w.bins = (uint32_t)N;
+    w.hz_low = -fs / 2; w.hz_step = fs / (double)N;
+    return w;
+}
+
 /* Enqueue the per-sample device pass for one batch whose bytes are at `src` (device memory): demod on k1s, clock
  * recovery lanes on as[set], everything that is sequential from batch to batch on cs.  Nothing here waits for the
  * device: refuted speculative lanes are re-run by on-device fix-up kernels, and the fallback from the two-phase
@@ -1249,22 +1291,14 @@ static int spec_batch(wmb_ctx *c, const uint8_t *src, uint64_t q0, uint64_t n_iq
     } else if (c->spec_open >= 0) {
         if (c->spec_open < r_last) lone = c->spec_open; else open = c->spec_open;
     }
-    const double fs = 0.8e6 * (double)c->d;
-    auto row = [&](int64_t r) {
-        wmb_spectrum_row w;
-        memset(&w, 0, sizeof(w));
-        w.record = (uint64_t)r; w.start_iq = (uint64_t)r * B * N; w.blocks = counted(r); w.bins = (uint32_t)N;
-        w.hz_low = -fs / 2; w.hz_step = fs / (double)N;
-        return w;
-    };
-    if (lone >= 0) c->spec_batch_rows.push_back(row(lone));
-    for (int64_t r = r_lo; r < r_hi; r++) c->spec_batch_rows.push_back(row(r));
+    if (lone >= 0) c->spec_batch_rows.push_back(spec_row(c, lone, counted(lone)));
+    for (int64_t r = r_lo; r < r_hi; r++) c->spec_batch_rows.push_back(spec_row(c, r, counted(r)));
     const uint32_t open_blocks = open >= 0 ? counted(open) : 0u;
     if (!c->spec_batch_rows.empty()) {
         SpecCloseParams q;
         memset(&q, 0, sizeof(q));
         q.sum = c->d_ssum_ring; q.peak = c->d_speak_ring;
-        q.out_sum = c->d_ssum + (size_t)slot * c->spec_cap; q.out_peak = c->d_speak + (size_t)slot * c->spec_cap;
+        q.out_sum = c->ssum.d + c->ssum.at(slot); q.out_peak = c->speak.d + c->speak.at(slot);
         q.lone = lone; q.r_lo = r_lo; q.n = (uint32_t)c->spec_batch_rows.size(); q.N = (uint32_t)N; q.R = c->spec_R;
         TRY(launch_spec_close(c, q, sk));
     }
@@ -1585,34 +1619,23 @@ static double chain_carrier_hz(const wmb_ctx *c, int chain)
     return 0.0;
 }
 
-/* one slot's burst records -> the queue; the frontier: where the next piece of any chain may start */
-static int book_bursts(wmb_ctx *c, int slot, uint64_t m_end, uint32_t spec, bool quality)
+/* one slot's burst records (fetched whole) -> the queue; the frontier: where the next piece of any chain may start */
+static void book_bursts(wmb_ctx *c, const wmb_ctx::InFlight &f)
 {
-    const BurstSlot bs = c->h_bslot[slot];
-    uint64_t frontier = m_end;
-    uint32_t most = 0;
+    const BurstSlot bs = c->h_bslot[f.slot];
+    uint64_t frontier = f.m_end;
     for (int ch = 0; ch < WMB_N_CHAINS; ch++) {
         if (!c->burst_level[ch] || !(c->chains & (1u << ch))) continue;
         const uint32_t n = bs.n[ch];
-        if (n > c->burst_cap) return set_err(WMB_E_STATE, "internal: burst records beyond their table");
-        const size_t at = ((size_t)slot * WMB_N_CHAINS + ch) * c->burst_cap;
-        if (n > spec) {
-            CUDA_TRY(cudaMemcpyAsync(c->h_brec + at + spec, c->d_brec + at + spec, (size_t)(n - spec) * sizeof(BurstRec),
-                                     cudaMemcpyDeviceToHost, c->xs));
-            if (quality)
-                CUDA_TRY(cudaMemcpyAsync(c->h_bqual + at + spec, c->d_bqual + at + spec, (size_t)(n - spec) * sizeof(QualAcc),
-                                         cudaMemcpyDeviceToHost, c->xs));
-            CUDA_TRY(cudaStreamSynchronize(c->xs));
-        }
-        c->st.d2h_bytes += (uint64_t)std::max(n, spec) * sizeof(BurstRec);
-        if (quality) c->st.d2h_bytes += (uint64_t)std::max(n, spec) * sizeof(QualAcc);
-        most = std::max(most, n);
+        const size_t at = c->brec.at(f.slot, ch);
+        c->st.d2h_bytes += (uint64_t)std::max(n, f.brec) * sizeof(BurstRec);
+        if (f.bqual) c->st.d2h_bytes += (uint64_t)std::max(n, f.bqual) * sizeof(QualAcc);
         for (uint32_t i = 0; i < n; i++) {
-            const BurstRec &r = c->h_brec[at + i];
+            const BurstRec &r = c->brec.h[at + i];
             QueuedBurst qb;
             wmb_burst &b = qb.b;
             memset(&b, 0, sizeof(b));
-            if (quality) qb.q = c->h_bqual[at + i]; else qual_zero(qb.q);
+            if (f.bqual) qb.q = c->bqual.h[at + i]; else qual_zero(qb.q);
             b.start_sample = r.start; b.end_sample = r.end; b.rssi_sum = r.rssi_sum; b.sum = r.sum; b.n = r.n;
             b.chain = r.chain; b.peak = r.peak; b.flags = r.flags;
             /* -a: the cross-product discriminator is not a frequency */
@@ -1624,9 +1647,7 @@ static int book_bursts(wmb_ctx *c, int slot, uint64_t m_end, uint32_t spec, bool
         if (bs.open[ch] && (uint64_t)bs.ps[ch] < frontier) frontier = (uint64_t)bs.ps[ch];
     }
     c->st.d2h_bytes += sizeof(BurstSlot);
-    if (most > c->burst_spec) c->burst_spec = std::min<uint32_t>(c->burst_cap, most + most / 4 + 64);
     c->burst_frontier = frontier;
-    return WMB_OK;
 }
 
 /* Enqueue the frame gather (K3), the device framer (K4) and the copies of their results into the host mirror of the
@@ -1639,7 +1660,7 @@ static int enqueue_gather(wmb_ctx *c, bool final, bool after_batch)
     const bool any_sync = c->o.rla_enabled || c->o.t2_enabled;
     if (c->inflight.size() >= WMB_NSLOT) TRY(consume_oldest(c));          /* the slot's host mirror must be free */
     const int slot = (int)(c->gather_no % WMB_NSLOT);
-    const size_t lb = (size_t)slot * c->slot_cap, pb = (size_t)slot * c->slot_pool;
+    wmb_ctx::InFlight f{};
     const bool quality = c->quality && !c->manual;  /* (a caller's frames carry no sums: manual mode takes none) */
     const bool bursts = bursts_on(c) && (after_batch || final);
     if (bursts) TRY(burst_alloc(c));
@@ -1665,25 +1686,24 @@ static int enqueue_gather(wmb_ctx *c, bool final, bool after_batch)
         p.m_first = (c->m_consumed - (uint64_t)c->last_M) & EVG_M_MASK;
         p.prefix = c->W; p.clip = (uint32_t)c->last_hist; p.batch_m = after_batch ? (uint32_t)c->last_M : 0u;
         p.gd = c->d_gd; p.rec = c->d_rec + slot;
-        p.hdr_log = c->d_hdr; p.dec_log = c->d_dec; p.log_base = (uint32_t)lb; p.log_cap = c->slot_cap;
+        p.hdr_log = c->hdr.d; p.dec_log = c->dec.d; p.log_base = (uint32_t)c->hdr.at(slot); p.log_cap = (uint32_t)c->hdr.cap;
         p.words = c->d_words; p.words_cap = c->frame_words_cap;
         p.cut_n = c->d_cut_n; p.agg = c->d_k3_agg; p.errors = c->d_errors;
         p.final = final ? 1u : 0u;
-        if (quality) { p.qual_log = c->d_qual; p.qual_skip = c->o.accurate_atan ? 0u : 1u; }
+        if (quality) { p.qual_log = c->qual.d; p.qual_skip = c->o.accurate_atan ? 0u : 1u; }
         K4Params q;
         memset(&q, 0, sizeof(q));
-        q.hdr = c->d_hdr; q.words = c->d_words; q.dec = c->d_dec;
-        q.pool = c->d_pool + pb; q.pool_cap = c->slot_pool; q.pool_n = GD_FIELD(c, pool_n); q.errors = c->d_errors; q.gd = c->d_gd;
+        q.hdr = c->hdr.d; q.words = c->d_words; q.dec = c->dec.d;
+        q.pool = c->pool.d + c->pool.at(slot); q.pool_cap = (uint32_t)c->pool.cap; q.pool_n = GD_FIELD(c, pool_n); q.errors = c->d_errors; q.gd = c->d_gd;
         TRY(launch_k3_k4(c, p, c->manual ? nullptr : &q));
         /* results -> pinned host mirror: the record and a prefix of the arrays it describes (the rest, if a batch ever
          * produces more, is fetched when the record has been read) */
         CUDA_TRY(cudaMemcpyAsync(c->h_rec + slot, c->d_rec + slot, sizeof(BatchRec), cudaMemcpyDeviceToHost, c->cs));
-        CUDA_TRY(cudaMemcpyAsync(c->h_hdr + lb, c->d_hdr + lb, (size_t)c->spec_n * sizeof(FrameHdr), cudaMemcpyDeviceToHost, c->cs));
-        if (quality)
-            CUDA_TRY(cudaMemcpyAsync(c->h_qual + lb, c->d_qual + lb, (size_t)c->spec_n * sizeof(QualAcc), cudaMemcpyDeviceToHost, c->cs));
+        TRY(c->hdr.enqueue(slot, 0, c->cs, &f.hdr));
+        if (quality) TRY(c->qual.enqueue(slot, 0, c->cs, &f.qual));
         if (!c->manual) {
-            CUDA_TRY(cudaMemcpyAsync(c->h_dec + lb, c->d_dec + lb, (size_t)c->spec_n * sizeof(DecHdr), cudaMemcpyDeviceToHost, c->cs));
-            CUDA_TRY(cudaMemcpyAsync(c->h_pool + pb, c->d_pool + pb, c->spec_pool, cudaMemcpyDeviceToHost, c->cs));
+            TRY(c->dec.enqueue(slot, 0, c->cs, &f.dec));
+            TRY(c->pool.enqueue(slot, 0, c->cs, &f.pool));
         }
     }
     /* the burst report: behind the demod kernel of the batch (cs waited for it), before ev_chain[set] releases the set */
@@ -1704,10 +1724,10 @@ static int enqueue_gather(wmb_ctx *c, bool final, bool after_batch)
             p.level = c->burst_level[ch]; p.chain = (uint32_t)ch; p.final_ = final ? 1u : 0u;
             p.nw = (uint32_t)((p.M + 31) / 32); p.units = (uint32_t)((p.M + WMB_BURST_UNIT - 1) / WMB_BURST_UNIT);
             p.mask = b.mask; p.cnt = b.cnt; p.base = b.base; p.ev = b.ev; p.bd = b.bd; p.items = b.items;
-            p.out = c->d_brec + ((size_t)slot * WMB_N_CHAINS + ch) * c->burst_cap;
+            p.out = c->brec.d + c->brec.at(slot, ch);
             p.slot = c->d_bslot + slot;
             if (bqual) {
-                p.qout = c->d_bqual + ((size_t)slot * WMB_N_CHAINS + ch) * c->burst_cap;
+                p.qout = c->bqual.d + c->bqual.at(slot, ch);
                 p.qual_skip = c->o.accurate_atan ? 0u : 1u;
             }
             TRY(launch_bursts(c, p, b.agg));
@@ -1715,15 +1735,12 @@ static int enqueue_gather(wmb_ctx *c, bool final, bool after_batch)
         CUDA_TRY(cudaMemcpyAsync(c->h_bslot + slot, c->d_bslot + slot, sizeof(BurstSlot), cudaMemcpyDeviceToHost, c->cs));
         for (int ch = 0; ch < WMB_N_CHAINS; ch++) {
             if (!c->burst_level[ch] || !(c->chains & (1u << ch))) continue;
-            const size_t at = ((size_t)slot * WMB_N_CHAINS + ch) * c->burst_cap;
-            CUDA_TRY(cudaMemcpyAsync(c->h_brec + at, c->d_brec + at, (size_t)c->burst_spec * sizeof(BurstRec), cudaMemcpyDeviceToHost, c->cs));
-            if (bqual)
-                CUDA_TRY(cudaMemcpyAsync(c->h_bqual + at, c->d_bqual + at, (size_t)c->burst_spec * sizeof(QualAcc), cudaMemcpyDeviceToHost, c->cs));
+            TRY(c->brec.enqueue(slot, ch, c->cs, &f.brec));
+            if (bqual) TRY(c->bqual.enqueue(slot, ch, c->cs, &f.bqual));
         }
     }
     /* the band survey: the rows the batch closed (its kernels ran on the demod stream), or at the end of input the
      * record still open */
-    bool spec = false;
     if (c->spec_bins) {
         std::vector<wmb_spectrum_row> &rows = c->spec_slot_rows[slot];
         rows.clear();
@@ -1737,28 +1754,21 @@ static int enqueue_gather(wmb_ctx *c, bool final, bool after_batch)
         if (after_batch && !c->spec_batch_rows.empty()) {
             rows.swap(c->spec_batch_rows);
         } else if (final && c->spec_open >= 0) {
-            const uint64_t N = c->spec_bins, B = c->spec_B;
-            const double fs = 0.8e6 * (double)c->d;
-            wmb_spectrum_row w;
-            memset(&w, 0, sizeof(w));
-            w.record = (uint64_t)c->spec_open; w.start_iq = w.record * B * N; w.blocks = c->spec_open_blocks;
-            w.bins = (uint32_t)N; w.hz_low = -fs / 2; w.hz_step = fs / (double)N;
-            rows.push_back(w);
+            rows.push_back(spec_row(c, c->spec_open, c->spec_open_blocks));
             SpecCloseParams q;
             memset(&q, 0, sizeof(q));
             q.sum = c->d_ssum_ring; q.peak = c->d_speak_ring;
-            q.out_sum = c->d_ssum + (size_t)slot * c->spec_cap; q.out_peak = c->d_speak + (size_t)slot * c->spec_cap;
-            q.lone = c->spec_open; q.n = 1; q.N = (uint32_t)N; q.R = c->spec_R;
+            q.out_sum = c->ssum.d + c->ssum.at(slot); q.out_peak = c->speak.d + c->speak.at(slot);
+            q.lone = c->spec_open; q.n = 1; q.N = c->spec_bins; q.R = c->spec_R;
             TRY(launch_spec_close(c, q, c->cs));
             CUDA_TRY(cudaEventRecord(c->ev_spec_flush, c->cs));
             c->spec_flush_pending = true;
             c->spec_open = -1; c->spec_open_blocks = 0;
         }
         if (!rows.empty()) {
-            const size_t at = (size_t)slot * c->spec_cap, n = rows.size() * (size_t)c->spec_bins;
-            CUDA_TRY(cudaMemcpyAsync(c->h_ssum + at, c->d_ssum + at, n * sizeof(uint64_t), cudaMemcpyDeviceToHost, c->cs));
-            CUDA_TRY(cudaMemcpyAsync(c->h_speak + at, c->d_speak + at, n * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->cs));
-            spec = true;
+            c->ssum.prefix = c->speak.prefix = (uint32_t)rows.size() * c->spec_bins;     /* exact */
+            TRY(c->ssum.enqueue(slot, 0, c->cs, &f.ssum));
+            TRY(c->speak.enqueue(slot, 0, c->cs, &f.speak));
         }
     }
     CUDA_TRY(cudaEventRecord(c->ev_res[slot], c->cs));
@@ -1768,11 +1778,7 @@ static int enqueue_gather(wmb_ctx *c, bool final, bool after_batch)
         CUDA_TRY(cudaEventRecord(c->ev_chain[c->last_set], c->cs));
         c->chain_recorded[c->last_set] = true;
     }
-    wmb_ctx::InFlight f;
-    f.slot = slot; f.final = final; f.has_timers = after_batch; f.m_end = c->m_consumed; f.bursts = bursts;
-    f.burst_spec = c->burst_spec;                    /* records the copies above fetched (burst_spec may grow before they are read) */
-    f.spec = spec;
-    f.quality = quality && any_sync; f.bquality = bqual;
+    f.slot = slot; f.final = final; f.has_timers = after_batch; f.m_end = c->m_consumed;
     c->inflight.push_back(f);
     c->gather_no++;
     return WMB_OK;
@@ -1788,7 +1794,6 @@ static int consume_oldest(wmb_ctx *c)
     if (c->inflight.empty()) return WMB_OK;
     const wmb_ctx::InFlight f = c->inflight.front();
     c->inflight.erase(c->inflight.begin());
-    const bool any_sync = c->o.rla_enabled || c->o.t2_enabled;
     const double t0 = wall_ms();
     CUDA_TRY(cudaEventSynchronize(c->ev_res[f.slot]));
     const double t1 = wall_ms();
@@ -1803,19 +1808,40 @@ static int consume_oldest(wmb_ctx *c)
         /* the whole per-sample pass of the push so far: first demod kernel -> this batch's last bit-sync kernel */
         if (cudaEventElapsedTime(&ms, c->ev_push_start, evt[3]) == cudaSuccess) c->acc_pass_ms = ms;
     }
-    if (f.bursts) TRY(book_bursts(c, f.slot, f.m_end, f.burst_spec, f.bquality));
-    if (f.spec) {                                    /* the slot's survey rows -> the queue */
-        const std::vector<wmb_spectrum_row> &rows = c->spec_slot_rows[f.slot];
-        const size_t at = (size_t)f.slot * c->spec_cap, n = rows.size() * (size_t)c->spec_bins;
-        c->spec_rows.insert(c->spec_rows.end(), rows.begin(), rows.end());
-        c->spec_sum.insert(c->spec_sum.end(), c->h_ssum + at, c->h_ssum + at + n);
-        c->spec_peak.insert(c->spec_peak.end(), c->h_speak + at, c->h_speak + at + n);
-        c->st.d2h_bytes += n * (sizeof(uint64_t) + sizeof(uint32_t));
+    /* what the prefix copies missed, on xs, and one wait for all of it: the slot is not written again before it is read */
+    const BatchRec r = f.hdr ? c->h_rec[f.slot] : BatchRec{};
+    uint32_t most = 0;                               /* burst records of the slot's fullest chain */
+    bool more = false;
+    for (int ch = 0; f.brec && ch < WMB_N_CHAINS; ch++) {
+        if (!c->burst_level[ch] || !(c->chains & (1u << ch))) continue;
+        const uint32_t n = c->h_bslot[f.slot].n[ch];
+        TRY(c->brec.fetch(f.slot, ch, f.brec, n, c->xs, &more));
+        if (f.bqual) TRY(c->bqual.fetch(f.slot, ch, f.bqual, n, c->xs, &more));
+        most = std::max(most, n);
     }
-    if (!any_sync) return WMB_OK;
-    const bool dev_decode = !c->manual;
-    const size_t lb = (size_t)f.slot * c->slot_cap, pb = (size_t)f.slot * c->slot_pool;
-    const BatchRec r = c->h_rec[f.slot];
+    TRY(c->hdr.fetch(f.slot, 0, f.hdr, r.n, c->xs, &more));
+    if (f.dec) TRY(c->dec.fetch(f.slot, 0, f.dec, r.n, c->xs, &more));
+    if (f.qual) TRY(c->qual.fetch(f.slot, 0, f.qual, r.n, c->xs, &more));
+    if (f.pool) TRY(c->pool.fetch(f.slot, 0, f.pool, r.pool_n, c->xs, &more));
+    if (!f.dec && r.n_words) {               /* manual mode reads after every batch: the frame words are this batch's */
+        CUDA_TRY(cudaMemcpyAsync(c->h_words, c->d_words, (size_t)r.n_words * 4, cudaMemcpyDeviceToHost, c->xs));
+        c->st.d2h_bytes += (uint64_t)r.n_words * 4;
+        more = true;
+    }
+    if (more) CUDA_TRY(cudaStreamSynchronize(c->xs));
+    /* the next batches probably look like this one: let the prefix copies cover them */
+    if (f.brec) { c->brec.grow(most); c->bqual.grow(most); }
+    if (f.hdr) { c->hdr.grow(r.n); c->dec.grow(r.n); c->qual.grow(r.n); c->pool.grow(r.pool_n); }
+    if (f.brec) book_bursts(c, f);
+    if (f.ssum) {                                    /* the slot's survey rows -> the queue */
+        const std::vector<wmb_spectrum_row> &rows = c->spec_slot_rows[f.slot];
+        const size_t at = c->ssum.at(f.slot);        /* = c->speak.at(f.slot): both hold rows x bins */
+        c->spec_rows.insert(c->spec_rows.end(), rows.begin(), rows.end());
+        c->spec_sum.insert(c->spec_sum.end(), c->ssum.h + at, c->ssum.h + at + f.ssum);
+        c->spec_peak.insert(c->spec_peak.end(), c->speak.h + at, c->speak.h + at + f.speak);
+        c->st.d2h_bytes += (uint64_t)f.ssum * sizeof(uint64_t) + (uint64_t)f.speak * sizeof(uint32_t);
+    }
+    if (!f.hdr) return WMB_OK;
     const uint32_t err = r.errors;
     if (err & 2u) return set_err(WMB_E_OVERFLOW, "run-length tracker left its defined range (the reference would spin here)");
     /* lane event buffer (1: a run-length lane emitted more than one bit per four samples plus one capped edge -- the
@@ -1824,28 +1850,8 @@ static int consume_oldest(wmb_ctx *c)
      * would have gone on decoding, so does the stream */
     if (err & K3_SOFT_ERRORS) c->st.overflow_batches++;
     if (err & 256u) return set_err(WMB_E_STATE, "internal: lane verification does not converge");
-    bool more = false;
-    if (r.n > c->spec_n) {
-        CUDA_TRY(cudaMemcpyAsync(c->h_hdr + lb + c->spec_n, c->d_hdr + lb + c->spec_n, (size_t)(r.n - c->spec_n) * sizeof(FrameHdr), cudaMemcpyDeviceToHost, c->xs));
-        if (dev_decode) CUDA_TRY(cudaMemcpyAsync(c->h_dec + lb + c->spec_n, c->d_dec + lb + c->spec_n, (size_t)(r.n - c->spec_n) * sizeof(DecHdr), cudaMemcpyDeviceToHost, c->xs));
-        if (f.quality) CUDA_TRY(cudaMemcpyAsync(c->h_qual + lb + c->spec_n, c->d_qual + lb + c->spec_n, (size_t)(r.n - c->spec_n) * sizeof(QualAcc), cudaMemcpyDeviceToHost, c->xs));
-        more = true;
-    }
-    if (dev_decode && r.pool_n > c->spec_pool) {
-        CUDA_TRY(cudaMemcpyAsync(c->h_pool + pb + c->spec_pool, c->d_pool + pb + c->spec_pool, r.pool_n - c->spec_pool, cudaMemcpyDeviceToHost, c->xs));
-        more = true;
-    }
-    if (!dev_decode && r.n_words) {          /* manual mode reads after every batch: the frame words are this batch's */
-        CUDA_TRY(cudaMemcpyAsync(c->h_words, c->d_words, (size_t)r.n_words * 4, cudaMemcpyDeviceToHost, c->xs));
-        c->st.d2h_bytes += (uint64_t)r.n_words * 4;
-        more = true;
-    }
-    if (more) CUDA_TRY(cudaStreamSynchronize(c->xs));       /* the slot is not written again before it is consumed */
-    /* the next batches probably look like this one: let the prefix copy cover them */
-    if (r.n > c->spec_n) c->spec_n = std::min<uint32_t>(c->slot_cap, r.n + r.n / 4 + 256);
-    if (r.pool_n > c->spec_pool) c->spec_pool = std::min<uint32_t>(c->slot_pool, r.pool_n + r.pool_n / 4 + 4096);
-    c->st.d2h_bytes += sizeof(BatchRec) + (size_t)r.n * sizeof(FrameHdr) + (dev_decode ? (size_t)r.n * sizeof(DecHdr) + r.pool_n : 0);
-    if (f.quality) c->st.d2h_bytes += (size_t)r.n * sizeof(QualAcc);
+    c->st.d2h_bytes += sizeof(BatchRec) + (size_t)r.n * sizeof(FrameHdr) + (f.dec ? (size_t)r.n * sizeof(DecHdr) + r.pool_n : 0);
+    if (f.qual) c->st.d2h_bytes += (size_t)r.n * sizeof(QualAcc);
     /* statistics kept on the device */
     c->st.lanes_rerun += r.lanes_rerun - c->stat_rerun_seen; c->st.lanes_run += r.lanes_rerun - c->stat_rerun_seen;
     c->stat_rerun_seen = r.lanes_rerun;
@@ -1861,13 +1867,13 @@ static int consume_oldest(wmb_ctx *c)
             if (f.has_timers) c->cb[ch].s[a].total_prev = c->cb[ch].s[a].total;
             c->cb[ch].s[a].total = r.total[k];
         }
-    if (r.n > c->slot_cap) return set_err(WMB_E_STATE, "internal: batch record beyond its slot");
-    FrameHdr *hdr = c->h_hdr + lb;
+    FrameHdr *hdr = c->hdr.h + c->hdr.at(f.slot);
     /* the device keeps 40 bits of the sample index; widen to the 64-bit stream position: the newest value
      * congruent to it that is not beyond the samples produced when the batch was gathered */
     for (uint32_t i = 0; i < r.n; i++) hdr[i].sync_sample = f.m_end - ((f.m_end - hdr[i].sync_sample) & EVG_M_MASK);
     int rc = WMB_OK;
-    if (dev_decode) rc = book_device_frames(c, hdr, c->h_dec + lb, f.quality ? c->h_qual + lb : nullptr, c->h_pool + pb, r.n, f.final);
+    if (f.dec) rc = book_device_frames(c, hdr, c->dec.h + c->dec.at(f.slot), f.qual ? c->qual.h + c->qual.at(f.slot) : nullptr,
+                                       c->pool.h + c->pool.at(f.slot), r.n, f.final);
     else {
         /* manual mode: keep the frames (newest version of a re-delivered partial one wins) for wmb_poll */
         for (uint32_t i = 0; i < r.n; i++) {
@@ -2179,11 +2185,25 @@ static int book_frames(wmb_ctx *c, size_t n, Meta meta, Lite lite, Fill fill)
     return WMB_OK;
 }
 
+/* a K4 verdict -> the decoded telegram, its datagram out of the slot's pool (K4_SKIP: a frame without any bit) */
+static void decoded_from(const DecHdr &d, uint64_t sync_sample, const uint8_t *pool, wmb_decoded &o)
+{
+    static const char modes[3][3] = { "T1", "C1", "S1" };
+    memset(&o, 0, sizeof(o));
+    o.status = d.status == K4_SKIP ? (int)WMB_DEC_NEED_MORE : (int)d.status;
+    o.consumed = d.consumed;
+    o.end_sample = d.status == K4_SKIP ? 0 : sync_sample + d.end_off;
+    if (d.status != K4_LINE) return;
+    memcpy(o.mode, modes[d.mode < 3 ? d.mode : 0], 3);
+    o.crc_ok = d.crc_ok; o.ok_3of6 = d.ok_3of6; o.packet_rssi = d.packet_rssi; o.current_rssi = d.current_rssi;
+    o.serial = d.serial; o.len = d.len;
+    memcpy(o.datagram, pool + d.data_off, d.len);
+}
+
 /* candidates of one gathered batch, decoded by K4 (already in stream order) */
 static int book_device_frames(wmb_ctx *c, const FrameHdr *hdr, const DecHdr *dec, const QualAcc *qual, const uint8_t *pool,
                               size_t n, bool final)
 {
-    static const char modes[3][3] = { "T1", "C1", "S1" };
     /* frames without any bit (candidate at the very end of the stream) are not decoded at all */
     std::vector<uint32_t> idx;
     idx.reserve(n);
@@ -2205,15 +2225,7 @@ static int book_device_frames(wmb_ctx *c, const FrameHdr *hdr, const DecHdr *dec
             l.status = d.status; l.consumed = d.consumed; l.end_sample = hdr[idx[k]].sync_sample + d.end_off; l.crc_ok = d.crc_ok;
             return l;
         },
-        [&](size_t k, wmb_decoded &o) {
-            const DecHdr &d = dec[idx[k]];
-            memset(&o, 0, sizeof(o));
-            o.status = WMB_DEC_LINE; o.consumed = d.consumed; o.end_sample = hdr[idx[k]].sync_sample + d.end_off;
-            memcpy(o.mode, modes[d.mode < 3 ? d.mode : 0], 3);
-            o.crc_ok = d.crc_ok; o.ok_3of6 = d.ok_3of6; o.packet_rssi = d.packet_rssi; o.current_rssi = d.current_rssi;
-            o.serial = d.serial; o.len = d.len;
-            memcpy(o.datagram, pool + d.data_off, d.len);
-        });
+        [&](size_t k, wmb_decoded &o) { decoded_from(dec[idx[k]], hdr[idx[k]].sync_sample, pool, o); });
 }
 
 /* Test hook (declared in wmb_framer.h, not part of the public ABI): run K4 on caller-made frames so
@@ -2226,7 +2238,7 @@ extern "C" int wmb_frame_decode_device(wmb_ctx *c, const wmb_frame *frames, size
     if (n > c->cand_cap) return set_err(WMB_E_INVAL, "too many frames");
     size_t words = 0;
     for (size_t i = 0; i < n; i++) {
-        FrameHdr &h = c->h_hdr[i];
+        FrameHdr &h = c->hdr.h[i];
         memset(&h, 0, sizeof(h));
         h.ordinal = frames[i].ordinal; h.sync_sample = frames[i].sync_sample; h.nbits = frames[i].nbits;
         h.word_off = (uint32_t)words; h.chain = frames[i].chain; h.algo = frames[i].algo; h.complete = 1;
@@ -2234,33 +2246,20 @@ extern "C" int wmb_frame_decode_device(wmb_ctx *c, const wmb_frame *frames, size
         memcpy(c->h_words + words, frames[i].bits, (size_t)h.nbits * 4);
         words += h.nbits;
     }
-    CUDA_TRY(cudaMemcpyAsync(c->d_hdr, c->h_hdr, n * sizeof(FrameHdr), cudaMemcpyHostToDevice, c->cs));
+    CUDA_TRY(cudaMemcpyAsync(c->hdr.d, c->hdr.h, n * sizeof(FrameHdr), cudaMemcpyHostToDevice, c->cs));
     CUDA_TRY(cudaMemcpyAsync(c->d_words, c->h_words, words * 4, cudaMemcpyHostToDevice, c->cs));
     if (!c->inflight.empty()) return set_err(WMB_E_STATE, "unread results");
     CUDA_TRY(cudaMemsetAsync(GD_FIELD(c, pool_n), 0, 4, c->cs));
     K4Params q;
     memset(&q, 0, sizeof(q));
-    q.hdr = c->d_hdr; q.n = (uint32_t)n; q.words = c->d_words; q.dec = c->d_dec;
-    q.pool = c->d_pool; q.pool_cap = c->slot_pool; q.pool_n = GD_FIELD(c, pool_n); q.errors = c->d_errors;
+    q.hdr = c->hdr.d; q.n = (uint32_t)n; q.words = c->d_words; q.dec = c->dec.d;
+    q.pool = c->pool.d; q.pool_cap = (uint32_t)c->pool.cap; q.pool_n = GD_FIELD(c, pool_n); q.errors = c->d_errors;
     TRY(launch_k4(c, q));
-    CUDA_TRY(cudaMemcpyAsync(c->h_dec, c->d_dec, n * sizeof(DecHdr), cudaMemcpyDeviceToHost, c->cs));
-    CUDA_TRY(cudaMemcpyAsync(c->h_pool, c->d_pool, c->slot_pool < (1u << 24) ? c->slot_pool : (1u << 24), cudaMemcpyDeviceToHost, c->cs));
+    TRY(c->dec.fetch(0, 0, 0, (uint32_t)n, c->cs));
+    TRY(c->pool.fetch(0, 0, 0, (uint32_t)std::min<size_t>(c->pool.cap, 1u << 24), c->cs));
     CUDA_TRY(cudaMemsetAsync(GD_FIELD(c, pool_n), 0, 4, c->cs));
     CUDA_TRY(cudaStreamSynchronize(c->cs));
-    static const char modes[3][3] = { "T1", "C1", "S1" };
-    for (size_t i = 0; i < n; i++) {
-        const DecHdr &d = c->h_dec[i];
-        wmb_decoded &o = out[i];
-        memset(&o, 0, sizeof(o));
-        o.status = d.status == K4_SKIP ? (int)WMB_DEC_NEED_MORE : (int)d.status;
-        o.consumed = d.consumed;
-        o.end_sample = d.status == K4_SKIP ? 0 : frames[i].sync_sample + d.end_off;
-        if (d.status != K4_LINE) continue;
-        memcpy(o.mode, modes[d.mode < 3 ? d.mode : 0], 3);
-        o.crc_ok = d.crc_ok; o.ok_3of6 = d.ok_3of6; o.packet_rssi = d.packet_rssi; o.current_rssi = d.current_rssi;
-        o.serial = d.serial; o.len = d.len;
-        memcpy(o.datagram, c->h_pool + d.data_off, d.len);
-    }
+    for (size_t i = 0; i < n; i++) decoded_from(c->dec.h[i], frames[i].sync_sample, c->pool.h, out[i]);
     return WMB_OK;
 }
 
@@ -2462,9 +2461,9 @@ extern "C" int wmb_reset(wmb_ctx *c)
         if (c->burst_allocated)                  /* no run open */
             for (int ch = 0; ch < WMB_N_CHAINS; ch++)
                 if (c->bb[ch].bd) CUDA_TRY(cudaMemsetAsync(c->bb[ch].bd, 0, sizeof(BurstDev), c->cs));
-        if (c->spec_cap) {                       /* no record open */
-            CUDA_TRY(cudaMemsetAsync(c->d_ssum_ring, 0, c->spec_cap * sizeof(uint64_t), c->cs));
-            CUDA_TRY(cudaMemsetAsync(c->d_speak_ring, 0, c->spec_cap * sizeof(uint32_t), c->cs));
+        if (c->speak.cap) {                      /* no record open */
+            CUDA_TRY(cudaMemsetAsync(c->d_ssum_ring, 0, c->speak.cap * sizeof(uint64_t), c->cs));
+            CUDA_TRY(cudaMemsetAsync(c->d_speak_ring, 0, c->speak.cap * sizeof(uint32_t), c->cs));
         }
         CUDA_TRY(cudaEventRecord(c->ev_reset, c->cs));
         c->reset_pending = true;

@@ -310,6 +310,18 @@ def ring_events(max_batch_mib, d):
     return p
 
 
+FIRST_LINE_PREFIX = 4096              # candidates a gather's first prefix copy fetches before their count is known
+
+
+def dense_8mib_capture():
+    """48 MiB of mixed traffic for 8 MiB batches: at DENSE each batch has more candidates than FIRST_LINE_PREFIX, so a
+    pipelined call grows the prefix while later batches are in flight with the one before"""
+    import importlib
+    synth = importlib.import_module("rtl-wmbus_b200.synth")
+    cap, _ = synth.synth_capture(48 << 20, fs=1.6e6, emitters=synth.default_emitters("mixed"), seed=0xB2000077)
+    return np.ascontiguousarray(cap.numpy())
+
+
 def densest_round(ref, lock, words=32):
     """(the most strobes any warp round -- an aligned run of `words` 32-sample words -- holds, per word; the most any
     one word holds): the time2 staging of a round is sized for 11 per word (T2_MAX_PER_WORD)"""

@@ -113,6 +113,17 @@ def test_batch_boundaries_inside_access_codes(pkg, hostsim_lib, name):
     print(f"[codes] {name}: batch boundaries inside access codes at {sorted(inside.items())}")
 
 
+def test_pipelined_batches_beyond_the_copy_prefix(pkg, hostsim_lib):
+    """8 MiB batches with more candidates than the first prefix copy fetches, several in flight: every candidate is
+    read, whichever prefix was current when its batch was gathered"""
+    cu8 = bsc.dense_8mib_capture()
+    ref = bsc.Reference(cu8, "-v")
+    for s in bsc.SETTINGS:
+        n, ovf, compared = bsc.run_pipelined(pkg, hostsim_lib, ref, cu8, s, max_batch_mib=8, min_batches=6)
+        assert compared, (bsc.setting_name(s), n, ovf)
+    assert sum(ref.sync_counts(bsc.DENSE).values()) / n > bsc.FIRST_LINE_PREFIX
+
+
 @pytest.mark.parametrize("order", [1, 2])
 def test_simulated_thread_order(hostsim_lib, order):
     """the checks above with the CPU build's threads run backwards (1) and scrambled (2), in a process of their own

@@ -111,6 +111,22 @@ def test_1gib_pipelined_as_128mib_batches(pkg, gpu_lib, t1x2):
         _report(f"pipelined 8 x 128 MiB {bsc.setting_name(s)}", overflow_batches=ovf, lines_compared=lines)
 
 
+def test_pipelined_8mib_batches_beyond_the_copy_prefix(pkg, gpu_lib):
+    """48 MiB in one process_device call of 8 MiB batches with more candidates than the first prefix copy fetches"""
+    import torch
+    cu8 = bsc.dense_8mib_capture()
+    ref = bsc.Reference(cu8, "-v")
+    dev = torch.from_numpy(cu8).cuda()
+    torch.cuda.synchronize()
+    for s in bsc.SETTINGS:
+        n, ovf, lines = bsc.run_pipelined(pkg, gpu_lib, ref, len(cu8), s, device_ptr=dev.data_ptr(), min_batches=6,
+                                          max_batch_mib=8)
+        assert lines, (bsc.setting_name(s), n, ovf)
+        _report(f"pipelined 8 MiB {bsc.setting_name(s)}", batches=n, sync_flags=ref.sync_counts(s), lines=len(ref.lines[s]))
+    assert sum(ref.sync_counts(bsc.DENSE).values()) / n > bsc.FIRST_LINE_PREFIX
+    del dev
+
+
 def test_densest_warp_round(t1x2):
     host, dev, ref = t1x2
     per_word, word = bsc.densest_round(ref, 1)
