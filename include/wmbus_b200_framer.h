@@ -11,7 +11,9 @@
  * wmb_decode_frames() (wmbus_b200.h) is these functions plus the stream-order bookkeeping; a
  * caller who keeps its own bookkeeping (or only wants the CRC / line format) binds them directly.
  * The default path decodes on the device (kernel K4); wmb_frame_decode() is its host twin and
- * wmb_frame_decode_device() lets a test compare the two candidate by candidate.
+ * wmb_frame_decode_device() lets a test compare the two candidate by candidate.  wmb_frame_repair() repairs T1 / S1
+ * candidates that lost a few chips (erasure decoding checked by the block CRCs), with the device twin
+ * wmb_frame_repair_device().
  */
 #ifndef WMBUS_B200_FRAMER_H
 #define WMBUS_B200_FRAMER_H
@@ -44,6 +46,43 @@ void wmb_frame_decode(const wmb_frame *f, wmb_decoded *out);
 
 /* The same decode done by the device framer (kernel K4), n frames at once. */
 int wmb_frame_decode_device(wmb_ctx *ctx, const wmb_frame *frames, size_t n, wmb_decoded *out);
+
+/* ---- erasure repair of one candidate ----------------------------------------------------------------------------
+ * T1 (3-out-of-6) and S1 (Manchester) say where a chip went wrong: one flipped chip makes a 6-bit word that is no
+ * code word (weight 2 or 4), or a "00" / "11" chip pair.  The block CRCs then tell which filling of those erasures
+ * is right.  With e_max in 1..3:
+ *   1. Candidates: a frame whose decode (wmb_frame_decode) is a line with crc_ok = 0, and an S1 frame whose decode
+ *      aborts on a Manchester violation after the L-field byte.  The L-field is never repaired.  The bit list must reach
+ *      P = 1 + 12 len (T1) or 1 + 16 len (S1) bits (else TRUNCATED) and no bit before bit P - 1 may have rssi < 5 (else
+ *      UNREPAIRABLE: the RSSI abort stays an abort).  C1 is NRZ and has no erasures.
+ *   2. Erasures: a T1 data or CRC symbol that is no code word.  Weight 2 or 4: its fillings are the code words at
+ *      Hamming distance 1 (2 to 4 of them); weight 0, 1, 5, 6 and the invalid weight-3 words 7, 21, 42, 56 make the
+ *      frame UNREPAIRABLE.  An S1 "00" / "11" pair: fillings 0 and 1.
+ *   3. Blocks of frame format A (12 bytes, then 18): a block with more than e_max erasures makes the frame TOO_MANY.
+ *      Otherwise, in block order, a block must have exactly one filling (of at most 4^e or 2^e) that passes its CRC --
+ *      as received when it has no erasure.  The first block with none makes the frame UNREPAIRABLE, with two or more
+ *      AMBIGUOUS.
+ *   4. REPAIRED: every block passes and at least one erasure was filled.  `line` is then the line the reference would
+ *      print for the repaired bytes: crc_ok = ok_3of6 = 1, CRC-stripped datagram, consumed = P, end_sample = the
+ *      sample of bit P - 1, packet_rssi / current_rssi at bits 1 and P - 1.
+ * Why wrong repairs stay rare: DESIGN.md section 8. */
+enum { WMB_REP_NONE = 0,          /* not a candidate (a good line, another abort, repair off)                    */
+       WMB_REP_REPAIRED = 1, WMB_REP_AMBIGUOUS = 2, WMB_REP_TOO_MANY = 3, WMB_REP_UNREPAIRABLE = 4,
+       WMB_REP_TRUNCATED = 5 };
+
+typedef struct wmb_repaired {
+    int         outcome;        /* WMB_REP_*                                            */
+    uint32_t    erasures;       /* REPAIRED: erasures filled                            */
+    uint32_t    blocks;         /* REPAIRED: blocks that had erasures                   */
+    uint32_t    had_line;       /* 1: the decode was a line with crc_ok = 0; 0: an S1 abort */
+    wmb_decoded line;           /* REPAIRED: the repaired line (status WMB_DEC_LINE)    */
+} wmb_repaired;
+
+/* Repair one candidate on the host, e_max = 0 (nothing is repaired: WMB_REP_NONE) .. 3; else WMB_E_INVAL. */
+int wmb_frame_repair(const wmb_frame *f, uint32_t e_max, wmb_repaired *out);
+
+/* The same repair done on the device (kernel K4R behind K4), n frames at once. */
+int wmb_frame_repair_device(wmb_ctx *ctx, const wmb_frame *frames, size_t n, uint32_t e_max, wmb_repaired *out);
 
 /* CRC-16, polynomial 0x3D65, complemented (t1_c1_packet_decoder.h:463-469) */
 uint16_t wmb_crc16(const uint8_t *data, size_t n);

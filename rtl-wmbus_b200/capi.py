@@ -24,6 +24,24 @@ class WmbFrame(C.Structure):
                 ("nbits", C.c_uint32), ("bits", C.POINTER(C.c_uint32))]
 
 
+class WmbDecoded(C.Structure):
+    """wmb_decoded (include/wmbus_b200_framer.h): one candidate's decode"""
+    _fields_ = [("status", C.c_int), ("consumed", C.c_uint32), ("end_sample", C.c_uint64), ("mode", C.c_char * 3),
+                ("crc_ok", C.c_uint8), ("ok_3of6", C.c_uint8), ("packet_rssi", C.c_uint32),
+                ("current_rssi", C.c_uint32), ("serial", C.c_uint32), ("len", C.c_uint32),
+                ("datagram", C.c_uint8 * 292)]
+
+
+class WmbRepaired(C.Structure):
+    """wmb_repaired (include/wmbus_b200_framer.h): one candidate's erasure repair"""
+    _fields_ = [("outcome", C.c_int), ("erasures", C.c_uint32), ("blocks", C.c_uint32), ("had_line", C.c_uint32),
+                ("line", WmbDecoded)]
+
+
+# wmb_repaired.outcome
+REP_NONE, REP_REPAIRED, REP_AMBIGUOUS, REP_TOO_MANY, REP_UNREPAIRABLE, REP_TRUNCATED = range(6)
+
+
 class WmbLineInfo(C.Structure):
     _fields_ = [("sync_sample", C.c_uint64), ("end_sample", C.c_uint64), ("chain", C.c_uint8), ("algo", C.c_uint8),
                 ("crc_ok", C.c_uint8), ("valid", C.c_uint8), ("n", C.c_uint32), ("sum", C.c_int64),
@@ -152,6 +170,8 @@ def _bind(lib):
     lib.wmb_boundary_state.restype = C.c_long
     lib.wmb_pending_before.argtypes = [C.c_void_p, C.c_uint64]
     lib.wmb_pending_before.restype = C.c_long
+    lib.wmb_frame_repair.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p]
+    lib.wmb_frame_repair_device.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint32, C.c_void_p]
     return lib
 
 
@@ -345,6 +365,26 @@ class WmbusB200:
 
     def decode_frames(self, arr, n):
         self._check(self.lib.wmb_decode_frames(self._ctx, arr, n))
+
+    def repair_frames(self, arr, n, e_max=2, device=True):
+        """Erasure repair (wmb_frame_repair_device, or the host twin wmb_frame_repair with device=False) of the first n
+        frames of arr, e.g. what poll() returned with manual_frames=1.  Returns an array of n WmbRepaired; lines of the
+        repaired ones format with repaired_line()."""
+        out = (WmbRepaired * max(n, 1))()
+        if device:
+            self._check(self.lib.wmb_frame_repair_device(self._ctx, C.addressof(arr), n, e_max, C.addressof(out)))
+        else:
+            for i in range(n):
+                self._check(self.lib.wmb_frame_repair(C.addressof(arr[i]), e_max, C.addressof(out[i])))
+        return out
+
+    def repaired_line(self, r, algo_prefix=b"", timestamp=b"TS"):
+        """the line of a repaired frame in the stdout format (without its newline)"""
+        fmt = C.CFUNCTYPE(C.c_size_t, C.c_void_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_size_t)(("wmb_format_line",
+                                                                                                  self.lib))
+        buf = C.create_string_buffer(2048)
+        k = fmt(C.addressof(r.line), algo_prefix, timestamp, buf, 2048)
+        return buf.raw[:k].decode().rstrip("\n")
 
     def take_lines(self, timestamp_mode=1, info=False, quality=False):
         """info=True: (lines, records), records a numpy structured array of wmb_line_info, one per line.

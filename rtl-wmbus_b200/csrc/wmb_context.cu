@@ -25,6 +25,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 #include <string>
 #include <vector>
 #include <thread>
@@ -2228,11 +2229,9 @@ static int book_device_frames(wmb_ctx *c, const FrameHdr *hdr, const DecHdr *dec
         [&](size_t k, wmb_decoded &o) { decoded_from(dec[idx[k]], hdr[idx[k]].sync_sample, pool, o); });
 }
 
-/* Test hook (declared in wmb_framer.h, not part of the public ABI): run K4 on caller-made frames so
- * that the device framer can be compared with its host twin candidate by candidate. */
-extern "C" int wmb_frame_decode_device(wmb_ctx *c, const wmb_frame *frames, size_t n, wmb_decoded *out)
+/* caller-made frames into the context's frame tables, and K4 on them; the datagram pool starts empty */
+static int upload_and_decode(wmb_ctx *c, const wmb_frame *frames, size_t n)
 {
-    if (!c || !frames || !out) return set_err(WMB_E_INVAL, "null argument");
     CUDA_TRY(cudaSetDevice(c->device));
     TRY(ctx_alloc(c));
     if (n > c->cand_cap) return set_err(WMB_E_INVAL, "too many frames");
@@ -2254,12 +2253,74 @@ extern "C" int wmb_frame_decode_device(wmb_ctx *c, const wmb_frame *frames, size
     memset(&q, 0, sizeof(q));
     q.hdr = c->hdr.d; q.n = (uint32_t)n; q.words = c->d_words; q.dec = c->dec.d;
     q.pool = c->pool.d; q.pool_cap = (uint32_t)c->pool.cap; q.pool_n = GD_FIELD(c, pool_n); q.errors = c->d_errors;
-    TRY(launch_k4(c, q));
+    return launch_k4(c, q);
+}
+
+/* Test hook (declared in wmb_framer.h, not part of the public ABI): run K4 on caller-made frames so
+ * that the device framer can be compared with its host twin candidate by candidate. */
+extern "C" int wmb_frame_decode_device(wmb_ctx *c, const wmb_frame *frames, size_t n, wmb_decoded *out)
+{
+    if (!c || !frames || !out) return set_err(WMB_E_INVAL, "null argument");
+    TRY(upload_and_decode(c, frames, n));
     TRY(c->dec.fetch(0, 0, 0, (uint32_t)n, c->cs));
     TRY(c->pool.fetch(0, 0, 0, (uint32_t)std::min<size_t>(c->pool.cap, 1u << 24), c->cs));
     CUDA_TRY(cudaMemsetAsync(GD_FIELD(c, pool_n), 0, 4, c->cs));
     CUDA_TRY(cudaStreamSynchronize(c->cs));
     for (size_t i = 0; i < n; i++) decoded_from(c->dec.h[i], frames[i].sync_sample, c->pool.h, out[i]);
+    return WMB_OK;
+}
+
+static int launch_k4r(wmb_ctx *c, const K4RParams &p)
+{
+#ifdef WMB_HOSTSIM
+    static K4RSmem sm;                  /* the block's phases need real barriers: one simulated thread */
+    hs_for(p.n, [&](uint32_t i) { k4r_repair(p, i, 0, 1, sm); });
+#else
+    k4r_repair_kernel<<<p.n ? p.n : 1, K4_THREADS, 0, c->cs>>>(p);
+    CUDA_TRY(cudaGetLastError());
+#endif
+    c->st.kernel_launches += 1;
+    return WMB_OK;
+}
+
+/* Test hook (wmbus_b200_framer.h): K4 and the erasure repair K4R on caller-made frames, to compare with the host twin
+ * wmb_frame_repair() frame by frame. */
+extern "C" int wmb_frame_repair_device(wmb_ctx *c, const wmb_frame *frames, size_t n, uint32_t e_max, wmb_repaired *out)
+{
+    static const char modes[3][3] = { "T1", "C1", "S1" };
+    if (!c || !frames || !out) return set_err(WMB_E_INVAL, "null argument");
+    if (e_max > K4R_MAX_ERASURES) return set_err(WMB_E_INVAL, "e_max %u out of range 0..%d", e_max, K4R_MAX_ERASURES);
+    memset(out, 0, n * sizeof(*out));
+    if (e_max == 0 || n == 0) return WMB_OK;
+    TRY(upload_and_decode(c, frames, n));
+    RepHdr *d_rep = nullptr;
+    if (cudaMalloc((void **)&d_rep, n * sizeof(RepHdr)) != cudaSuccess) return set_err(WMB_E_NOMEM, "cudaMalloc of the repair table failed");
+    std::unique_ptr<RepHdr, cudaError_t (*)(void *)> guard(d_rep, cudaFree);
+    K4RParams r;
+    memset(&r, 0, sizeof(r));
+    r.hdr = c->hdr.d; r.dec = c->dec.d; r.n = (uint32_t)n; r.words = c->d_words; r.rep = d_rep;
+    r.pool = c->pool.d; r.pool_cap = (uint32_t)c->pool.cap; r.pool_n = GD_FIELD(c, pool_n); r.errors = c->d_errors;
+    r.e_max = e_max;
+    TRY(launch_k4r(c, r));
+    std::vector<RepHdr> rep(n);
+    CUDA_TRY(cudaMemcpyAsync(rep.data(), d_rep, n * sizeof(RepHdr), cudaMemcpyDeviceToHost, c->cs));
+    TRY(c->pool.fetch(0, 0, 0, (uint32_t)std::min<size_t>(c->pool.cap, 1u << 24), c->cs));
+    CUDA_TRY(cudaMemsetAsync(GD_FIELD(c, pool_n), 0, 4, c->cs));
+    CUDA_TRY(cudaStreamSynchronize(c->cs));
+    for (size_t i = 0; i < n; i++) {
+        const RepHdr &h = rep[i];
+        wmb_repaired &o = out[i];
+        o.outcome = h.outcome; o.had_line = h.had_line;
+        if (h.outcome != K4R_REPAIRED) continue;
+        if (h.data_off == 0xFFFFFFFFu) return set_err(WMB_E_OVERFLOW, "datagram pool full: hand in fewer frames at once");
+        o.erasures = h.erasures; o.blocks = h.blocks;
+        wmb_decoded &d = o.line;
+        d.status = WMB_DEC_LINE; d.consumed = h.consumed; d.end_sample = frames[i].sync_sample + h.end_off;
+        memcpy(d.mode, modes[frames[i].chain == WMB_CHAIN_T1C1 ? 0 : 2], 3);
+        d.crc_ok = 1; d.ok_3of6 = 1; d.packet_rssi = h.packet_rssi; d.current_rssi = h.current_rssi;
+        d.serial = h.serial; d.len = h.len;
+        memcpy(d.datagram, c->pool.h + h.data_off, h.len);
+    }
     return WMB_OK;
 }
 

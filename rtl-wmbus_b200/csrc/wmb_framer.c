@@ -8,6 +8,7 @@
  *   :463-536 (block CRCs), :551-636 (CRC strip)   and   s1_packet_decoder.h:132-282.
  */
 #include "wmb_framer.h"
+#include "wmb_frame_a.h"
 
 #include <stdio.h>
 #include <string.h>
@@ -262,6 +263,131 @@ void wmb_frame_decode(const wmb_frame *f, wmb_decoded *d)
     if (WMB_BIT_RSSI(f->bits[0]) < CAPTURE_THRESHOLD) { c.stop = STOP_ABORT; stopped(&c, d); return; }
     if (f->chain == WMB_CHAIN_T1C1) decode_t1c1(&c, d);
     else decode_s1(&c, d);
+}
+
+/* ---- erasure repair (definition in wmbus_b200_framer.h; device twin: K4R, wmb_kernels.cuh) ------- */
+
+#define REP_MAX_ERASURES 3u
+
+typedef struct erasure {
+    unsigned byte, shift, n;            /* the byte, where the filling goes in it, how many fillings */
+    uint8_t  fill[6];
+} erasure;
+
+/* the code words at Hamming distance 1 from a 6-bit word, lowest flipped bit first: 2..4 of them for an invalid word of
+ * weight 2 or 4, none for weight 0, 1, 5, 6 or an invalid word of weight 3 */
+static unsigned fillings_3of6(unsigned w, uint8_t *fill)
+{
+    unsigned n = 0;
+    for (unsigned k = 0; k < 6; k++) {
+        const unsigned v = nibble_3of6(w ^ (1u << k));
+        if (v != 0xFFu) fill[n++] = (uint8_t)v;
+    }
+    return n;
+}
+
+static unsigned bits_at(const wmb_bit *b, unsigned first, unsigned n)      /* MSB first */
+{
+    unsigned v = 0;
+    for (unsigned k = 0; k < n; k++) v = (v << 1) | WMB_BIT_DATA(b[first + k]);
+    return v;
+}
+
+int wmb_frame_repair(const wmb_frame *f, uint32_t e_max, wmb_repaired *out)
+{
+    memset(out, 0, sizeof(*out));
+    if (e_max > REP_MAX_ERASURES) return WMB_E_INVAL;
+    if (e_max == 0 || f->nbits == 0) return WMB_OK;
+    const wmb_bit *b = f->bits;
+    const int t1 = f->chain == WMB_CHAIN_T1C1;
+
+    /* candidates: a line whose CRCs fail, an S1 abort on a Manchester violation after the L-field byte */
+    wmb_decoded d;
+    wmb_frame_decode(f, &d);
+    if (d.status == WMB_DEC_LINE && !d.crc_ok) {
+        out->had_line = 1;
+        if (d.mode[0] == 'C') { out->outcome = WMB_REP_UNREPAIRABLE; return WMB_OK; }     /* NRZ: no erasures */
+    } else if (d.status == WMB_DEC_ABORT && !t1) {
+        const unsigned pos = d.consumed - 1;
+        if (pos < 18 || (pos & 1u) || WMB_BIT_DATA(b[pos]) != WMB_BIT_DATA(b[pos - 1])) return WMB_OK;
+    } else return WMB_OK;
+
+    unsigned L = 0;
+    if (t1) L = (nibble_3of6(bits_at(b, 1, 6)) << 4) | nibble_3of6(bits_at(b, 7, 6));
+    else for (unsigned k = 0; k < 8; k++) L = (L << 1) | WMB_BIT_DATA(b[2 + 2 * k]);
+    const unsigned len = wmb_tlg_length_format_a(L);
+    const unsigned P = 1 + (t1 ? 12u : 16u) * len;
+    if (f->nbits < P) { out->outcome = WMB_REP_TRUNCATED; return WMB_OK; }
+    if (len < 12) { out->outcome = WMB_REP_UNREPAIRABLE; return WMB_OK; }
+    for (unsigned i = 0; i + 1 < P; i++)
+        if (WMB_BIT_RSSI(b[i]) < CAPTURE_THRESHOLD) { out->outcome = WMB_REP_UNREPAIRABLE; return WMB_OK; }
+
+    /* the received bytes with their erasures zeroed, and the erasures in chip order */
+    uint8_t pkt[292];
+    static __thread erasure er[8 * 292];
+    unsigned ner = 0;
+    memset(pkt, 0, sizeof(pkt));
+    pkt[0] = (uint8_t)L;
+    for (unsigned l = 1; l < len; l++) {
+        unsigned v = 0;
+        if (t1) {
+            for (unsigned s = 0; s < 2; s++) {
+                const unsigned w = bits_at(b, 1 + 12 * l + 6 * s, 6), shift = s ? 0u : 4u, nib = nibble_3of6(w);
+                if (nib != 0xFFu) { v |= nib << shift; continue; }
+                erasure *e = &er[ner++];
+                e->byte = l; e->shift = shift; e->n = fillings_3of6(w, e->fill);
+                if (!e->n) { out->outcome = WMB_REP_UNREPAIRABLE; return WMB_OK; }
+            }
+        } else {
+            for (unsigned k = 0; k < 8; k++) {
+                const unsigned a = WMB_BIT_DATA(b[1 + 16 * l + 2 * k]), c = WMB_BIT_DATA(b[2 + 16 * l + 2 * k]);
+                if (a != c) { v |= c << (7 - k); continue; }
+                erasure *e = &er[ner++];
+                e->byte = l; e->shift = 7 - k; e->n = 2; e->fill[0] = 0; e->fill[1] = 1;
+            }
+        }
+        pkt[l] = (uint8_t)v;
+    }
+    const unsigned nblk = wmb_nblk_a(len);
+    for (unsigned j = 0, k = 0; j < nblk; j++) {
+        const unsigned off = wmb_blk_off_a(j), blk = wmb_blk_len_a(len, j);
+        unsigned ne = 0;
+        while (k < ner && er[k].byte < off + blk) { k++; ne++; }
+        if (ne > e_max) { out->outcome = WMB_REP_TOO_MANY; return WMB_OK; }
+    }
+
+    /* block by block, in frame order: exactly one filling (mixed radix, the block's first erasure lowest) passes */
+    unsigned k = 0, erasures = 0, blocks = 0;
+    for (unsigned j = 0; j < nblk; j++) {
+        const unsigned off = wmb_blk_off_a(j), blk = wmb_blk_len_a(len, j);
+        unsigned nf = 1, pass = 0, first = 0;
+        const erasure *e = &er[k];
+        unsigned ne = 0;
+        while (k < ner && er[k].byte < off + blk) { nf *= er[k].n; k++; ne++; }
+        for (unsigned i = 0; i < nf; i++) {
+            uint8_t q[18];
+            memcpy(q, pkt + off, blk);
+            for (unsigned m = 0, rest = i; m < ne; m++) {
+                q[e[m].byte - off] |= (uint8_t)(e[m].fill[rest % e[m].n] << e[m].shift);
+                rest /= e[m].n;
+            }
+            if (block_ok(q, blk)) { if (!pass) first = i; pass++; }
+        }
+        if (pass != 1) { out->outcome = pass ? WMB_REP_AMBIGUOUS : WMB_REP_UNREPAIRABLE; return WMB_OK; }
+        for (unsigned m = 0, rest = first; m < ne; m++) {
+            pkt[e[m].byte] |= (uint8_t)(e[m].fill[rest % e[m].n] << e[m].shift);
+            rest /= e[m].n;
+        }
+        erasures += ne; blocks += ne ? 1u : 0u;
+    }
+    if (!erasures) { out->outcome = WMB_REP_UNREPAIRABLE; return WMB_OK; }
+
+    const cursor c = { f, P - 1, 0 };
+    finish(&c, &out->line, t1 ? "T1" : "S1", pkt, len, 0, 0);
+    out->outcome = WMB_REP_REPAIRED;
+    out->erasures = erasures;
+    out->blocks = blocks;
+    return WMB_OK;
 }
 
 /* ---- output --------------------------------------------------------------------- */

@@ -1561,6 +1561,217 @@ WMB_D void k4_decode(const K4Params &p, uint32_t f, int tid, int nthr, K4Smem &s
     }
 }
 
+/* =========================================================================== */
+/* K4R: erasure repair of the candidates K4 has decoded (definition in wmbus_b200_framer.h, host twin wmb_frame_repair()
+ * in wmb_framer.c).  One warp per candidate.  The lanes decode the bytes and mark the erasures in parallel; then, block
+ * by block, each lane checks the CRC of one filling at a time (at most 4^3 = 64), the passes are counted with an atomic
+ * and the lowest passing filling is kept.  It reads K4's verdict from the DecHdr table, so K4 itself is unchanged. */
+#include "wmb_frame_a.h"
+
+#define K4R_MAX_ERASURES 3
+enum { K4R_NONE = 0, K4R_REPAIRED = 1, K4R_AMBIGUOUS = 2, K4R_TOO_MANY = 3, K4R_UNREPAIRABLE = 4, K4R_TRUNCATED = 5 };
+
+struct RepHdr {                     /* one per candidate, parallel to DecHdr, device -> host */
+    uint32_t consumed;              /* P: bits of the repaired telegram incl. the flagged one */
+    uint32_t end_off;               /* sample offset (from sync_sample) of bit P - 1       */
+    uint32_t serial;
+    uint32_t data_off;              /* byte offset of the repaired datagram in the pool (0xFFFFFFFF: no room) */
+    uint16_t len;                   /* datagram bytes after the CRC strip                  */
+    uint8_t  outcome;               /* K4R_*                                               */
+    uint8_t  erasures, blocks, had_line, packet_rssi, current_rssi;
+};
+
+struct K4RParams {
+    const FrameHdr *hdr; const DecHdr *dec; uint32_t n;
+    const uint32_t *words;
+    RepHdr *rep;
+    uint8_t *pool; uint32_t pool_cap; uint32_t *pool_n;
+    uint32_t *errors;
+    uint32_t e_max;                 /* 1..3 */
+};
+
+struct K4RSmem {
+    uint8_t  pkt[296];              /* the received bytes, erased nibbles / bits zero       */
+    uint8_t  em[296];               /* erased: T1 0x10 high nibble, 0x01 low nibble; S1 the bits of the erased pairs */
+    uint16_t sym[296];              /* T1: the two received 6-bit words, high << 6 | low   */
+    uint32_t bad;                   /* 1: rssi < 5 or a T1 word with no filling; 2: a block with too many erasures */
+    uint32_t npass;
+    int      best;
+    uint32_t ne, nf;                /* the current block's erasures and fillings           */
+    uint16_t er_byte[K4R_MAX_ERASURES];
+    uint8_t  er_shift[K4R_MAX_ERASURES], er_n[K4R_MAX_ERASURES], er_fill[K4R_MAX_ERASURES][4];
+    uint32_t data_off;
+};
+
+/* the code words at Hamming distance 1 from a 6-bit word, lowest flipped bit first: 2..4 of them for an invalid word of
+ * weight 2 or 4, none for weight 0, 1, 5, 6 or an invalid word of weight 3 */
+WMB_D uint32_t k4r_fillings(uint32_t w, uint8_t *fill)
+{
+    uint32_t n = 0;
+    for (uint32_t k = 0; k < 6; k++) {
+        const uint32_t v = wmb_dec3of6(w ^ (1u << k));
+        if (v != 0xFFu) fill[n++] = (uint8_t)v;
+    }
+    return n;
+}
+
+WMB_D void k4r_repair(const K4RParams &p, uint32_t f, int tid, int nthr, K4RSmem &sm)
+{
+    if (f >= p.n) return;
+    const FrameHdr h = p.hdr[f];
+    const DecHdr d = p.dec[f];
+    const uint32_t *b = p.words + h.word_off;
+    const uint32_t nbits = h.nbits;
+    const bool t1 = h.chain == WMB_CHAIN_T1C1;
+    RepHdr r;
+    r.consumed = 0; r.end_off = 0; r.serial = 0; r.data_off = 0; r.len = 0; r.outcome = K4R_NONE;
+    r.erasures = 0; r.blocks = 0; r.had_line = 0; r.packet_rssi = 0; r.current_rssi = 0;
+
+    /* candidates: a line whose CRCs fail, an S1 abort on a Manchester violation after the L-field byte */
+    if (nbits == 0 || d.status == K4_SKIP) { if (tid == 0) p.rep[f] = r; return; }
+    if (d.status == K4_LINE && !d.crc_ok) {
+        r.had_line = 1;
+        if (d.mode == 1) { r.outcome = K4R_UNREPAIRABLE; if (tid == 0) p.rep[f] = r; return; }   /* C1: no erasures */
+    } else if (d.status == K4_ABORT && !t1) {
+        const uint32_t pos = d.consumed - 1;
+        if (pos < 18 || (pos & 1u) || WMB_BIT_DATA(b[pos]) != WMB_BIT_DATA(b[pos - 1])) { if (tid == 0) p.rep[f] = r; return; }
+    } else { if (tid == 0) p.rep[f] = r; return; }
+
+    uint32_t L = 0;
+    if (t1) L = (wmb_dec3of6(k4_bits(b, 1, 6)) << 4) | wmb_dec3of6(k4_bits(b, 7, 6));
+    else for (uint32_t k = 0; k < 8; k++) L = (L << 1) | WMB_BIT_DATA(b[2 + 2 * k]);
+    const uint32_t len = wmb_tlg_len_a(L);
+    const uint32_t P = 1 + (t1 ? 12u : 16u) * len;
+    if (nbits < P) { r.outcome = K4R_TRUNCATED; if (tid == 0) p.rep[f] = r; return; }
+    if (len < 12) { r.outcome = K4R_UNREPAIRABLE; if (tid == 0) p.rep[f] = r; return; }
+
+    if (tid == 0) sm.bad = 0;
+    K4_SYNC();
+    for (uint32_t i = (uint32_t)tid; i + 1 < P; i += (uint32_t)nthr)
+        if (WMB_BIT_RSSI(b[i]) < K4_CAPTURE_THRESHOLD) k4_sor(&sm.bad, 1u);
+    for (uint32_t l = (uint32_t)tid; l < len; l += (uint32_t)nthr) {
+        uint32_t v = 0, em = 0, sym = 0;
+        if (l == 0) v = L;
+        else if (t1) {
+            const uint32_t hi6 = k4_bits(b, 1 + 12 * l, 6), lo6 = k4_bits(b, 7 + 12 * l, 6);
+            const uint32_t hv = wmb_dec3of6(hi6), lv = wmb_dec3of6(lo6);
+            uint8_t fill[6];
+            if (hv == 0xFFu) { em |= 0x10u; if (!k4r_fillings(hi6, fill)) k4_sor(&sm.bad, 1u); } else v |= hv << 4;
+            if (lv == 0xFFu) { em |= 0x01u; if (!k4r_fillings(lo6, fill)) k4_sor(&sm.bad, 1u); } else v |= lv;
+            sym = (hi6 << 6) | lo6;
+        } else {
+            for (uint32_t k = 0; k < 8; k++) {
+                const uint32_t a = WMB_BIT_DATA(b[1 + 16 * l + 2 * k]), c = WMB_BIT_DATA(b[2 + 16 * l + 2 * k]);
+                if (a == c) em |= 0x80u >> k;
+                else v |= c << (7 - k);
+            }
+        }
+        sm.pkt[l] = (uint8_t)v; sm.em[l] = (uint8_t)em; sm.sym[l] = (uint16_t)sym;
+    }
+    K4_SYNC();
+    const uint32_t nblk = wmb_nblk_a(len);
+    for (uint32_t j = (uint32_t)tid; j < nblk; j += (uint32_t)nthr) {
+        const uint32_t off = wmb_blk_off_a(j), blk = wmb_blk_len_a(len, j);
+        uint32_t ne = 0;
+        for (uint32_t i = 0; i < blk; i++) ne += (uint32_t)wmb_popc(sm.em[off + i]);
+        if (ne > p.e_max) k4_sor(&sm.bad, 2u);
+    }
+    K4_SYNC();
+    const uint32_t bad = sm.bad;
+    uint32_t outcome = (bad & 1u) ? K4R_UNREPAIRABLE : (bad & 2u) ? K4R_TOO_MANY : K4R_NONE;
+
+    /* block by block, in frame order: exactly one filling must pass the CRC */
+    uint32_t erasures = 0, blocks = 0;
+    for (uint32_t j = 0; j < nblk && outcome == K4R_NONE; j++) {
+        const uint32_t off = wmb_blk_off_a(j), blk = wmb_blk_len_a(len, j);
+        if (tid == 0) {
+            uint32_t ne = 0, nf = 1;
+            for (uint32_t i = 0; i < blk; i++) {
+                const uint32_t l = off + i, em = sm.em[l];
+                if (!em) continue;
+                if (t1) {
+                    for (uint32_t s = 0; s < 2; s++) {
+                        const uint32_t shift = s ? 0u : 4u;
+                        if (!(em & (1u << shift))) continue;
+                        sm.er_byte[ne] = (uint16_t)l; sm.er_shift[ne] = (uint8_t)shift;
+                        sm.er_n[ne] = (uint8_t)k4r_fillings(s ? sm.sym[l] & 63u : sm.sym[l] >> 6, sm.er_fill[ne]);
+                        nf *= sm.er_n[ne]; ne++;
+                    }
+                } else {
+                    for (uint32_t k = 0; k < 8; k++) {
+                        if (!(em & (0x80u >> k))) continue;
+                        sm.er_byte[ne] = (uint16_t)l; sm.er_shift[ne] = (uint8_t)(7 - k); sm.er_n[ne] = 2;
+                        sm.er_fill[ne][0] = 0; sm.er_fill[ne][1] = 1;
+                        nf *= 2; ne++;
+                    }
+                }
+            }
+            sm.ne = ne; sm.nf = nf; sm.npass = 0; sm.best = 0x7FFFFFFF;
+        }
+        K4_SYNC();
+        const uint32_t ne = sm.ne, nf = sm.nf;
+        for (uint32_t i = (uint32_t)tid; i < nf; i += (uint32_t)nthr) {
+            uint8_t q[18];
+            for (uint32_t k = 0; k < blk; k++) q[k] = sm.pkt[off + k];
+            uint32_t rest = i;                                   /* mixed radix, the block's first erasure lowest */
+            for (uint32_t e = 0; e < ne; e++) {
+                q[sm.er_byte[e] - off] |= (uint8_t)(sm.er_fill[e][rest % sm.er_n[e]] << sm.er_shift[e]);
+                rest /= sm.er_n[e];
+            }
+            if (k4_block_ok(q, blk)) { k4_gadd(&sm.npass, 1u); k4_smin(&sm.best, (int)i); }
+        }
+        K4_SYNC();
+        const uint32_t npass = sm.npass;
+        if (npass != 1) outcome = npass ? K4R_AMBIGUOUS : K4R_UNREPAIRABLE;
+        else {
+            if (tid == 0) {
+                uint32_t rest = (uint32_t)sm.best;
+                for (uint32_t e = 0; e < ne; e++) {
+                    sm.pkt[sm.er_byte[e]] |= (uint8_t)(sm.er_fill[e][rest % sm.er_n[e]] << sm.er_shift[e]);
+                    rest /= sm.er_n[e];
+                }
+            }
+            erasures += ne; blocks += ne ? 1u : 0u;
+        }
+        K4_SYNC();
+    }
+    if (outcome == K4R_NONE) outcome = erasures ? K4R_REPAIRED : K4R_UNREPAIRABLE;
+    r.outcome = (uint8_t)outcome;
+    if (outcome != K4R_REPAIRED) { if (tid == 0) p.rep[f] = r; return; }
+
+    /* the repaired telegram: CRC-stripped datagram (format A, :551-592) into the pool */
+    const uint32_t out_len = len - 2 * nblk;
+    if (tid == 0) {
+        const uint32_t room = (out_len + 3u) & ~3u;
+        uint32_t off = k4_gadd(p.pool_n, room);
+        if (off > p.pool_cap || room > p.pool_cap - off) {
+#ifdef WMB_HOSTSIM
+            *p.errors |= 8u;
+#else
+            atomicOr(p.errors, 8u);
+#endif
+            off = 0xFFFFFFFFu;
+        }
+        sm.data_off = off;
+    }
+    K4_SYNC();
+    const uint32_t data_off = sm.data_off;
+    if (data_off != 0xFFFFFFFFu)
+        for (uint32_t i = (uint32_t)tid; i < out_len; i += (uint32_t)nthr)
+            p.pool[data_off + i] = sm.pkt[wmb_strip_src_a(i)];
+    if (tid == 0) {
+        r.consumed = P;
+        r.end_off = WMB_BIT_OFFSET(b[P - 1]);
+        r.serial = (uint32_t)sm.pkt[4] | ((uint32_t)sm.pkt[5] << 8) | ((uint32_t)sm.pkt[6] << 16) | ((uint32_t)sm.pkt[7] << 24);
+        r.data_off = data_off;
+        r.len = (uint16_t)(data_off == 0xFFFFFFFFu ? 0 : out_len);
+        r.erasures = (uint8_t)erasures; r.blocks = (uint8_t)blocks;
+        r.packet_rssi = (uint8_t)WMB_BIT_RSSI(b[1]);
+        r.current_rssi = (uint8_t)WMB_BIT_RSSI(b[P - 1]);
+        p.rep[f] = r;
+    }
+}
+
 /* wmb_reset: a new capture starts -- carried states, stream bookkeeping, gather state and error flags back to their
  * initial values, in stream order (no host copies, no synchronisation) */
 struct ResetParams {
@@ -1940,6 +2151,14 @@ __global__ void __launch_bounds__(K4_THREADS) k4_decode_kernel(const K4Params p)
     const uint32_t n = k4_count(p);
     for (uint32_t f = blockIdx.x; f < n; f += gridDim.x) {
         k4_decode(p, f, threadIdx.x, blockDim.x, sm);
+        __syncthreads();
+    }
+}
+__global__ void __launch_bounds__(K4_THREADS) k4r_repair_kernel(const K4RParams p)
+{
+    __shared__ K4RSmem sm;
+    for (uint32_t f = blockIdx.x; f < p.n; f += gridDim.x) {
+        k4r_repair(p, f, threadIdx.x, blockDim.x, sm);
         __syncthreads();
     }
 }

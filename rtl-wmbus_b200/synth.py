@@ -111,6 +111,7 @@ class Emitter:
     manufacturer: int = 0x5068
     seed: int = 1
     sync_flips: tuple = ()       # chips of the access code sent inverted in every telegram, counted back from its last chip
+    data_flips: tuple = ()       # chips after the access code sent inverted in every telegram (0: the L-field's first chip)
     chip_rate: float = field(init=False)
 
     def __post_init__(self):
@@ -136,10 +137,13 @@ class Emitter:
 
     def chips(self, k: int) -> np.ndarray:
         c = self._chips(k)
+        end = 2 * 40 + len(SYNC_S1) if self.mode == "S1" else 2 * 24 + len(SYNC_T1C1)
         if self.sync_flips:      # a receiver accepts these only with access-code errors allowed (wmb_set_receiver)
-            end = 2 * 40 + len(SYNC_S1) if self.mode == "S1" else 2 * 24 + len(SYNC_T1C1)
             c = c.copy()
             c[end - 1 - np.asarray(self.sync_flips)] ^= 1
+        if self.data_flips:      # T1 symbols / S1 chip pairs that lose a chip: erasures for wmb_frame_repair
+            c = c.copy()
+            c[end + np.asarray(self.data_flips)] ^= 1
         return c
 
     def _chips(self, k: int) -> np.ndarray:
