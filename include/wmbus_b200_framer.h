@@ -84,6 +84,37 @@ int wmb_frame_repair(const wmb_frame *f, uint32_t e_max, wmb_repaired *out);
 /* The same repair done on the device (kernel K4R behind K4), n frames at once. */
 int wmb_frame_repair_device(wmb_ctx *ctx, const wmb_frame *frames, size_t n, uint32_t e_max, wmb_repaired *out);
 
+/* ---- erasure repair on the streaming path (wmb_push / wmb_push_device / wmb_process*) ------------------------------
+ * Off by default.  wmb_set_repair(ctx, e_max), e_max 1..3, turns it on (0: off); e_max > 3 is WMB_E_INVAL, and so is a
+ * manual_frames context (it repairs its polled frames with wmb_frame_repair_device).  Like wmb_set_line_quality it is
+ * valid before the first push or right after wmb_reset / wmb_seek (else WMB_E_STATE) and survives both.
+ *   1. Candidates: exactly the frames that the context's own framer books -- the stream-order rule accepted them (a
+ *      match that lies inside a telegram already accepted on its stream is ignored) and the match lies in the line
+ *      window (wmb_set_line_window) -- whose decode is a candidate of wmb_frame_repair above: a line with crc_ok = 0, or
+ *      an S1 abort on a Manchester violation after the L-field.
+ *   2. Each is repaired as wmb_frame_repair defines, on its bit list once that holds P bits.  No record is made when the
+ *      list ends before P (a run-length reset, the end of input) or when the outcome is NONE: every record is REPAIRED,
+ *      AMBIGUOUS, TOO_MANY or UNREPAIRABLE.  (A REPAIRED one whose datagram found no room in the batch's pool is not
+ *      reported either; the batch counts as an overflow batch.)
+ *   3. Records come out in (end_sample, chain * 2 + (algo == t2a), sync_sample) order; end_sample is the sample of bit
+ *      P - 1 (of a C1 line, which is never repaired, its last bit), and a record becomes final in the gather whose batch
+ *      produced that bit.
+ *   4. A repair is an additional report: the lines and their info / quality records, the bursts, the band survey, the
+ *      busy bookkeeping and every wmb_stats field but kernel_launches (one more per gather) and d2h_bytes stay as they
+ *      are with repair off. */
+typedef struct wmb_repair_record {
+    uint64_t     sync_sample;   /* access-code match (decimated sample)                 */
+    uint64_t     end_sample;    /* decimated sample of bit P - 1 (a C1 line: its last bit) */
+    uint8_t      chain, algo;   /* WMB_CHAIN_*, WMB_ALGO_*                              */
+    uint8_t      reserved[6];
+    wmb_repaired repair;        /* outcome; REPAIRED: the repaired line                 */
+} wmb_repair_record;
+
+int wmb_set_repair(wmb_ctx *ctx, uint32_t e_max);
+
+/* Hand out at most cap of the queued records, in order; the rest stay queued.  *n: records written. */
+int wmb_take_repairs(wmb_ctx *ctx, wmb_repair_record *out, size_t cap, size_t *n);
+
 /* CRC-16, polynomial 0x3D65, complemented (t1_c1_packet_decoder.h:463-469) */
 uint16_t wmb_crc16(const uint8_t *data, size_t n);
 

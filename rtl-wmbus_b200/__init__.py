@@ -10,10 +10,10 @@ missing.
 Import with ``importlib.import_module("rtl-wmbus_b200")`` (the directory name carries the
 reference's hyphen).
 """
-from .capi import (WmbOpts, WmbStats, WmbFrame, WmbLineInfo, WmbDecoded, WmbRepaired, WmbusB200, load_library, library_path, build,
+from .capi import (WmbOpts, WmbStats, WmbFrame, WmbLineInfo, WmbDecoded, WmbRepaired, WmbRepairRecord, WmbusB200, load_library, library_path, build,
                    opts_from_flags, line_info_dtype, burst_dtype, BURST_CONTINUED, BURST_CUT, BURST_AT_END, spectrum_dtype,
                    line_quality_dtype, burst_quality_dtype, LIB_NAME)
 
-__all__ = ["WmbOpts", "WmbStats", "WmbFrame", "WmbLineInfo", "WmbDecoded", "WmbRepaired", "WmbusB200", "load_library", "library_path", "build",
+__all__ = ["WmbOpts", "WmbStats", "WmbFrame", "WmbLineInfo", "WmbDecoded", "WmbRepaired", "WmbRepairRecord", "WmbusB200", "load_library", "library_path", "build",
            "opts_from_flags", "line_info_dtype", "burst_dtype", "BURST_CONTINUED", "BURST_CUT", "BURST_AT_END", "spectrum_dtype",
            "line_quality_dtype", "burst_quality_dtype", "LIB_NAME"]

@@ -42,6 +42,16 @@ class WmbRepaired(C.Structure):
 REP_NONE, REP_REPAIRED, REP_AMBIGUOUS, REP_TOO_MANY, REP_UNREPAIRABLE, REP_TRUNCATED = range(6)
 
 
+class WmbRepairRecord(C.Structure):
+    """wmb_repair_record (include/wmbus_b200_framer.h): the repair of one candidate of the streaming framer"""
+    _fields_ = [("sync_sample", C.c_uint64), ("end_sample", C.c_uint64), ("chain", C.c_uint8), ("algo", C.c_uint8),
+                ("reserved", C.c_uint8 * 6), ("repair", WmbRepaired)]
+
+    @property
+    def line(self):
+        return self.repair.line
+
+
 class WmbLineInfo(C.Structure):
     _fields_ = [("sync_sample", C.c_uint64), ("end_sample", C.c_uint64), ("chain", C.c_uint8), ("algo", C.c_uint8),
                 ("crc_ok", C.c_uint8), ("valid", C.c_uint8), ("n", C.c_uint32), ("sum", C.c_int64),
@@ -172,6 +182,8 @@ def _bind(lib):
     lib.wmb_pending_before.restype = C.c_long
     lib.wmb_frame_repair.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p]
     lib.wmb_frame_repair_device.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint32, C.c_void_p]
+    lib.wmb_set_repair.argtypes = [C.c_void_p, C.c_uint32]
+    lib.wmb_take_repairs.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
     return lib
 
 
@@ -230,10 +242,12 @@ class WmbusB200:
     spectrum=(bins, blocks_per_record): the band survey, see wmb_set_spectrum() (None: off, the default); it survives
     reset() and seek().  take_spectrum() hands out the closed records.
     quality=True: the signal-quality report, see wmb_set_line_quality() (off by default); it survives reset() and
-    seek().  take_lines(quality=True) and take_bursts(quality=True) hand out its records."""
+    seek().  take_lines(quality=True) and take_bursts(quality=True) hand out its records.
+    repair=e_max (1..3): erasure repair of the framer's T1 / S1 candidates, see wmb_set_repair() (0: off, the default);
+    it survives reset() and seek().  take_repairs() hands out its records."""
 
     def __init__(self, flags: str = "", device: int = 0, lib=None, clock_lock=None, access_code_errors=None,
-                 burst_level=None, spectrum=None, quality=False, **tuning):
+                 burst_level=None, spectrum=None, quality=False, repair=0, **tuning):
         self.lib = lib or load_library()
         self.opts = opts_from_flags(self.lib, flags, **tuning)
         self._ctx = C.c_void_p()
@@ -266,6 +280,12 @@ class WmbusB200:
         if quality:
             try:
                 self.set_line_quality(True)
+            except Exception:
+                self.close()
+                raise
+        if repair:
+            try:
+                self.set_repair(repair)
             except Exception:
                 self.close()
                 raise
@@ -379,7 +399,8 @@ class WmbusB200:
         return out
 
     def repaired_line(self, r, algo_prefix=b"", timestamp=b"TS"):
-        """the line of a repaired frame in the stdout format (without its newline)"""
+        """the line of a repaired frame (a WmbRepaired, or a WmbRepairRecord of take_repairs()) in the stdout format
+        (without its newline)"""
         fmt = C.CFUNCTYPE(C.c_size_t, C.c_void_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_size_t)(("wmb_format_line",
                                                                                                   self.lib))
         buf = C.create_string_buffer(2048)
@@ -470,6 +491,23 @@ class WmbusB200:
     def set_line_quality(self, on: bool):
         """signal-quality report on / off (before the first push, or after reset/seek)"""
         self._check(self.lib.wmb_set_line_quality(self._ctx, 1 if on else 0))
+
+    def set_repair(self, e_max: int):
+        """erasure repair of the streaming framer's candidates, e_max 1..3 (0 = off; before the first push, or after
+        reset/seek)"""
+        self._check(self.lib.wmb_set_repair(self._ctx, e_max))
+
+    def take_repairs(self, cap=1 << 12):
+        """the repair records not taken yet, in (end_sample, chain * 2 + (algo == t2a), sync_sample) order: a list of
+        WmbRepairRecord; the lines of the REPAIRED ones format with repaired_line()"""
+        out = []
+        while True:
+            arr = (WmbRepairRecord * cap)()
+            n = C.c_size_t(0)
+            self._check(self.lib.wmb_take_repairs(self._ctx, arr, cap, C.byref(n)))
+            out += list(arr[:n.value])
+            if n.value < cap:
+                return out
 
     def set_spectrum(self, bins: int, blocks_per_record: int):
         """band survey: bins 256 .. 2048 (0 = off), blocks per record (before the first push, or after reset/seek)"""

@@ -39,6 +39,12 @@
  *   WMBUS_B200_BURST_QUALITY=<path> (with WMBUS_B200_BURSTS) write one record per burst piece, in the burst file's
  *                              order: CHAIN;START_SAMPLE;DEVIATION_HZ;EYE_SNR_DB (wmb_burst_quality; nan where not valid).
  *   Either turns the quality report on (wmb_set_line_quality).  A path that cannot be opened is an error at start-up.
+ *   WMBUS_B200_REPAIRED=<path> repair T1 and S1 telegrams that lost a few chips (wmb_set_repair) and write the line of
+ *                              each repaired one, formatted as stdout's lines are (with the rla; / t2a; prefix under -v and
+ *                              the wall-clock timestamp of the hand-over's stdout lines), flushed with stdout.
+ *   WMBUS_B200_REPAIR_ERASURES=<n>  erasures repaired per CRC block, 1..3 (default 1: the lowest rate of wrong repairs,
+ *                              DESIGN.md 8).  A path that cannot be opened, a bad value, or this variable without
+ *                              WMBUS_B200_REPAIRED is an error at start-up.  stdout does not change.
  */
 #define _GNU_SOURCE
 #include <errno.h>
@@ -54,6 +60,7 @@
 #include <unistd.h>
 
 #include "wmbus_b200.h"
+#include "wmbus_b200_framer.h"
 
 static void print_usage(const char *program_name)
 {
@@ -242,16 +249,45 @@ static void emit_spectrum(wmb_ctx *ctx)
     fflush(g_spec_file);
 }
 
+/* WMBUS_B200_REPAIRED: the line of each REPAIRED record, with the timestamp of the hand-over's stdout lines */
+static FILE *g_rep_file = NULL;
+#define REP_CAP 256
+static wmb_repair_record g_reps[REP_CAP];
+
+static void emit_repairs(wmb_ctx *ctx, const char *ts, int show_algorithm)
+{
+    if (!g_rep_file) return;
+    for (;;) {
+        size_t n = 0;
+        if (wmb_take_repairs(ctx, g_reps, REP_CAP, &n) != WMB_OK || !n) break;
+        for (size_t i = 0; i < n; i++) {
+            const wmb_repair_record *r = &g_reps[i];
+            if (r->repair.outcome != WMB_REP_REPAIRED) continue;
+            char line[1024];
+            const char *prefix = show_algorithm ? (r->algo == WMB_ALGO_RLA ? "rla;" : "t2a;") : "";
+            fwrite(line, 1, wmb_format_line(&r->repair.line, prefix, ts, line, sizeof(line)), g_rep_file);
+        }
+        if (n < REP_CAP) break;
+    }
+    fflush(g_rep_file);
+}
+
 static int emit_lines(wmb_ctx *ctx, char *out, size_t outcap, int show_algorithm)
 {
     emit_bursts(ctx);
     emit_spectrum(ctx);
+    /* the repaired lines carry the hand-over's wall-clock time, taken as its stdout lines are formatted */
+    char ts[64];
+    wmb_make_time_string(ts, sizeof(ts));
     for (;;) {
         size_t nl = 0;
         const size_t n = g_info_file || g_qual_file
             ? wmb_take_lines_quality(ctx, out, outcap, &nl, 0, g_info_file ? g_info : NULL, g_qual_file ? g_qual : NULL, INFO_CAP)
             : wmb_take_lines(ctx, out, outcap, &nl, 0);
-        if (!nl) return 0;
+        if (!nl) {
+            emit_repairs(ctx, ts, show_algorithm);
+            return 0;
+        }
         fwrite(out, 1, n, stdout);
         fflush(stdout);                                 /* t1_c1_packet_decoder.h:698-699 */
         if (g_info_file || g_qual_file) {
@@ -387,6 +423,24 @@ int main(int argc, char *argv[])
         }
     }
 
+    unsigned long repair_e = 1;
+    if ((e = getenv("WMBUS_B200_REPAIR_ERASURES")) != NULL) {
+        char *end = NULL;
+        repair_e = strtoul(e, &end, 10);
+        if (!getenv("WMBUS_B200_REPAIRED")) {
+            fprintf(stderr, "rtl_wmbus_b200: WMBUS_B200_REPAIR_ERASURES needs WMBUS_B200_REPAIRED\n");
+            return EXIT_FAILURE;
+        }
+        if (e[0] < '0' || e[0] > '9' || *end || repair_e < 1 || repair_e > 3) {
+            fprintf(stderr, "rtl_wmbus_b200: WMBUS_B200_REPAIR_ERASURES=%s: expected 1, 2 or 3\n", e);
+            return EXIT_FAILURE;
+        }
+    }
+    if ((e = getenv("WMBUS_B200_REPAIRED")) != NULL && (g_rep_file = fopen(e, "w")) == NULL) {
+        fprintf(stderr, "rtl_wmbus_b200: WMBUS_B200_REPAIRED=%s: %s\n", e, strerror(errno));
+        return EXIT_FAILURE;
+    }
+
     wmb_ctx *ctx = NULL;
     if (wmb_create(&o, device, &ctx) != WMB_OK) {
         fprintf(stderr, "rtl_wmbus_b200: %s\n", wmb_last_error());
@@ -404,6 +458,10 @@ int main(int argc, char *argv[])
                 return EXIT_FAILURE;
             }
     if ((g_qual_file || g_bqual_file) && wmb_set_line_quality(ctx, 1) != WMB_OK) {
+        fprintf(stderr, "rtl_wmbus_b200: %s\n", wmb_last_error());
+        return EXIT_FAILURE;
+    }
+    if (g_rep_file && wmb_set_repair(ctx, (uint32_t)repair_e) != WMB_OK) {
         fprintf(stderr, "rtl_wmbus_b200: %s\n", wmb_last_error());
         return EXIT_FAILURE;
     }
@@ -498,6 +556,10 @@ int main(int argc, char *argv[])
     }
     if (g_bqual_file && fclose(g_bqual_file) != 0 && rc == WMB_OK) {
         fprintf(stderr, "rtl_wmbus_b200: WMBUS_B200_BURST_QUALITY: %s\n", strerror(errno));
+        return EXIT_FAILURE;
+    }
+    if (g_rep_file && fclose(g_rep_file) != 0 && rc == WMB_OK) {
+        fprintf(stderr, "rtl_wmbus_b200: WMBUS_B200_REPAIRED: %s\n", strerror(errno));
         return EXIT_FAILURE;
     }
     return rc == WMB_OK ? EXIT_SUCCESS : EXIT_FAILURE;

@@ -84,6 +84,7 @@ struct Stream {                     /* one (chain, algo) bit stream */
     uint64_t total_prev = 0;        /* ... before the last batch read (stage tap) */
     /* host framer bookkeeping */
     int64_t busy_until = -1;        /* last ordinal consumed by an accepted packet */
+    std::vector<uint64_t> rep_wait; /* repair on: accepted S1 aborts booked while partial, waiting for bit P - 1 (ordinals, ascending) */
 };
 
 /* Buffers that the demod / clock-recovery stage of batch i+1 writes while the bit-stream stage of batch i still
@@ -236,7 +237,7 @@ struct wmb_ctx {
     uint64_t *d_k3_agg = nullptr;
     /* a gathered batch; per table, the elements its prefix copy fetched (0: the table was not copied) */
     struct InFlight { int slot; bool final; bool has_timers; uint64_t m_end;
-                      uint32_t hdr, dec, qual, pool, brec, bqual, ssum, speak; };
+                      uint32_t hdr, dec, qual, pool, brec, bqual, ssum, speak, rep; };
     std::vector<InFlight> inflight;                  /* gathered batches whose results the host has not read yet */
     uint64_t stat_rerun_seen = 0, stat_fallback_seen = 0;
     double acc_demod_ms = 0, acc_bitsync_ms = 0, acc_pass_ms = 0;    /* timers of the current push */
@@ -273,6 +274,12 @@ struct wmb_ctx {
     bool quality = false;
     SlotTable<QualAcc> qual;                        /* parallel to hdr */
     SlotTable<QualAcc> bqual;                        /* parallel to brec */
+
+    /* erasure repair of the framer's candidates (wmb_set_repair; survives wmb_reset).  0: off, nothing is allocated,
+     * launched or copied */
+    uint32_t repair_e = 0;
+    SlotTable<RepHdr> rep;                           /* parallel to hdr */
+    std::vector<wmb_repair_record> repairs;          /* records not taken yet */
 
     /* band survey (wmb_set_spectrum; the setting survives wmb_reset).  Bins 0: off, nothing is allocated or launched */
     uint32_t spec_bins = 0, spec_B = 0;
@@ -322,6 +329,21 @@ static int launch_k2p_fold(wmb_ctx *c, const P1State *p1_end_last, RlState *p2_o
                            const RlState *mono_end, cudaStream_t)
 {
     return launch_k2p_fold(c, p1_end_last, p2_out, carry, pd, mono_end);
+}
+/* the gather with the erasure repair K4R (r given): on the device K4R runs between K4 and k3_publish, which reads the
+ * pool_n that K4R adds to.  Here the simulated gather has published already, so K4R runs behind it and the batch is
+ * published again, with the capacity flags the first publish cleared (n_pend's clamp is idempotent): the record is the
+ * one the device writes */
+static int launch_k3_k4(wmb_ctx *c, const K3Params &p, const K4Params *q, const K4RParams *r)
+{
+    const int rc = launch_k3_k4(c, p, q);
+    if (rc || !r) return rc;
+    static K4RSmem sm;                  /* the block's phases need real barriers: one simulated thread */
+    hs_for(p.gd->n, [&](uint32_t i) { k4r_repair(*r, i, 0, 1, sm); });
+    c->st.kernel_launches += 1;
+    *p.errors |= p.rec->errors & K3_SOFT_ERRORS;
+    k3_publish(p);
+    return WMB_OK;
 }
 #else
 static int g_k1_ctas = 0;                /* WMBUS_B200_K1_CTAS: resident demod blocks per SM (0: as many as fit) */
@@ -509,8 +531,9 @@ static int launch_k2c(wmb_ctx *c, const K2cParams &p, cudaStream_t st)
     return WMB_OK;
 }
 
-/* the whole gather + device framer; grids are fixed (the kernels loop over however many candidates there are) */
-static int launch_k3_k4(wmb_ctx *c, const K3Params &p, const K4Params *q)
+/* the whole gather + device framer (+ the erasure repair K4R when r is given); grids are fixed (the kernels loop over
+ * however many candidates there are).  K4R adds its datagrams to pool_n, which k3_publish reads: it goes before that */
+static int launch_k3_k4(wmb_ctx *c, const K3Params &p, const K4Params *q, const K4RParams *r)
 {
     static int sms = 0;
     if (!sms) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c->device);
@@ -524,6 +547,10 @@ static int launch_k3_k4(wmb_ctx *c, const K3Params &p, const K4Params *q)
     c->st.kernel_launches += 8;
     if (q) {
         k4_decode_kernel<<<sms * 64, K4_THREADS, 0, c->cs>>>(*q);
+        c->st.kernel_launches += 1;
+    }
+    if (r) {
+        k4r_repair_kernel<<<sms * 64, K4_THREADS, 0, c->cs>>>(*r);
         c->st.kernel_launches += 1;
     }
     k3_publish_kernel<<<1, 32, 0, c->cs>>>(p);
@@ -1666,6 +1693,8 @@ static int enqueue_gather(wmb_ctx *c, bool final, bool after_batch)
     const bool bursts = bursts_on(c) && (after_batch || final);
     if (bursts) TRY(burst_alloc(c));
     if (quality) TRY(qual_alloc(c));
+    const bool repair = c->repair_e && !c->manual;
+    if (repair && !c->rep.d) TRY(c->rep.alloc(c, 1, c->hdr.cap, c->hdr.prefix, 256));     /* first gather with repair on */
     if (any_sync) {
         K3Params p;
         memset(&p, 0, sizeof(p));
@@ -1696,7 +1725,11 @@ static int enqueue_gather(wmb_ctx *c, bool final, bool after_batch)
         memset(&q, 0, sizeof(q));
         q.hdr = c->hdr.d; q.words = c->d_words; q.dec = c->dec.d;
         q.pool = c->pool.d + c->pool.at(slot); q.pool_cap = (uint32_t)c->pool.cap; q.pool_n = GD_FIELD(c, pool_n); q.errors = c->d_errors; q.gd = c->d_gd;
-        TRY(launch_k3_k4(c, p, c->manual ? nullptr : &q));
+        K4RParams r;
+        memset(&r, 0, sizeof(r));
+        r.hdr = q.hdr; r.dec = q.dec; r.words = q.words; r.rep = c->rep.d; r.pool = q.pool; r.pool_cap = q.pool_cap;
+        r.pool_n = q.pool_n; r.errors = q.errors; r.e_max = c->repair_e; r.gd = q.gd;
+        TRY(launch_k3_k4(c, p, c->manual ? nullptr : &q, repair ? &r : nullptr));
         /* results -> pinned host mirror: the record and a prefix of the arrays it describes (the rest, if a batch ever
          * produces more, is fetched when the record has been read) */
         CUDA_TRY(cudaMemcpyAsync(c->h_rec + slot, c->d_rec + slot, sizeof(BatchRec), cudaMemcpyDeviceToHost, c->cs));
@@ -1705,6 +1738,7 @@ static int enqueue_gather(wmb_ctx *c, bool final, bool after_batch)
         if (!c->manual) {
             TRY(c->dec.enqueue(slot, 0, c->cs, &f.dec));
             TRY(c->pool.enqueue(slot, 0, c->cs, &f.pool));
+            if (repair) TRY(c->rep.enqueue(slot, 0, c->cs, &f.rep));
         }
     }
     /* the burst report: behind the demod kernel of the batch (cs waited for it), before ev_chain[set] releases the set */
@@ -1785,8 +1819,8 @@ static int enqueue_gather(wmb_ctx *c, bool final, bool after_batch)
     return WMB_OK;
 }
 
-static int book_device_frames(wmb_ctx *c, const FrameHdr *hdr, const DecHdr *dec, const QualAcc *qual, const uint8_t *pool,
-                              size_t n, bool final);
+static int book_device_frames(wmb_ctx *c, const FrameHdr *hdr, const DecHdr *dec, const QualAcc *qual, const RepHdr *rep,
+                              const uint8_t *pool, size_t n, bool final);
 
 /* Wait for the oldest gathered batch's results (an event, not a stream: later batches keep running), fetch what the
  * prefix copy did not cover, and run the stream-order bookkeeping over it. */
@@ -1824,6 +1858,7 @@ static int consume_oldest(wmb_ctx *c)
     if (f.dec) TRY(c->dec.fetch(f.slot, 0, f.dec, r.n, c->xs, &more));
     if (f.qual) TRY(c->qual.fetch(f.slot, 0, f.qual, r.n, c->xs, &more));
     if (f.pool) TRY(c->pool.fetch(f.slot, 0, f.pool, r.pool_n, c->xs, &more));
+    if (f.rep) TRY(c->rep.fetch(f.slot, 0, f.rep, r.n, c->xs, &more));
     if (!f.dec && r.n_words) {               /* manual mode reads after every batch: the frame words are this batch's */
         CUDA_TRY(cudaMemcpyAsync(c->h_words, c->d_words, (size_t)r.n_words * 4, cudaMemcpyDeviceToHost, c->xs));
         c->st.d2h_bytes += (uint64_t)r.n_words * 4;
@@ -1832,7 +1867,7 @@ static int consume_oldest(wmb_ctx *c)
     if (more) CUDA_TRY(cudaStreamSynchronize(c->xs));
     /* the next batches probably look like this one: let the prefix copies cover them */
     if (f.brec) { c->brec.grow(most); c->bqual.grow(most); }
-    if (f.hdr) { c->hdr.grow(r.n); c->dec.grow(r.n); c->qual.grow(r.n); c->pool.grow(r.pool_n); }
+    if (f.hdr) { c->hdr.grow(r.n); c->dec.grow(r.n); c->qual.grow(r.n); c->rep.grow(r.n); c->pool.grow(r.pool_n); }
     if (f.brec) book_bursts(c, f);
     if (f.ssum) {                                    /* the slot's survey rows -> the queue */
         const std::vector<wmb_spectrum_row> &rows = c->spec_slot_rows[f.slot];
@@ -1853,6 +1888,7 @@ static int consume_oldest(wmb_ctx *c)
     if (err & 256u) return set_err(WMB_E_STATE, "internal: lane verification does not converge");
     c->st.d2h_bytes += sizeof(BatchRec) + (size_t)r.n * sizeof(FrameHdr) + (f.dec ? (size_t)r.n * sizeof(DecHdr) + r.pool_n : 0);
     if (f.qual) c->st.d2h_bytes += (size_t)r.n * sizeof(QualAcc);
+    if (f.rep) c->st.d2h_bytes += (size_t)r.n * sizeof(RepHdr);
     /* statistics kept on the device */
     c->st.lanes_rerun += r.lanes_rerun - c->stat_rerun_seen; c->st.lanes_run += r.lanes_rerun - c->stat_rerun_seen;
     c->stat_rerun_seen = r.lanes_rerun;
@@ -1874,7 +1910,7 @@ static int consume_oldest(wmb_ctx *c)
     for (uint32_t i = 0; i < r.n; i++) hdr[i].sync_sample = f.m_end - ((f.m_end - hdr[i].sync_sample) & EVG_M_MASK);
     int rc = WMB_OK;
     if (f.dec) rc = book_device_frames(c, hdr, c->dec.h + c->dec.at(f.slot), f.qual ? c->qual.h + c->qual.at(f.slot) : nullptr,
-                                       c->pool.h + c->pool.at(f.slot), r.n, f.final);
+                                       f.rep ? c->rep.h + c->rep.at(f.slot) : nullptr, c->pool.h + c->pool.at(f.slot), r.n, f.final);
     else {
         /* manual mode: keep the frames (newest version of a re-delivered partial one wins) for wmb_poll */
         for (uint32_t i = 0; i < r.n; i++) {
@@ -2113,13 +2149,14 @@ extern "C" int wmb_poll(wmb_ctx *c, wmb_frame *out, size_t cap, size_t *n, int f
 /* Stream-order bookkeeping over decoded candidates (sorted by chain, algorithm, ordinal): a decoder
  * that is receiving ignores further access-code matches (t1_c1_packet_decoder.h:272-278 honours the
  * flag only in idle), so a candidate inside the telegram of an earlier one is dropped; the rest
- * become lines, queued in the order the reference prints them. */
+ * become lines, queued in the order the reference prints them.  accepted (if given): the indices of the frames that the rule
+ * accepted, in input order. */
 struct FrameMeta { uint8_t chain, algo, partial, truncated, ofs_valid; uint64_t ordinal, sync_sample; int64_t ofs_sum; uint32_t ofs_n;
                    const QualAcc *qual; /* null: no quality sums */ };
 struct DecLite { int status; uint32_t consumed; uint64_t end_sample; uint8_t crc_ok; };
 
 template <class Meta, class Lite, class Fill>
-static int book_frames(wmb_ctx *c, size_t n, Meta meta, Lite lite, Fill fill)
+static int book_frames(wmb_ctx *c, size_t n, Meta meta, Lite lite, Fill fill, std::vector<size_t> *accepted = nullptr)
 {
     struct Key { uint64_t end_sample; uint32_t prio, seq; size_t fi; uint8_t algo; };
     bool blocked[WMB_N_CHAINS][WMB_N_ALGOS] = {{false, false}, {false, false}};
@@ -2135,9 +2172,11 @@ static int book_frames(wmb_ctx *c, size_t n, Meta meta, Lite lite, Fill fill)
             if (!f.truncated) return set_err(WMB_E_STATE, "internal: frame shorter than its header demands");
             /* cut by a run-length reset or by the end of input: the reference's decoder is reset too */
             s.busy_until = (int64_t)(f.ordinal + d.consumed - 1);
+            if (accepted) accepted->push_back(fi);
             continue;
         }
         s.busy_until = (int64_t)(f.ordinal + d.consumed - 1);
+        if (accepted) accepted->push_back(fi);
         if (d.status == WMB_DEC_LINE && f.sync_sample >= c->win_lo && f.sync_sample < c->win_hi) {
             Key k;
             k.end_sample = d.end_sample;
@@ -2201,15 +2240,94 @@ static void decoded_from(const DecHdr &d, uint64_t sync_sample, const uint8_t *p
     memcpy(o.datagram, pool + d.data_off, d.len);
 }
 
-/* candidates of one gathered batch, decoded by K4 (already in stream order) */
-static int book_device_frames(wmb_ctx *c, const FrameHdr *hdr, const DecHdr *dec, const QualAcc *qual, const uint8_t *pool,
-                              size_t n, bool final)
+/* a K4R verdict -> the repair of one candidate, its datagram out of the pool */
+static void repaired_from(const RepHdr &h, uint64_t sync_sample, int chain, const uint8_t *pool, wmb_repaired &o)
+{
+    static const char modes[3][3] = { "T1", "C1", "S1" };
+    memset(&o, 0, sizeof(o));
+    o.outcome = h.outcome; o.had_line = h.had_line;
+    if (h.outcome != K4R_REPAIRED) return;
+    o.erasures = h.erasures; o.blocks = h.blocks;
+    wmb_decoded &d = o.line;
+    d.status = WMB_DEC_LINE; d.consumed = h.consumed; d.end_sample = sync_sample + h.end_off;
+    memcpy(d.mode, modes[chain == WMB_CHAIN_T1C1 ? 0 : 2], 3);
+    d.crc_ok = 1; d.ok_3of6 = 1; d.packet_rssi = h.packet_rssi; d.current_rssi = h.current_rssi;
+    d.serial = h.serial; d.len = h.len;
+    memcpy(d.datagram, pool + h.data_off, h.len);
+}
+
+/* The repair records of one gathered batch (wmb_set_repair).  A candidate that book_frames accepted gets its record in
+ * the gather that delivers it with all its bits (not partial).  An S1 abort is accepted as soon as K4 sees the
+ * violation, usually long before bit P - 1: K3 carries it on, and it waits in its stream's rep_wait list for that
+ * gather.  A waiting frame that a gather does not deliver was lost in an overflow (counted there). */
+static void book_repairs(wmb_ctx *c, const FrameHdr *hdr, const RepHdr *rep, const uint8_t *pool, size_t n,
+                         const std::vector<uint32_t> &idx, const std::vector<size_t> &accepted, bool final)
+{
+    std::vector<wmb_repair_record> fresh;
+    auto partial = [&](uint32_t i) { return !hdr[i].complete && !final; };
+    auto take = [&](uint32_t i) {
+        const RepHdr &h = rep[i];
+        if (h.outcome == K4R_NONE || h.outcome == K4R_TRUNCATED) return;
+        if (h.outcome == K4R_REPAIRED && h.data_off == 0xFFFFFFFFu) return;      /* no room in the pool: an overflow batch */
+        wmb_repair_record r;
+        memset(&r, 0, sizeof(r));
+        r.sync_sample = hdr[i].sync_sample; r.end_sample = hdr[i].sync_sample + h.end_off;
+        r.chain = hdr[i].chain; r.algo = hdr[i].algo;
+        repaired_from(h, hdr[i].sync_sample, hdr[i].chain, pool, r.repair);
+        fresh.push_back(r);
+    };
+    /* the frames of a gather are in stream order: (chain, algo, ordinal) ascending */
+    auto find = [&](int ch, int a, uint64_t ord) -> long {
+        const FrameHdr *e = hdr + n;
+        const FrameHdr *it = std::lower_bound(hdr, e, 0, [&](const FrameHdr &h, int) {
+            if (h.chain != ch) return h.chain < ch;
+            if (h.algo != a) return h.algo < a;
+            return h.ordinal < ord;
+        });
+        return (it != e && it->chain == ch && it->algo == a && it->ordinal == ord && it->nbits) ? (long)(it - hdr) : -1;
+    };
+    for (int ch = 0; ch < WMB_N_CHAINS; ch++)
+        for (int a = 0; a < WMB_N_ALGOS; a++) {
+            std::vector<uint64_t> &w = c->cb[ch].s[a].rep_wait;
+            size_t keep = 0;
+            for (uint64_t ord : w) {
+                const long i = find(ch, a, ord);
+                if (i < 0) continue;
+                if (partial((uint32_t)i)) { w[keep++] = ord; continue; }
+                take((uint32_t)i);
+            }
+            w.resize(keep);
+        }
+    for (size_t k : accepted) {
+        const uint32_t i = idx[k];
+        const FrameHdr &h = hdr[i];
+        if (h.sync_sample < c->win_lo || h.sync_sample >= c->win_hi) continue;
+        if (partial(i)) {
+            /* a candidate whose list has not reached P yet (only an S1 abort can be booked so early) */
+            if (rep[i].outcome == K4R_TRUNCATED) c->cb[h.chain].s[h.algo].rep_wait.push_back(h.ordinal);
+            continue;
+        }
+        take(i);
+    }
+    std::sort(fresh.begin(), fresh.end(), [](const wmb_repair_record &x, const wmb_repair_record &y) {
+        if (x.end_sample != y.end_sample) return x.end_sample < y.end_sample;
+        const int px = x.chain * 2 + (x.algo == WMB_ALGO_T2A), py = y.chain * 2 + (y.algo == WMB_ALGO_T2A);
+        if (px != py) return px < py;
+        return x.sync_sample < y.sync_sample;
+    });
+    c->repairs.insert(c->repairs.end(), fresh.begin(), fresh.end());
+}
+
+/* candidates of one gathered batch, decoded by K4 (already in stream order); rep: K4R's verdicts when repair is on */
+static int book_device_frames(wmb_ctx *c, const FrameHdr *hdr, const DecHdr *dec, const QualAcc *qual, const RepHdr *rep,
+                              const uint8_t *pool, size_t n, bool final)
 {
     /* frames without any bit (candidate at the very end of the stream) are not decoded at all */
     std::vector<uint32_t> idx;
     idx.reserve(n);
     for (size_t i = 0; i < n; i++) if (hdr[i].nbits) idx.push_back((uint32_t)i);
-    return book_frames(c, idx.size(),
+    std::vector<size_t> accepted;
+    TRY(book_frames(c, idx.size(),
         [&](size_t k) {
             const FrameHdr &h = hdr[idx[k]];
             FrameMeta m;
@@ -2226,7 +2344,10 @@ static int book_device_frames(wmb_ctx *c, const FrameHdr *hdr, const DecHdr *dec
             l.status = d.status; l.consumed = d.consumed; l.end_sample = hdr[idx[k]].sync_sample + d.end_off; l.crc_ok = d.crc_ok;
             return l;
         },
-        [&](size_t k, wmb_decoded &o) { decoded_from(dec[idx[k]], hdr[idx[k]].sync_sample, pool, o); });
+        [&](size_t k, wmb_decoded &o) { decoded_from(dec[idx[k]], hdr[idx[k]].sync_sample, pool, o); },
+        rep ? &accepted : nullptr));
+    if (rep) book_repairs(c, hdr, rep, pool, n, idx, accepted, final);
+    return WMB_OK;
 }
 
 /* caller-made frames into the context's frame tables, and K4 on them; the datagram pool starts empty */
@@ -2287,7 +2408,6 @@ static int launch_k4r(wmb_ctx *c, const K4RParams &p)
  * wmb_frame_repair() frame by frame. */
 extern "C" int wmb_frame_repair_device(wmb_ctx *c, const wmb_frame *frames, size_t n, uint32_t e_max, wmb_repaired *out)
 {
-    static const char modes[3][3] = { "T1", "C1", "S1" };
     if (!c || !frames || !out) return set_err(WMB_E_INVAL, "null argument");
     if (e_max > K4R_MAX_ERASURES) return set_err(WMB_E_INVAL, "e_max %u out of range 0..%d", e_max, K4R_MAX_ERASURES);
     memset(out, 0, n * sizeof(*out));
@@ -2309,17 +2429,9 @@ extern "C" int wmb_frame_repair_device(wmb_ctx *c, const wmb_frame *frames, size
     CUDA_TRY(cudaStreamSynchronize(c->cs));
     for (size_t i = 0; i < n; i++) {
         const RepHdr &h = rep[i];
-        wmb_repaired &o = out[i];
-        o.outcome = h.outcome; o.had_line = h.had_line;
-        if (h.outcome != K4R_REPAIRED) continue;
-        if (h.data_off == 0xFFFFFFFFu) return set_err(WMB_E_OVERFLOW, "datagram pool full: hand in fewer frames at once");
-        o.erasures = h.erasures; o.blocks = h.blocks;
-        wmb_decoded &d = o.line;
-        d.status = WMB_DEC_LINE; d.consumed = h.consumed; d.end_sample = frames[i].sync_sample + h.end_off;
-        memcpy(d.mode, modes[frames[i].chain == WMB_CHAIN_T1C1 ? 0 : 2], 3);
-        d.crc_ok = 1; d.ok_3of6 = 1; d.packet_rssi = h.packet_rssi; d.current_rssi = h.current_rssi;
-        d.serial = h.serial; d.len = h.len;
-        memcpy(d.datagram, c->pool.h + h.data_off, h.len);
+        if (h.outcome == K4R_REPAIRED && h.data_off == 0xFFFFFFFFu)
+            return set_err(WMB_E_OVERFLOW, "datagram pool full: hand in fewer frames at once");
+        repaired_from(h, frames[i].sync_sample, frames[i].chain, c->pool.h, out[i]);
     }
     return WMB_OK;
 }
@@ -2493,7 +2605,7 @@ extern "C" int wmb_reset(wmb_ctx *c)
     for (cudaStream_t st : { c->cs, c->xs, c->k1s, c->as[0], c->as[1], c->as2[0], c->as2[1], c->ts, c->s2, c->rs })
         if (st && cudaStreamQuery(st) != cudaSuccess) CUDA_TRY(cudaStreamSynchronize(st));
     c->iq_consumed = 0; c->m_consumed = 0; c->hist_m = 0; c->hist_iq = 0;
-    c->remainder.clear(); c->lines.clear(); c->held.clear(); c->held_prev.clear();
+    c->remainder.clear(); c->lines.clear(); c->held.clear(); c->held_prev.clear(); c->repairs.clear();
     c->batch_no = 0; c->last_M = 0; c->prev_M = 0; c->last_hist = 0; c->last_set = 0; c->inflight.clear();
     c->chain_recorded[0] = c->chain_recorded[1] = false;
     c->stat_rerun_seen = 0; c->stat_fallback_seen = 0;
@@ -2501,7 +2613,10 @@ extern "C" int wmb_reset(wmb_ctx *c)
     c->spec_open = -1; c->spec_open_blocks = 0; c->spec_batch_rows.clear(); c->spec_enqueued = false;
     c->spec_rows.clear(); c->spec_sum.clear(); c->spec_peak.clear();
     for (int ch = 0; ch < WMB_N_CHAINS; ch++)
-        for (int a = 0; a < WMB_N_ALGOS; a++) { Stream &s = c->cb[ch].s[a]; s.total = 0; s.total_prev = 0; s.busy_until = -1; }
+        for (int a = 0; a < WMB_N_ALGOS; a++) {
+            Stream &s = c->cb[ch].s[a];
+            s.total = 0; s.total_prev = 0; s.busy_until = -1; s.rep_wait.clear();
+        }
     if (c->allocated) {
         /* device state back to the start of a stream, in stream order on cs: one small kernel, no host copy, no wait;
          * the first batch's kernels on the other streams wait for it (ev_reset) */
@@ -2612,6 +2727,27 @@ extern "C" int wmb_set_line_quality(wmb_ctx *c, int on)
     return WMB_OK;
 }
 
+extern "C" int wmb_set_repair(wmb_ctx *c, uint32_t e_max)
+{
+    if (!c) return set_err(WMB_E_INVAL, "null argument");
+    if (c->manual) return set_err(WMB_E_INVAL, "wmb_set_repair on a manual_frames context (repair the polled frames with wmb_frame_repair_device)");
+    if (e_max > K4R_MAX_ERASURES) return set_err(WMB_E_INVAL, "e_max %u out of range 0 (off) .. %d", e_max, K4R_MAX_ERASURES);
+    if (c->batch_no != 0 || !c->remainder.empty())
+        return set_err(WMB_E_STATE, "wmb_set_repair after samples were pushed (call it before the first push or after wmb_reset / wmb_seek)");
+    c->repair_e = e_max;
+    return WMB_OK;
+}
+
+extern "C" int wmb_take_repairs(wmb_ctx *c, wmb_repair_record *out, size_t cap, size_t *n)
+{
+    if (!c || !n || (!out && cap)) return set_err(WMB_E_INVAL, "null argument");
+    const size_t k = std::min(cap, c->repairs.size());
+    if (k) memcpy(out, c->repairs.data(), k * sizeof(wmb_repair_record));
+    c->repairs.erase(c->repairs.begin(), c->repairs.begin() + (long)k);
+    *n = k;
+    return WMB_OK;
+}
+
 extern "C" int wmb_set_spectrum(wmb_ctx *c, uint32_t bins, uint32_t blocks_per_record)
 {
     if (!c) return set_err(WMB_E_INVAL, "null argument");
@@ -2662,6 +2798,12 @@ extern "C" int wmb_set_line_window(wmb_ctx *c, uint64_t sync_lo, uint64_t sync_h
     if (!c || sync_lo > sync_hi) return set_err(WMB_E_INVAL, "bad window");
     c->win_lo = sync_lo; c->win_hi = sync_hi;
     return WMB_OK;
+}
+
+/* repair on: the candidate at ordinal ord of stream s is booked and waits for its repair (book_repairs) */
+static bool rep_waiting(const wmb_ctx *c, const Stream &s, uint64_t ord)
+{
+    return c->repair_e && std::binary_search(s.rep_wait.begin(), s.rep_wait.end(), ord);
 }
 
 extern "C" long wmb_boundary_state(wmb_ctx *c, uint8_t *buf, size_t cap)
@@ -2719,13 +2861,16 @@ extern "C" long wmb_boundary_state(wmb_ctx *c, uint8_t *buf, size_t cap)
                     CUDA_TRY(cudaMemcpy(ev.data() + i, s.ring + at, (size_t)run * 8, cudaMemcpyDeviceToHost));
                     i += run;
                 }
-                /* a match inside a telegram that is already decoded will be ignored (busy decoder) */
-                const uint32_t n32 = (uint32_t)n | (((int64_t)ord <= s.busy_until) ? 0x80000000u : 0u);
+                /* a match inside a telegram that is already decoded will be ignored (busy decoder); bit 30: a candidate
+                 * booked already that waits for its repair */
+                const uint32_t n32 = (uint32_t)n | (((int64_t)ord <= s.busy_until) ? 0x80000000u : 0u)
+                                   | (rep_waiting(c, s, ord) ? 0x40000000u : 0u);
                 put(&n32, 4);
                 put(ev.data(), ev.size() * 8);
             }
         }
     }
+    if (c->repair_e) put(&c->repair_e, 4);             /* contexts that repair differently never agree */
     if (out.size() > cap) return set_err(WMB_E_INVAL, "buffer too small (%zu bytes needed)", out.size());
     memcpy(buf, out.data(), out.size());
     return (long)out.size();
@@ -2753,7 +2898,8 @@ extern "C" long wmb_pending_before(wmb_ctx *c, uint64_t sync_hi)
             if (pend.empty()) continue;
             CUDA_TRY(cudaMemcpy(pend.data(), s.pend, pend.size() * 8, cudaMemcpyDeviceToHost));
             for (uint64_t ord : pend) {
-                if ((int64_t)ord <= s.busy_until) continue;              /* inside a telegram already decoded: will be ignored */
+                /* inside a telegram already decoded: will be ignored -- unless it is that telegram, waiting for its repair */
+                if ((int64_t)ord <= s.busy_until && !rep_waiting(c, s, ord)) continue;
                 uint64_t ev = 0;                                         /* the flagged bit's event: its sample is the match */
                 CUDA_TRY(cudaMemcpy(&ev, s.ring + (ord & (s.ring_cap - 1)), 8, cudaMemcpyDeviceToHost));
                 const uint64_t m = c->m_consumed - ((c->m_consumed - EVG_M(ev)) & EVG_M_MASK);   /* 40 bits -> stream position */

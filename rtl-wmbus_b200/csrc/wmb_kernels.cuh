@@ -1572,8 +1572,8 @@ WMB_D void k4_decode(const K4Params &p, uint32_t f, int tid, int nthr, K4Smem &s
 enum { K4R_NONE = 0, K4R_REPAIRED = 1, K4R_AMBIGUOUS = 2, K4R_TOO_MANY = 3, K4R_UNREPAIRABLE = 4, K4R_TRUNCATED = 5 };
 
 struct RepHdr {                     /* one per candidate, parallel to DecHdr, device -> host */
-    uint32_t consumed;              /* P: bits of the repaired telegram incl. the flagged one */
-    uint32_t end_off;               /* sample offset (from sync_sample) of bit P - 1       */
+    uint32_t consumed;              /* P: bits of the telegram incl. the flagged one (0: NONE, TRUNCATED) */
+    uint32_t end_off;               /* sample offset (from sync_sample) of bit P - 1 (the streaming record's end) */
     uint32_t serial;
     uint32_t data_off;              /* byte offset of the repaired datagram in the pool (0xFFFFFFFF: no room) */
     uint16_t len;                   /* datagram bytes after the CRC strip                  */
@@ -1582,13 +1582,16 @@ struct RepHdr {                     /* one per candidate, parallel to DecHdr, de
 };
 
 struct K4RParams {
-    const FrameHdr *hdr; const DecHdr *dec; uint32_t n;
+    const FrameHdr *hdr; const DecHdr *dec; uint32_t n;    /* gd == null: n candidates at hdr / dec / rep (test hook) */
     const uint32_t *words;
     RepHdr *rep;
     uint8_t *pool; uint32_t pool_cap; uint32_t *pool_n;
     uint32_t *errors;
     uint32_t e_max;                 /* 1..3 */
+    const GatherDev *gd;            /* else: the current batch's candidates, gd->n of them from gd->base on (as K4) */
 };
+
+WMB_D uint32_t k4r_count(const K4RParams &p) { return p.gd ? p.gd->n : p.n; }
 
 struct K4RSmem {
     uint8_t  pkt[296];              /* the received bytes, erased nibbles / bits zero       */
@@ -1617,9 +1620,11 @@ WMB_D uint32_t k4r_fillings(uint32_t w, uint8_t *fill)
 
 WMB_D void k4r_repair(const K4RParams &p, uint32_t f, int tid, int nthr, K4RSmem &sm)
 {
-    if (f >= p.n) return;
-    const FrameHdr h = p.hdr[f];
-    const DecHdr d = p.dec[f];
+    if (f >= k4r_count(p)) return;
+    const uint32_t lb = p.gd ? p.gd->base : 0u;
+    RepHdr *const rep_out = p.rep + lb;
+    const FrameHdr h = p.hdr[lb + f];
+    const DecHdr d = p.dec[lb + f];
     const uint32_t *b = p.words + h.word_off;
     const uint32_t nbits = h.nbits;
     const bool t1 = h.chain == WMB_CHAIN_T1C1;
@@ -1628,22 +1633,28 @@ WMB_D void k4r_repair(const K4RParams &p, uint32_t f, int tid, int nthr, K4RSmem
     r.erasures = 0; r.blocks = 0; r.had_line = 0; r.packet_rssi = 0; r.current_rssi = 0;
 
     /* candidates: a line whose CRCs fail, an S1 abort on a Manchester violation after the L-field byte */
-    if (nbits == 0 || d.status == K4_SKIP) { if (tid == 0) p.rep[f] = r; return; }
+    if (nbits == 0 || d.status == K4_SKIP) { if (tid == 0) rep_out[f] = r; return; }
     if (d.status == K4_LINE && !d.crc_ok) {
         r.had_line = 1;
-        if (d.mode == 1) { r.outcome = K4R_UNREPAIRABLE; if (tid == 0) p.rep[f] = r; return; }   /* C1: no erasures */
+        if (d.mode == 1) {                              /* C1: no erasures; the record ends at the line's last bit */
+            r.outcome = K4R_UNREPAIRABLE; r.consumed = d.consumed; r.end_off = d.end_off;
+            if (tid == 0) rep_out[f] = r;
+            return;
+        }
     } else if (d.status == K4_ABORT && !t1) {
         const uint32_t pos = d.consumed - 1;
-        if (pos < 18 || (pos & 1u) || WMB_BIT_DATA(b[pos]) != WMB_BIT_DATA(b[pos - 1])) { if (tid == 0) p.rep[f] = r; return; }
-    } else { if (tid == 0) p.rep[f] = r; return; }
+        if (pos < 18 || (pos & 1u) || WMB_BIT_DATA(b[pos]) != WMB_BIT_DATA(b[pos - 1])) { if (tid == 0) rep_out[f] = r; return; }
+    } else { if (tid == 0) rep_out[f] = r; return; }
 
     uint32_t L = 0;
     if (t1) L = (wmb_dec3of6(k4_bits(b, 1, 6)) << 4) | wmb_dec3of6(k4_bits(b, 7, 6));
     else for (uint32_t k = 0; k < 8; k++) L = (L << 1) | WMB_BIT_DATA(b[2 + 2 * k]);
     const uint32_t len = wmb_tlg_len_a(L);
     const uint32_t P = 1 + (t1 ? 12u : 16u) * len;
-    if (nbits < P) { r.outcome = K4R_TRUNCATED; if (tid == 0) p.rep[f] = r; return; }
-    if (len < 12) { r.outcome = K4R_UNREPAIRABLE; if (tid == 0) p.rep[f] = r; return; }
+    if (nbits < P) { r.outcome = K4R_TRUNCATED; if (tid == 0) rep_out[f] = r; return; }
+    r.consumed = P;                                      /* every outcome from here on: the record's end is bit P - 1 */
+    r.end_off = WMB_BIT_OFFSET(b[P - 1]);
+    if (len < 12) { r.outcome = K4R_UNREPAIRABLE; if (tid == 0) rep_out[f] = r; return; }
 
     if (tid == 0) sm.bad = 0;
     K4_SYNC();
@@ -1737,7 +1748,7 @@ WMB_D void k4r_repair(const K4RParams &p, uint32_t f, int tid, int nthr, K4RSmem
     }
     if (outcome == K4R_NONE) outcome = erasures ? K4R_REPAIRED : K4R_UNREPAIRABLE;
     r.outcome = (uint8_t)outcome;
-    if (outcome != K4R_REPAIRED) { if (tid == 0) p.rep[f] = r; return; }
+    if (outcome != K4R_REPAIRED) { if (tid == 0) rep_out[f] = r; return; }
 
     /* the repaired telegram: CRC-stripped datagram (format A, :551-592) into the pool */
     const uint32_t out_len = len - 2 * nblk;
@@ -1760,15 +1771,13 @@ WMB_D void k4r_repair(const K4RParams &p, uint32_t f, int tid, int nthr, K4RSmem
         for (uint32_t i = (uint32_t)tid; i < out_len; i += (uint32_t)nthr)
             p.pool[data_off + i] = sm.pkt[wmb_strip_src_a(i)];
     if (tid == 0) {
-        r.consumed = P;
-        r.end_off = WMB_BIT_OFFSET(b[P - 1]);
         r.serial = (uint32_t)sm.pkt[4] | ((uint32_t)sm.pkt[5] << 8) | ((uint32_t)sm.pkt[6] << 16) | ((uint32_t)sm.pkt[7] << 24);
         r.data_off = data_off;
         r.len = (uint16_t)(data_off == 0xFFFFFFFFu ? 0 : out_len);
         r.erasures = (uint8_t)erasures; r.blocks = (uint8_t)blocks;
         r.packet_rssi = (uint8_t)WMB_BIT_RSSI(b[1]);
         r.current_rssi = (uint8_t)WMB_BIT_RSSI(b[P - 1]);
-        p.rep[f] = r;
+        rep_out[f] = r;
     }
 }
 
@@ -2157,7 +2166,8 @@ __global__ void __launch_bounds__(K4_THREADS) k4_decode_kernel(const K4Params p)
 __global__ void __launch_bounds__(K4_THREADS) k4r_repair_kernel(const K4RParams p)
 {
     __shared__ K4RSmem sm;
-    for (uint32_t f = blockIdx.x; f < p.n; f += gridDim.x) {
+    const uint32_t n = k4r_count(p);
+    for (uint32_t f = blockIdx.x; f < n; f += gridDim.x) {
         k4r_repair(p, f, threadIdx.x, blockDim.x, sm);
         __syncthreads();
     }

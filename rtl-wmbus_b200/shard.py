@@ -130,6 +130,17 @@ def merge_spectrum(parts):
     return out, s, p
 
 
+def repair_key(r):
+    """(end_sample, chain * 2 + (algo == t2a), sync_sample): the order of the repair records (wmb_repair_record)"""
+    return r.end_sample, r.chain * 2 + (1 if r.algo == 1 else 0), r.sync_sample
+
+
+def merge_repairs(parts):
+    """Repair records (lists of WmbRepairRecord) of several time chunks, each holding those whose match lies in its
+    chunk -> the sequential run's records, in repair_key() order."""
+    return sorted((r for part in parts for r in part), key=repair_key)
+
+
 def find_carriers(rows, sum, peak, fs: float, threshold_db: float = 15.0, bridge_hz: float = 110e3,
                   tone_hz: float = 20e3):
     """Carriers worth decoding in a band survey (take_spectrum / merge_spectrum output, or a CLI spectrum file read
@@ -175,7 +186,7 @@ def find_carriers(rows, sum, peak, fs: float, threshold_db: float = 15.0, bridge
 
 
 def decode_time_chunk(ctx, push, n_bytes: int, d: int, rank: int, world: int, halo_m: int = 1 << 18, info=False,
-                      bursts=False, spectrum=False, quality=False):
+                      bursts=False, spectrum=False, quality=False, repairs=False):
     """Decode rank `rank`'s chunk of a capture of n_bytes cu8 bytes.  `push(byte_lo, byte_hi)` feeds that byte
     range of the capture to ctx (host or device memory: the caller's business).
     Returns (lines, digest_start, digest_end, halo_start_iq): digest_start is None for a chunk that starts at 0.
@@ -190,13 +201,17 @@ def decode_time_chunk(ctx, push, n_bytes: int, d: int, rank: int, world: int, ha
     window counts the chunk's blocks only, so merge_spectrum() over the chunks gives the sequential records.
     quality=True (ctx made with quality=True): the lines' wmb_line_quality records follow the line records, and with
     bursts=True the bursts' wmb_burst_quality records follow the bursts: (lines[, records], quality[, bursts,
-    burst_quality][, spectrum]).  Their windows are the offset windows, so they are the sequential run's as well."""
+    burst_quality][, spectrum]).  Their windows are the offset windows, so they are the sequential run's as well.
+    repairs=True (ctx made with repair=e_max): the repair records (take_repairs()) of the candidates matched in the chunk
+    come last; merge_repairs() over the chunks gives the sequential records.  A candidate that waits for its repair
+    counts in pending_before(), so the right halo goes on until its record is made."""
     import hashlib
     recs = []
     qrecs = []
     brecs = []
     bqrecs = []
     srecs = []
+    rrecs = []
 
     def take_s():
         if spectrum:
@@ -211,6 +226,8 @@ def decode_time_chunk(ctx, push, n_bytes: int, d: int, rank: int, world: int, ha
             brecs.append(ctx.take_bursts())
 
     def take():
+        if repairs:
+            rrecs.extend(ctx.take_repairs())
         if quality:
             got = ctx.take_lines(2, info=True, quality=True)
             recs.append(got[1])
@@ -277,6 +294,8 @@ def decode_time_chunk(ctx, push, n_bytes: int, d: int, rank: int, world: int, ha
         srecs = [x for x in srecs if len(x[0])] or srecs[:1]
         out.append((np.concatenate([x[0] for x in srecs]), np.concatenate([x[1] for x in srecs]),
                     np.concatenate([x[2] for x in srecs])))
+    if repairs:
+        out.append(rrecs)
     lines = tuple(out) if len(out) > 1 else lines
     return lines, dig_start, dig_end, start
 

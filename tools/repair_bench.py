@@ -1,0 +1,123 @@
+"""What erasure repair on the streaming path (wmb_set_repair) costs and what it gains.
+    python tools/repair_bench.py cost [steps]          GPU: step times, repair off against e_max 3
+    python tools/repair_bench.py gain [--cpu] [MiB]    the noise sweep (GPU library, or the CPU build with --cpu)
+
+cost: the benchmark's default step -- 1 GiB of synthetic 1.6 MS/s cu8 with two T1 emitters, `-p S`, device-resident, one
+process_device per step -- then the same at clock lock 1 with T1/C1 access-code errors 3 (about 486 k matches per
+step).  A context with repair off and one at e_max 3 alternate step by step in one process; each step is timed with
+CUDA events and the medians are printed, with kernel launches and D2H bytes per step, the device and its power limit.
+
+gain: for each noise sigma, a capture with T1 and S1 emitters whose chips are all sent right (no data_flips), decoded
+at e_max 1, 2 and 3: the telegrams sent, those decoded CRC-ok by either algorithm, those recovered only by repair, and
+the wrong repairs (a REPAIRED datagram that was never sent).  The counts are exact: the GPU and the CPU build agree."""
+import importlib
+import os
+import subprocess
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
+import numpy as np
+
+pkg = importlib.import_module("rtl-wmbus_b200")
+synth = importlib.import_module("rtl-wmbus_b200.synth")
+shard = importlib.import_module("rtl-wmbus_b200.shard")
+
+SIGMAS = (8.0, 56.0, 64.0, 72.0, 80.0, 88.0, 96.0, 112.0)
+
+
+def power_limit():
+    import torch
+    try:
+        return subprocess.run(["nvidia-smi", "--id=%d" % torch.cuda.current_device(), "--query-gpu=power.limit",
+                               "--format=csv,noheader"], capture_output=True, text=True, timeout=30).stdout.strip()
+    except Exception as e:                               # the query is informational
+        return f"unknown ({e})"
+
+
+def cost(steps):
+    import torch
+    lib = pkg.load_library()
+    n = 1 << 30
+    cap, _ = synth.synth_capture(n, fs=1.6e6, emitters=synth.default_emitters("t1x2"), seed=shard.capture_seed(2, 0),
+                                 device="cuda")
+    torch.cuda.synchronize()
+    print(f"device: {torch.cuda.get_device_name()}  power limit: {power_limit()}")
+    for name, rx in (("defaults", {}), ("clock lock 1, T1/C1 access-code errors 3",
+                                        dict(clock_lock=(1, 2), access_code_errors=(3, 0)))):
+        # two contexts with repair off: where a step overflows its tables, they show how far the lines of two
+        # contexts agree without repair
+        ctxs = {"off": pkg.WmbusB200("-p S", lib=lib, max_batch_mib=1024, **rx),
+                "e_max 3": pkg.WmbusB200("-p S", lib=lib, max_batch_mib=1024, repair=3, **rx),
+                "off (2)": pkg.WmbusB200("-p S", lib=lib, max_batch_mib=1024, **rx)}
+        times = {k: [] for k in ctxs}
+        out = {}
+        for rep in range(steps + 2):                     # the first two rounds warm up
+            for k, ctx in ctxs.items():
+                ctx.reset()
+                before = ctx.stats()
+                a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                torch.cuda.synchronize()
+                a.record()
+                lines = ctx.process_device(cap.data_ptr(), n, flush=True, raw=True)
+                b.record()
+                torch.cuda.synchronize()
+                if rep >= 2:
+                    times[k].append(a.elapsed_time(b))
+                st = ctx.stats()
+                out[k] = (lines, ctx.take_repairs(), st.kernel_launches - before.kernel_launches,
+                          st.d2h_bytes - before.d2h_bytes, st.candidates[0][0] + st.candidates[0][1],
+                          st.overflow_batches - before.overflow_batches)
+        print(f"-- {name}: {out['off'][4]} access-code matches per step, overflow batches per step {out['off'][5]}")
+        for k in ctxs:
+            t = sorted(times[k])
+            lines, recs, launches, d2h, _m, _o = out[k]
+            print(f"  repair {k:8s}: step {t[len(t) // 2]:.2f} ms median, {t[0]:.2f}-{t[-1]:.2f} ms over {len(t)} steps; "
+                  f"kernel launches {launches}, d2h bytes {d2h}, records {len(recs)}, "
+                  f"{lines.count(b'\n')} lines, same lines as 'off': {lines == out['off'][0]}")
+        for ctx in ctxs.values():
+            ctx.close()
+
+
+def gain(cpu, mib):
+    if cpu:
+        from conftest import HOSTSIM_SO
+        lib = pkg.load_library(HOSTSIM_SO)
+    else:
+        import torch
+        lib = pkg.load_library()
+        print(f"device: {torch.cuda.get_device_name()}  power limit: {power_limit()}")
+    ems = [synth.Emitter("T1", 0x71200023, amp=90.0, offset_hz=8e3, l_field=0x29, period_s=0.10, start_s=0.004, seed=31),
+           synth.Emitter("S1", 0x19131290, amp=90.0, offset_hz=2e3, l_field=0x19, period_s=0.10, start_s=0.054, seed=32)]
+    print(f"{mib} MiB of 1.6 MS/s cu8 per sigma, one T1 (L = 0x29) and one S1 (L = 0x19) emitter at amplitude 90, -v, "
+          f"{'CPU build' if cpu else 'GPU'}")
+    print("sigma  sent  crc_ok  +rep1  +rep2  +rep3  wrong1  wrong2  wrong3")
+    for sigma in SIGMAS:
+        cu8, plan = synth.synth_capture(mib << 20, emitters=ems, seed=0xB2000100 + int(sigma), noise_sigma=sigma)
+        cu8 = np.ascontiguousarray(cu8.numpy())
+        sent = {ems[p.emitter].payload(p.k) for p in plan}
+        row = [len(plan)]
+        ok = None
+        for e_max in (1, 2, 3):
+            with pkg.WmbusB200("-v", lib=lib, repair=e_max, max_batch_mib=min(mib, 1024)) as ctx:
+                lines = ctx.process(cu8.ctypes.data, len(cu8), flush=True)
+                recs = ctx.take_repairs()
+            if ok is None:
+                ok = {bytes.fromhex(l.split(";")[8][2:]) for l in lines if l.split(";")[2] == "1"} & sent
+                row.append(len(ok))
+            rep = {bytes(r.line.datagram[:r.line.len]) for r in recs if r.repair.outcome == 1}
+            row.append(len((rep & sent) - ok))
+            row.append(len(rep - sent))
+        print(f"{sigma:5.1f}  {row[0]:4d}  {row[1]:6d}  {row[2]:5d}  {row[4]:5d}  {row[6]:5d}  {row[3]:6d}  {row[5]:6d}  "
+              f"{row[7]:6d}")
+
+
+if __name__ == "__main__":
+    what = sys.argv[1] if len(sys.argv) > 1 else "cost"
+    if what == "cost":
+        cost(int(sys.argv[2]) if len(sys.argv) > 2 else 8)
+    elif what == "gain":
+        rest = [a for a in sys.argv[2:] if a != "--cpu"]
+        gain("--cpu" in sys.argv[2:], int(rest[0]) if rest else 32)
+    else:
+        raise SystemExit(__doc__)
