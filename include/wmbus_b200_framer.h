@@ -13,7 +13,8 @@
  * The default path decodes on the device (kernel K4); wmb_frame_decode() is its host twin and
  * wmb_frame_decode_device() lets a test compare the two candidate by candidate.  wmb_frame_repair() repairs T1 / S1
  * candidates that lost a few chips (erasure decoding checked by the block CRCs), with the device twin
- * wmb_frame_repair_device().
+ * wmb_frame_repair_device(); wmb_frame_repair_soft() / wmb_frame_repair_soft_device() also repair C1 candidates from the
+ * soft values of their bits (wmb_set_soft_bits, wmb_frame_soft).
  */
 #ifndef WMBUS_B200_FRAMER_H
 #define WMBUS_B200_FRAMER_H
@@ -114,6 +115,64 @@ int wmb_set_repair(wmb_ctx *ctx, uint32_t e_max);
 
 /* Hand out at most cap of the queued records, in order; the rest stay queued.  *n: records written. */
 int wmb_take_repairs(wmb_ctx *ctx, wmb_repair_record *out, size_t cap, size_t *n);
+
+/* ---- soft values of the T1/C1 chain's bits ------------------------------------------------------------------------
+ * How sure the slicer was of a bit.  Bit event e of a T1/C1 stream lies at decimated sample m.  Its chip centre is
+ *   t2a:  c = m - WMB_SOFT_D_T2;
+ *   rla:  c = m - WMB_SOFT_D_RL - 8 (n - 1 - i), e being the i-th of the n events that share sample m (one edge emits
+ *         its whole run of bits at one sample).
+ * v = clamp(floor(sum over q in [c - 2, c + 3) of rint(dphi[q] * 2^24) / 2^12), -32767, 32767), as an int16, where dphi
+ * is the post-FIR discriminator output before the DC block (the signal the carrier-offset and quality windows read).
+ * WMB_SOFT_NONE means "no value": the window starts before the first sample pushed since the last reset / seek, or
+ * n - 1 - i > 63.  The values are sums of exact integer terms: they do not depend on batch cuts or thread order.
+ * D_RL maximises the mean of (2 bit - 1) v over clean C1 telegrams.  D_T2 does so only among the values >= 2, for which
+ * the window ends at the event's own sample: a deliberate departure from the plain argmax (D = 1, 4 % more mean margin),
+ * whose window would need the sample after the event, which the event's batch may not hold (DESIGN.md section 8).
+ * wmb_set_soft_bits(ctx, on) makes the device gather of a manual_frames context compute them (WMB_E_INVAL on any other
+ * context: its soft values serve wmb_set_repair_soft below); the setter follows wmb_set_line_quality's state rules and
+ * the setting survives wmb_reset / wmb_seek.  wmb_frame_soft() returns them for a frame of the last wmb_poll: parallel to
+ * f->bits, valid as long as f->bits; NULL for S1 frames or when soft values are off. */
+#define WMB_SOFT_NONE  (-32768)
+#define WMB_SOFT_D_T2  2
+#define WMB_SOFT_D_RL  7
+
+int wmb_set_soft_bits(wmb_ctx *ctx, int on);
+int wmb_frame_soft(wmb_ctx *ctx, const wmb_frame *f, const int16_t **soft);
+
+/* ---- C1 soft repair of one candidate --------------------------------------------------------------------------------
+ * C1 is NRZ: a wrong bit leaves no trace in the code, only in its soft value.  With k_max in 1..WMB_SOFT_K_MAX:
+ *   1. Candidates: a C1 frame (format A or B) whose decode is a line with crc_ok = 0 and len >= 12 bytes (else
+ *      UNREPAIRABLE).  P = 17 + 8 len; byte l occupies frame bits [17 + 8 l, 25 + 8 l).  The L byte is never flipped.
+ *   2. Reliability: over the bits [17, P) without WMB_SOFT_NONE, n1 and S1 are the count and the sum of v of the bits
+ *      decided 1, n0 and S0 those of the bits decided 0.  r_j = (2 bit_j - 1) (v_j 2 n0 n1 - (S1 n0 + S0 n1)) in int64,
+ *      the distance from a threshold midway between the telegram's own tone means; if n0 n1 = 0, r_j = (2 bit_j - 1) v_j.
+ *      A bit without a value ranks lowest.
+ *   3. Blocks: frame A as wmb_frame_repair (12 bytes, then 18); frame B 128-byte blocks from byte 0.  A block that
+ *      passes its CRC as received is left alone.
+ *   4. Search: in a failing block take the K = min(k_max, flippable bits) bits of lowest r (ties: lower bit index).
+ *      Exactly one of the 2^K - 1 non-zero flip patterns must pass the block's CRC.  In block order, the first block
+ *      where none does makes the frame UNREPAIRABLE, where two or more do AMBIGUOUS.
+ *   5. REPAIRED: every block passes.  `line` is the line the reference would print for the corrected bytes (crc_ok =
+ *      ok_3of6 = 1, CRC-stripped datagram, consumed = P, end_sample = bit P - 1); erasures = bits flipped, blocks = blocks
+ *      changed, had_line = 1.
+ * Any other frame, or k_max = 0, or soft = NULL, is repaired exactly as wmb_frame_repair(f, e_max) does.
+ * Why a wrong repair stays rare: DESIGN.md section 8. */
+#define WMB_SOFT_K_MAX 6
+
+int wmb_frame_repair_soft(const wmb_frame *f, const int16_t *soft, uint32_t e_max, uint32_t k_max, wmb_repaired *out);
+
+/* The same done on the device (K4, the erasure repair K4R, then the soft repair K4S), n frames at once; softs[i] is
+ * frame i's soft values (NULL: none). */
+int wmb_frame_repair_soft_device(wmb_ctx *ctx, const wmb_frame *frames, const int16_t *const *softs, size_t n,
+                                 uint32_t e_max, uint32_t k_max, wmb_repaired *out);
+
+/* C1 soft repair on the streaming path.  wmb_set_repair_soft(ctx, k_max), k_max 0 (off, the default) .. WMB_SOFT_K_MAX,
+ * else WMB_E_INVAL; WMB_E_INVAL on a manual_frames context; the state rules of wmb_set_repair, and the setting survives
+ * wmb_reset / wmb_seek.  While wmb_set_repair has repair on, the C1 candidates of the streaming repair (lines with
+ * crc_ok = 0) follow the rule above (wmb_frame_repair_soft with the soft values the gather computes) instead of being
+ * UNREPAIRABLE; their record's end_sample is bit P - 1, the line's last bit, as before.  T1 and S1 candidates are
+ * unchanged.  wmb_boundary_state appends k_max when it is not 0. */
+int wmb_set_repair_soft(wmb_ctx *ctx, uint32_t k_max);
 
 /* CRC-16, polynomial 0x3D65, complemented (t1_c1_packet_decoder.h:463-469) */
 uint16_t wmb_crc16(const uint8_t *data, size_t n);

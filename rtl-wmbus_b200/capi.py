@@ -184,6 +184,12 @@ def _bind(lib):
     lib.wmb_frame_repair_device.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint32, C.c_void_p]
     lib.wmb_set_repair.argtypes = [C.c_void_p, C.c_uint32]
     lib.wmb_take_repairs.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
+    lib.wmb_set_soft_bits.argtypes = [C.c_void_p, C.c_int]
+    lib.wmb_set_repair_soft.argtypes = [C.c_void_p, C.c_uint32]
+    lib.wmb_frame_soft.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.POINTER(C.c_int16))]
+    lib.wmb_frame_repair_soft.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p]
+    lib.wmb_frame_repair_soft_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint32, C.c_uint32,
+                                                 C.c_void_p]
     return lib
 
 
@@ -244,10 +250,14 @@ class WmbusB200:
     quality=True: the signal-quality report, see wmb_set_line_quality() (off by default); it survives reset() and
     seek().  take_lines(quality=True) and take_bursts(quality=True) hand out its records.
     repair=e_max (1..3): erasure repair of the framer's T1 / S1 candidates, see wmb_set_repair() (0: off, the default);
-    it survives reset() and seek().  take_repairs() hands out its records."""
+    it survives reset() and seek().  take_repairs() hands out its records.
+    repair_soft=k_max (1..6): with repair on, the C1 candidates are repaired from the soft values of their bits, see
+    wmb_set_repair_soft() (0: off, the default); it survives reset() and seek().
+    soft_bits=True (manual_frames=1 only): the soft value of every T1/C1 bit, see wmb_set_soft_bits() (off by default); it
+    survives reset() and seek().  frame_soft() returns a polled frame's values and repair_frames(k_max=...) uses them."""
 
     def __init__(self, flags: str = "", device: int = 0, lib=None, clock_lock=None, access_code_errors=None,
-                 burst_level=None, spectrum=None, quality=False, repair=0, **tuning):
+                 burst_level=None, spectrum=None, quality=False, repair=0, repair_soft=0, soft_bits=False, **tuning):
         self.lib = lib or load_library()
         self.opts = opts_from_flags(self.lib, flags, **tuning)
         self._ctx = C.c_void_p()
@@ -286,6 +296,18 @@ class WmbusB200:
         if repair:
             try:
                 self.set_repair(repair)
+            except Exception:
+                self.close()
+                raise
+        if repair_soft:
+            try:
+                self.set_repair_soft(repair_soft)
+            except Exception:
+                self.close()
+                raise
+        if soft_bits:
+            try:
+                self.set_soft_bits(True)
             except Exception:
                 self.close()
                 raise
@@ -386,11 +408,27 @@ class WmbusB200:
     def decode_frames(self, arr, n):
         self._check(self.lib.wmb_decode_frames(self._ctx, arr, n))
 
-    def repair_frames(self, arr, n, e_max=2, device=True):
+    def repair_frames(self, arr, n, e_max=2, device=True, k_max=0, soft=None):
         """Erasure repair (wmb_frame_repair_device, or the host twin wmb_frame_repair with device=False) of the first n
         frames of arr, e.g. what poll() returned with manual_frames=1.  Returns an array of n WmbRepaired; lines of the
-        repaired ones format with repaired_line()."""
+        repaired ones format with repaired_line().
+        k_max (1..6): C1 soft repair too (wmb_frame_repair_soft_device / wmb_frame_repair_soft), with soft[i] the int16
+        soft values of frame i (None: none); soft=None takes frame_soft() of every frame."""
         out = (WmbRepaired * max(n, 1))()
+        if k_max:
+            import numpy as np
+            if soft is None:
+                soft = [self.frame_soft(arr[i]) for i in range(n)]
+            soft = [None if v is None else np.ascontiguousarray(v, np.int16) for v in soft]
+            ptrs = (C.c_void_p * max(n, 1))(*[None if v is None else v.ctypes.data for v in soft[:n]])
+            if device:
+                self._check(self.lib.wmb_frame_repair_soft_device(self._ctx, C.addressof(arr), ptrs, n, e_max, k_max,
+                                                                  C.addressof(out)))
+            else:
+                for i in range(n):
+                    self._check(self.lib.wmb_frame_repair_soft(C.addressof(arr[i]), ptrs[i], e_max, k_max,
+                                                               C.addressof(out[i])))
+            return out
         if device:
             self._check(self.lib.wmb_frame_repair_device(self._ctx, C.addressof(arr), n, e_max, C.addressof(out)))
         else:
@@ -491,6 +529,25 @@ class WmbusB200:
     def set_line_quality(self, on: bool):
         """signal-quality report on / off (before the first push, or after reset/seek)"""
         self._check(self.lib.wmb_set_line_quality(self._ctx, 1 if on else 0))
+
+    def set_repair_soft(self, k_max: int):
+        """C1 soft repair of the streaming framer's candidates, k_max 1..6 (0 = off; before the first push, or after reset()
+        / seek()); it acts while set_repair() has repair on"""
+        self._check(self.lib.wmb_set_repair_soft(self._ctx, k_max))
+
+    def set_soft_bits(self, on: bool):
+        """soft values of the T1/C1 bits (before the first push, or after reset() / seek())"""
+        self._check(self.lib.wmb_set_soft_bits(self._ctx, int(bool(on))))
+
+    def frame_soft(self, frame):
+        """the int16 soft values of a frame of the last poll(), parallel to its bits (a copy); None for S1 frames or
+        when soft values are off"""
+        import numpy as np
+        p = C.POINTER(C.c_int16)()
+        self._check(self.lib.wmb_frame_soft(self._ctx, C.addressof(frame), C.byref(p)))
+        if not p:
+            return None
+        return np.ctypeslib.as_array(p, (frame.nbits,)).copy()
 
     def set_repair(self, e_max: int):
         """erasure repair of the streaming framer's candidates, e_max 1..3 (0 = off; before the first push, or after

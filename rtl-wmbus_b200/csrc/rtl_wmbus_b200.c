@@ -45,6 +45,10 @@
  *   WMBUS_B200_REPAIR_ERASURES=<n>  erasures repaired per CRC block, 1..3 (default 1: the lowest rate of wrong repairs,
  *                              DESIGN.md 8).  A path that cannot be opened, a bad value, or this variable without
  *                              WMBUS_B200_REPAIRED is an error at start-up.  stdout does not change.
+ *   WMBUS_B200_REPAIR_SOFT_BITS=<k>  also repair C1 telegrams from the soft values of their bits, searching the k (1..6)
+ *                              least reliable bits of each failing CRC block (wmb_set_repair_soft; DESIGN.md 8).  Unset:
+ *                              C1 is not repaired.  A bad value, or this variable without WMBUS_B200_REPAIRED, is an
+ *                              error at start-up.
  */
 #define _GNU_SOURCE
 #include <errno.h>
@@ -436,6 +440,19 @@ int main(int argc, char *argv[])
             return EXIT_FAILURE;
         }
     }
+    unsigned long repair_k = 0;
+    if ((e = getenv("WMBUS_B200_REPAIR_SOFT_BITS")) != NULL) {
+        char *end = NULL;
+        repair_k = strtoul(e, &end, 10);
+        if (!getenv("WMBUS_B200_REPAIRED")) {
+            fprintf(stderr, "rtl_wmbus_b200: WMBUS_B200_REPAIR_SOFT_BITS needs WMBUS_B200_REPAIRED\n");
+            return EXIT_FAILURE;
+        }
+        if (e[0] < '0' || e[0] > '9' || *end || repair_k < 1 || repair_k > WMB_SOFT_K_MAX) {
+            fprintf(stderr, "rtl_wmbus_b200: WMBUS_B200_REPAIR_SOFT_BITS=%s: expected 1 .. %d\n", e, WMB_SOFT_K_MAX);
+            return EXIT_FAILURE;
+        }
+    }
     if ((e = getenv("WMBUS_B200_REPAIRED")) != NULL && (g_rep_file = fopen(e, "w")) == NULL) {
         fprintf(stderr, "rtl_wmbus_b200: WMBUS_B200_REPAIRED=%s: %s\n", e, strerror(errno));
         return EXIT_FAILURE;
@@ -461,7 +478,7 @@ int main(int argc, char *argv[])
         fprintf(stderr, "rtl_wmbus_b200: %s\n", wmb_last_error());
         return EXIT_FAILURE;
     }
-    if (g_rep_file && wmb_set_repair(ctx, (uint32_t)repair_e) != WMB_OK) {
+    if (g_rep_file && (wmb_set_repair(ctx, (uint32_t)repair_e) != WMB_OK || wmb_set_repair_soft(ctx, (uint32_t)repair_k) != WMB_OK)) {
         fprintf(stderr, "rtl_wmbus_b200: %s\n", wmb_last_error());
         return EXIT_FAILURE;
     }

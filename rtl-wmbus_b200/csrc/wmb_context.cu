@@ -79,6 +79,7 @@ struct Stream {                     /* one (chain, algo) bit stream */
     uint64_t *pend = nullptr;       /* device: candidates waiting for more bits   */
     OfsAcc *pend_ofs = nullptr;     /* device: their carrier-offset sums          */
     QualAcc *pend_qual = nullptr;   /* device: their quality sums (quality on)    */
+    int16_t *soft_ring = nullptr;   /* device: soft values beside ring (soft values on, T1/C1 only) */
     uint64_t *agg = nullptr;        /* scan scratch [tiles]                       */
     uint64_t total = 0;             /* host mirror of sd->total at the last read  */
     uint64_t total_prev = 0;        /* ... before the last batch read (stage tap) */
@@ -281,6 +282,12 @@ struct wmb_ctx {
     SlotTable<RepHdr> rep;                           /* parallel to hdr */
     std::vector<wmb_repair_record> repairs;          /* records not taken yet */
 
+    /* soft values of the T1/C1 bits (wmb_set_soft_bits on a manual_frames context, or the streaming soft repair; both survive
+     * wmb_reset).  Off: nothing is allocated or launched */
+    bool soft = false;
+    uint32_t repair_k = 0;                           /* wmb_set_repair_soft: k_max of the C1 soft repair K4S (0: off) */
+    int16_t *d_soft_words = nullptr, *h_soft_words = nullptr;    /* parallel to d_words / h_words */
+
     /* band survey (wmb_set_spectrum; the setting survives wmb_reset).  Bins 0: off, nothing is allocated or launched */
     uint32_t spec_bins = 0, spec_B = 0;
     uint32_t spec_R = 0;                             /* ring rows = rows of a result slot: batch blocks / B + 2 */
@@ -305,7 +312,7 @@ struct wmb_ctx {
     /* results */
     uint64_t win_lo = 0, win_hi = ~0ull;             /* line window (access-code match sample) */
     /* manual mode (opts.manual_frames): frames wait here for wmb_poll */
-    struct Held { wmb_frame f; std::vector<uint32_t> words; };
+    struct Held { wmb_frame f; std::vector<uint32_t> words; std::vector<int16_t> soft; /* empty: none */ };
     std::vector<Held> held, held_prev;
     std::vector<wmb_frame> poll_frames;
     bool manual = false;
@@ -334,13 +341,28 @@ static int launch_k2p_fold(wmb_ctx *c, const P1State *p1_end_last, RlState *p2_o
  * pool_n that K4R adds to.  Here the simulated gather has published already, so K4R runs behind it and the batch is
  * published again, with the capacity flags the first publish cleared (n_pend's clamp is idempotent): the record is the
  * one the device writes */
-static int launch_k3_k4(wmb_ctx *c, const K3Params &p, const K4Params *q, const K4RParams *r)
+static int launch_k3_k4(wmb_ctx *c, const K3Params &p, const K4Params *q, const K4RParams *r, const K4SParams *sp)
 {
     const int rc = launch_k3_k4(c, p, q);
-    if (rc || !r) return rc;
+    if (rc) return rc;
+    /* soft values: on the device k3_soft runs between k3_cut and k3_copy.  It reads only what k3_size and k3_cut wrote
+     * (cut_n, never changed again), so here it runs behind the simulated gather, and the copy is redone (the frame words
+     * it writes are the same again) */
+    if (p.soft_words) {
+        const uint32_t n = p.gd->n;
+        hs_for(n, [&](uint32_t i) { hs_for(4, [&](uint32_t t) { k3_soft(p, i, t, 4); }); });
+        hs_for(n, [&](uint32_t i) { hs_for(4, [&](uint32_t t) { k3_copy(p, i, t, 4); }); });
+        c->st.kernel_launches += 1;
+    }
+    if (!r) return WMB_OK;
     static K4RSmem sm;                  /* the block's phases need real barriers: one simulated thread */
     hs_for(p.gd->n, [&](uint32_t i) { k4r_repair(*r, i, 0, 1, sm); });
     c->st.kernel_launches += 1;
+    if (sp) {
+        static K4SSmem ss;
+        hs_for(p.gd->n, [&](uint32_t i) { k4s_repair(*sp, i, 0, 1, ss); });
+        c->st.kernel_launches += 1;
+    }
     *p.errors |= p.rec->errors & K3_SOFT_ERRORS;
     k3_publish(p);
     return WMB_OK;
@@ -533,7 +555,7 @@ static int launch_k2c(wmb_ctx *c, const K2cParams &p, cudaStream_t st)
 
 /* the whole gather + device framer (+ the erasure repair K4R when r is given); grids are fixed (the kernels loop over
  * however many candidates there are).  K4R adds its datagrams to pool_n, which k3_publish reads: it goes before that */
-static int launch_k3_k4(wmb_ctx *c, const K3Params &p, const K4Params *q, const K4RParams *r)
+static int launch_k3_k4(wmb_ctx *c, const K3Params &p, const K4Params *q, const K4RParams *r, const K4SParams *sp)
 {
     static int sms = 0;
     if (!sms) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c->device);
@@ -541,6 +563,10 @@ static int launch_k3_k4(wmb_ctx *c, const K3Params &p, const K4Params *q, const 
     k3_fill_kernel<<<sms * 2, 256, 0, c->cs>>>(p);
     k3_size_kernel<<<sms, 128, 0, c->cs>>>(p);
     k3_cut_kernel<<<sms * 32, 64, 0, c->cs>>>(p);
+    if (p.soft_words) {
+        k3_soft_kernel<<<sms * 32, 64, 0, c->cs>>>(p);
+        c->st.kernel_launches += 1;
+    }
     k3_offsets_kernel<<<1, SCAN_THREADS, 0, c->cs>>>(p);
     k3_copy_kernel<<<sms * 32, 128, 0, c->cs>>>(p);
     k3_carry_kernel<<<sms, 128, 0, c->cs>>>(p);
@@ -551,6 +577,10 @@ static int launch_k3_k4(wmb_ctx *c, const K3Params &p, const K4Params *q, const 
     }
     if (r) {
         k4r_repair_kernel<<<sms * 64, K4_THREADS, 0, c->cs>>>(*r);
+        c->st.kernel_launches += 1;
+    }
+    if (sp) {                                /* C1 soft repair: overwrites K4R's record of a C1 line with CRC errors */
+        k4s_repair_kernel<<<sms * 64, K4_THREADS, 0, c->cs>>>(*sp);
         c->st.kernel_launches += 1;
     }
     k3_publish_kernel<<<1, 32, 0, c->cs>>>(p);
@@ -998,6 +1028,19 @@ static int qual_alloc(wmb_ctx *c)
         TRY(c->qual.alloc(c, 1, c->hdr.cap, c->hdr.prefix, 256));
     }
     if (c->burst_allocated && !c->bqual.d) TRY(c->bqual.alloc(c, WMB_N_CHAINS, c->brec.cap, c->brec.prefix, 64));
+    return WMB_OK;
+}
+
+/* soft values: a ring beside each T1/C1 stream's ring, the frame words' twin, and its host mirror for manual mode */
+static int soft_alloc(wmb_ctx *c)
+{
+    if (c->d_soft_words) return WMB_OK;
+    for (int a = 0; a < WMB_N_ALGOS; a++) {
+        Stream &s = c->cb[WMB_CHAIN_T1C1].s[a];
+        if (s.ring) TRY(dev_alloc(c, &s.soft_ring, s.ring_cap));
+    }
+    TRY(dev_alloc(c, &c->d_soft_words, c->frame_words_cap));
+    if (c->manual) TRY(host_alloc(c, &c->h_soft_words, c->frame_words_cap));
     return WMB_OK;
 }
 
@@ -1694,7 +1737,10 @@ static int enqueue_gather(wmb_ctx *c, bool final, bool after_batch)
     if (bursts) TRY(burst_alloc(c));
     if (quality) TRY(qual_alloc(c));
     const bool repair = c->repair_e && !c->manual;
+    const bool repair_soft = repair && c->repair_k;          /* C1 candidates: K4S behind K4R, on the soft values */
+    const bool soft = c->soft || repair_soft;
     if (repair && !c->rep.d) TRY(c->rep.alloc(c, 1, c->hdr.cap, c->hdr.prefix, 256));     /* first gather with repair on */
+    if (soft) TRY(soft_alloc(c));
     if (any_sync) {
         K3Params p;
         memset(&p, 0, sizeof(p));
@@ -1707,6 +1753,7 @@ static int enqueue_gather(wmb_ctx *c, bool final, bool after_batch)
                 p.ring[k] = s.ring; p.ring_mask[k] = s.ring_cap - 1; p.sd[k] = s.sd; p.cand[k] = s.cand; p.pend[k] = s.pend;
                 p.pend_ofs[k] = s.pend_ofs;
                 if (quality) p.pend_qual[k] = s.pend_qual;
+                if (soft) p.soft_ring[k] = s.soft_ring;
             }
             p.dphi[ch] = c->cb[ch].set[c->last_set].dphi;
         }
@@ -1721,6 +1768,7 @@ static int enqueue_gather(wmb_ctx *c, bool final, bool after_batch)
         p.cut_n = c->d_cut_n; p.agg = c->d_k3_agg; p.errors = c->d_errors;
         p.final = final ? 1u : 0u;
         if (quality) { p.qual_log = c->qual.d; p.qual_skip = c->o.accurate_atan ? 0u : 1u; }
+        if (soft) p.soft_words = c->d_soft_words;
         K4Params q;
         memset(&q, 0, sizeof(q));
         q.hdr = c->hdr.d; q.words = c->d_words; q.dec = c->dec.d;
@@ -1729,7 +1777,11 @@ static int enqueue_gather(wmb_ctx *c, bool final, bool after_batch)
         memset(&r, 0, sizeof(r));
         r.hdr = q.hdr; r.dec = q.dec; r.words = q.words; r.rep = c->rep.d; r.pool = q.pool; r.pool_cap = q.pool_cap;
         r.pool_n = q.pool_n; r.errors = q.errors; r.e_max = c->repair_e; r.gd = q.gd;
-        TRY(launch_k3_k4(c, p, c->manual ? nullptr : &q, repair ? &r : nullptr));
+        K4SParams sp;
+        memset(&sp, 0, sizeof(sp));
+        sp.hdr = r.hdr; sp.dec = r.dec; sp.words = r.words; sp.soft = c->d_soft_words; sp.rep = r.rep; sp.pool = r.pool;
+        sp.pool_cap = r.pool_cap; sp.pool_n = r.pool_n; sp.errors = r.errors; sp.k_max = c->repair_k; sp.gd = r.gd;
+        TRY(launch_k3_k4(c, p, c->manual ? nullptr : &q, repair ? &r : nullptr, repair_soft ? &sp : nullptr));
         /* results -> pinned host mirror: the record and a prefix of the arrays it describes (the rest, if a batch ever
          * produces more, is fetched when the record has been read) */
         CUDA_TRY(cudaMemcpyAsync(c->h_rec + slot, c->d_rec + slot, sizeof(BatchRec), cudaMemcpyDeviceToHost, c->cs));
@@ -1862,6 +1914,10 @@ static int consume_oldest(wmb_ctx *c)
     if (!f.dec && r.n_words) {               /* manual mode reads after every batch: the frame words are this batch's */
         CUDA_TRY(cudaMemcpyAsync(c->h_words, c->d_words, (size_t)r.n_words * 4, cudaMemcpyDeviceToHost, c->xs));
         c->st.d2h_bytes += (uint64_t)r.n_words * 4;
+        if (c->soft) {
+            CUDA_TRY(cudaMemcpyAsync(c->h_soft_words, c->d_soft_words, (size_t)r.n_words * 2, cudaMemcpyDeviceToHost, c->xs));
+            c->st.d2h_bytes += (uint64_t)r.n_words * 2;
+        }
         more = true;
     }
     if (more) CUDA_TRY(cudaStreamSynchronize(c->xs));
@@ -1928,6 +1984,8 @@ static int consume_oldest(wmb_ctx *c)
             if (!slot) { c->held.emplace_back(); slot = &c->held.back(); }
             slot->f = fr;
             slot->words.assign(c->h_words + h.word_off, c->h_words + h.word_off + h.nbits);
+            if (c->soft && h.chain == WMB_CHAIN_T1C1) slot->soft.assign(c->h_soft_words + h.word_off, c->h_soft_words + h.word_off + h.nbits);
+            else slot->soft.clear();
         }
     }
     c->st.host_decode_ms += wall_ms() - t1;
@@ -2240,8 +2298,15 @@ static void decoded_from(const DecHdr &d, uint64_t sync_sample, const uint8_t *p
     memcpy(o.datagram, pool + d.data_off, d.len);
 }
 
-/* a K4R verdict -> the repair of one candidate, its datagram out of the pool */
-static void repaired_from(const RepHdr &h, uint64_t sync_sample, int chain, const uint8_t *pool, wmb_repaired &o)
+/* the mode of a candidate's repaired line: K4R repairs T1 and S1 telegrams, K4S C1 lines (K4's verdict says which) */
+static int rep_mode(int chain, const DecHdr &d)
+{
+    if (chain != WMB_CHAIN_T1C1) return 2;
+    return d.status == K4_LINE && d.mode == 1 ? 1 : 0;
+}
+
+/* a K4R / K4S verdict -> the repair of one candidate, its datagram out of the pool */
+static void repaired_from(const RepHdr &h, uint64_t sync_sample, int mode, const uint8_t *pool, wmb_repaired &o)
 {
     static const char modes[3][3] = { "T1", "C1", "S1" };
     memset(&o, 0, sizeof(o));
@@ -2250,7 +2315,7 @@ static void repaired_from(const RepHdr &h, uint64_t sync_sample, int chain, cons
     o.erasures = h.erasures; o.blocks = h.blocks;
     wmb_decoded &d = o.line;
     d.status = WMB_DEC_LINE; d.consumed = h.consumed; d.end_sample = sync_sample + h.end_off;
-    memcpy(d.mode, modes[chain == WMB_CHAIN_T1C1 ? 0 : 2], 3);
+    memcpy(d.mode, modes[mode], 3);
     d.crc_ok = 1; d.ok_3of6 = 1; d.packet_rssi = h.packet_rssi; d.current_rssi = h.current_rssi;
     d.serial = h.serial; d.len = h.len;
     memcpy(d.datagram, pool + h.data_off, h.len);
@@ -2260,7 +2325,7 @@ static void repaired_from(const RepHdr &h, uint64_t sync_sample, int chain, cons
  * the gather that delivers it with all its bits (not partial).  An S1 abort is accepted as soon as K4 sees the
  * violation, usually long before bit P - 1: K3 carries it on, and it waits in its stream's rep_wait list for that
  * gather.  A waiting frame that a gather does not deliver was lost in an overflow (counted there). */
-static void book_repairs(wmb_ctx *c, const FrameHdr *hdr, const RepHdr *rep, const uint8_t *pool, size_t n,
+static void book_repairs(wmb_ctx *c, const FrameHdr *hdr, const DecHdr *dec, const RepHdr *rep, const uint8_t *pool, size_t n,
                          const std::vector<uint32_t> &idx, const std::vector<size_t> &accepted, bool final)
 {
     std::vector<wmb_repair_record> fresh;
@@ -2273,7 +2338,7 @@ static void book_repairs(wmb_ctx *c, const FrameHdr *hdr, const RepHdr *rep, con
         memset(&r, 0, sizeof(r));
         r.sync_sample = hdr[i].sync_sample; r.end_sample = hdr[i].sync_sample + h.end_off;
         r.chain = hdr[i].chain; r.algo = hdr[i].algo;
-        repaired_from(h, hdr[i].sync_sample, hdr[i].chain, pool, r.repair);
+        repaired_from(h, hdr[i].sync_sample, rep_mode(hdr[i].chain, dec[i]), pool, r.repair);
         fresh.push_back(r);
     };
     /* the frames of a gather are in stream order: (chain, algo, ordinal) ascending */
@@ -2346,7 +2411,7 @@ static int book_device_frames(wmb_ctx *c, const FrameHdr *hdr, const DecHdr *dec
         },
         [&](size_t k, wmb_decoded &o) { decoded_from(dec[idx[k]], hdr[idx[k]].sync_sample, pool, o); },
         rep ? &accepted : nullptr));
-    if (rep) book_repairs(c, hdr, rep, pool, n, idx, accepted, final);
+    if (rep) book_repairs(c, hdr, dec, rep, pool, n, idx, accepted, final);
     return WMB_OK;
 }
 
@@ -2431,7 +2496,76 @@ extern "C" int wmb_frame_repair_device(wmb_ctx *c, const wmb_frame *frames, size
         const RepHdr &h = rep[i];
         if (h.outcome == K4R_REPAIRED && h.data_off == 0xFFFFFFFFu)
             return set_err(WMB_E_OVERFLOW, "datagram pool full: hand in fewer frames at once");
-        repaired_from(h, frames[i].sync_sample, frames[i].chain, c->pool.h, out[i]);
+        repaired_from(h, frames[i].sync_sample, frames[i].chain == WMB_CHAIN_T1C1 ? 0 : 2, c->pool.h, out[i]);
+    }
+    return WMB_OK;
+}
+
+static int launch_k4s(wmb_ctx *c, const K4SParams &p)
+{
+#ifdef WMB_HOSTSIM
+    static K4SSmem sm;                  /* the block's phases need real barriers: one simulated thread */
+    hs_for(p.n, [&](uint32_t i) { k4s_repair(p, i, 0, 1, sm); });
+#else
+    k4s_repair_kernel<<<p.n ? p.n : 1, K4_THREADS, 0, c->cs>>>(p);
+    CUDA_TRY(cudaGetLastError());
+#endif
+    c->st.kernel_launches += 1;
+    return WMB_OK;
+}
+
+/* Test hook (wmbus_b200_framer.h): K4, the erasure repair K4R and the C1 soft repair K4S on caller-made frames, to compare
+ * with the host twin wmb_frame_repair_soft() frame by frame. */
+extern "C" int wmb_frame_repair_soft_device(wmb_ctx *c, const wmb_frame *frames, const int16_t *const *softs, size_t n,
+                                            uint32_t e_max, uint32_t k_max, wmb_repaired *out)
+{
+    if (!c || !frames || !out || (!softs && n)) return set_err(WMB_E_INVAL, "null argument");
+    if (k_max > WMB_SOFT_K_MAX) return set_err(WMB_E_INVAL, "k_max %u out of range 0..%d", k_max, WMB_SOFT_K_MAX);
+    if (k_max == 0) return wmb_frame_repair_device(c, frames, n, e_max, out);
+    if (e_max > K4R_MAX_ERASURES) return set_err(WMB_E_INVAL, "e_max %u out of range 0..%d", e_max, K4R_MAX_ERASURES);
+    memset(out, 0, n * sizeof(*out));
+    if (n == 0) return WMB_OK;
+    TRY(upload_and_decode(c, frames, n));
+    std::vector<int16_t> hsoft;
+    std::vector<uint8_t> hok(n);
+    for (size_t i = 0; i < n; i++) {
+        hok[i] = softs[i] ? 1 : 0;
+        for (uint32_t j = 0; j < frames[i].nbits; j++) hsoft.push_back(softs[i] ? softs[i][j] : (int16_t)WMB_SOFT_NONE);
+    }
+    RepHdr *d_rep = nullptr;
+    int16_t *d_soft = nullptr;
+    uint8_t *d_ok = nullptr;
+    if (cudaMalloc((void **)&d_rep, n * sizeof(RepHdr)) != cudaSuccess) return set_err(WMB_E_NOMEM, "cudaMalloc of the repair table failed");
+    std::unique_ptr<RepHdr, cudaError_t (*)(void *)> guard(d_rep, cudaFree);
+    if (cudaMalloc((void **)&d_soft, std::max<size_t>(hsoft.size(), 1) * 2) != cudaSuccess) return set_err(WMB_E_NOMEM, "cudaMalloc of the soft values failed");
+    std::unique_ptr<int16_t, cudaError_t (*)(void *)> guard_s(d_soft, cudaFree);
+    if (cudaMalloc((void **)&d_ok, n) != cudaSuccess) return set_err(WMB_E_NOMEM, "cudaMalloc of the soft flags failed");
+    std::unique_ptr<uint8_t, cudaError_t (*)(void *)> guard_o(d_ok, cudaFree);
+    CUDA_TRY(cudaMemcpyAsync(d_soft, hsoft.data(), hsoft.size() * 2, cudaMemcpyHostToDevice, c->cs));
+    CUDA_TRY(cudaMemcpyAsync(d_ok, hok.data(), n, cudaMemcpyHostToDevice, c->cs));
+    K4RParams r;
+    memset(&r, 0, sizeof(r));
+    r.hdr = c->hdr.d; r.dec = c->dec.d; r.n = (uint32_t)n; r.words = c->d_words; r.rep = d_rep;
+    r.pool = c->pool.d; r.pool_cap = (uint32_t)c->pool.cap; r.pool_n = GD_FIELD(c, pool_n); r.errors = c->d_errors;
+    r.e_max = e_max;
+    if (e_max) TRY(launch_k4r(c, r));
+    else CUDA_TRY(cudaMemsetAsync(d_rep, 0, n * sizeof(RepHdr), c->cs));      /* every record NONE, as K4R's off */
+    K4SParams s;
+    memset(&s, 0, sizeof(s));
+    s.hdr = r.hdr; s.dec = r.dec; s.n = r.n; s.words = r.words; s.soft = d_soft; s.soft_ok = d_ok; s.rep = d_rep;
+    s.pool = r.pool; s.pool_cap = r.pool_cap; s.pool_n = r.pool_n; s.errors = r.errors; s.k_max = k_max;
+    TRY(launch_k4s(c, s));
+    std::vector<RepHdr> rep(n);
+    CUDA_TRY(cudaMemcpyAsync(rep.data(), d_rep, n * sizeof(RepHdr), cudaMemcpyDeviceToHost, c->cs));
+    TRY(c->dec.fetch(0, 0, 0, (uint32_t)n, c->cs));                          /* (the mode of a repaired line) */
+    TRY(c->pool.fetch(0, 0, 0, (uint32_t)std::min<size_t>(c->pool.cap, 1u << 24), c->cs));
+    CUDA_TRY(cudaMemsetAsync(GD_FIELD(c, pool_n), 0, 4, c->cs));
+    CUDA_TRY(cudaStreamSynchronize(c->cs));
+    for (size_t i = 0; i < n; i++) {
+        const RepHdr &h = rep[i];
+        if (h.outcome == K4R_REPAIRED && h.data_off == 0xFFFFFFFFu)
+            return set_err(WMB_E_OVERFLOW, "datagram pool full: hand in fewer frames at once");
+        repaired_from(h, frames[i].sync_sample, rep_mode(frames[i].chain, c->dec.h[i]), c->pool.h, out[i]);
     }
     return WMB_OK;
 }
@@ -2738,6 +2872,40 @@ extern "C" int wmb_set_repair(wmb_ctx *c, uint32_t e_max)
     return WMB_OK;
 }
 
+extern "C" int wmb_set_soft_bits(wmb_ctx *c, int on)
+{
+    if (!c) return set_err(WMB_E_INVAL, "null argument");
+    if (on != 0 && on != 1) return set_err(WMB_E_INVAL, "soft bits %d: 0 (off) or 1 (on)", on);
+    if (!c->manual) return set_err(WMB_E_INVAL, "wmb_set_soft_bits needs a manual_frames context (the streaming framer's soft repair: wmb_set_repair_soft)");
+    if (c->batch_no != 0 || !c->remainder.empty())
+        return set_err(WMB_E_STATE, "wmb_set_soft_bits after samples were pushed (call it before the first push or after wmb_reset / wmb_seek)");
+    c->soft = on != 0;
+    return WMB_OK;
+}
+
+extern "C" int wmb_set_repair_soft(wmb_ctx *c, uint32_t k_max)
+{
+    if (!c) return set_err(WMB_E_INVAL, "null argument");
+    if (c->manual) return set_err(WMB_E_INVAL, "wmb_set_repair_soft on a manual_frames context (repair the polled frames with wmb_frame_repair_soft_device)");
+    if (k_max > WMB_SOFT_K_MAX) return set_err(WMB_E_INVAL, "k_max %u out of range 0 (off) .. %d", k_max, WMB_SOFT_K_MAX);
+    if (c->batch_no != 0 || !c->remainder.empty())
+        return set_err(WMB_E_STATE, "wmb_set_repair_soft after samples were pushed (call it before the first push or after wmb_reset / wmb_seek)");
+    c->repair_k = k_max;
+    return WMB_OK;
+}
+
+extern "C" int wmb_frame_soft(wmb_ctx *c, const wmb_frame *f, const int16_t **soft)
+{
+    if (!c || !f || !soft) return set_err(WMB_E_INVAL, "null argument");
+    *soft = nullptr;
+    for (const auto &h : c->held_prev)
+        if (h.words.data() == f->bits) {
+            if (!h.soft.empty()) *soft = h.soft.data();
+            return WMB_OK;
+        }
+    return set_err(WMB_E_INVAL, "not a frame of the last wmb_poll");
+}
+
 extern "C" int wmb_take_repairs(wmb_ctx *c, wmb_repair_record *out, size_t cap, size_t *n)
 {
     if (!c || !n || (!out && cap)) return set_err(WMB_E_INVAL, "null argument");
@@ -2871,6 +3039,7 @@ extern "C" long wmb_boundary_state(wmb_ctx *c, uint8_t *buf, size_t cap)
         }
     }
     if (c->repair_e) put(&c->repair_e, 4);             /* contexts that repair differently never agree */
+    if (c->repair_k) put(&c->repair_k, 4);
     if (out.size() > cap) return set_err(WMB_E_INVAL, "buffer too small (%zu bytes needed)", out.size());
     memcpy(buf, out.data(), out.size());
     return (long)out.size();

@@ -58,15 +58,12 @@ static int crc_check_a(const uint8_t *p, size_t n)
     return 1;
 }
 
-/* format B: CRC over the first 126 bytes, then over the rest (:508-536) */
+/* format B: CRC over the first 126 bytes, then over the rest (:508-536); layout in wmb_frame_a.h */
 static int crc_check_b(const uint8_t *p, size_t n)
 {
     if (n < 12) return 0;
-    for (size_t off = 0; off < n;) {
-        const size_t blk = (n - off >= 128) ? 128 : n - off;
-        if (!block_ok(p + off, blk)) return 0;
-        off += blk;
-    }
+    for (uint32_t j = 0; j < wmb_nblk_b((uint32_t)n); j++)
+        if (!block_ok(p + wmb_blk_off_b(j), wmb_blk_len_b((uint32_t)n, j))) return 0;
     return 1;
 }
 
@@ -388,6 +385,97 @@ int wmb_frame_repair(const wmb_frame *f, uint32_t e_max, wmb_repaired *out)
     out->erasures = erasures;
     out->blocks = blocks;
     return WMB_OK;
+}
+
+/* ---- C1 soft repair (definition in wmbus_b200_framer.h; device twin: K4S, wmb_kernels.cuh) ------------------------ */
+
+/* a before b in the search order: a bit without a value first, then lower r, then lower index */
+static int soft_before(int sa, int64_t ra, unsigned ja, int sb, int64_t rb, unsigned jb)
+{
+    if (sa != sb) return sa < sb;
+    if (ra != rb) return ra < rb;
+    return ja < jb;
+}
+
+static void repair_soft_c1(const wmb_frame *f, const int16_t *soft, uint32_t k_max, wmb_repaired *out)
+{
+    const wmb_bit *b = f->bits;
+    out->had_line = 1;
+    out->outcome = WMB_REP_UNREPAIRABLE;
+    const int bframe = bits_at(b, 1, 12) == 0x543u;
+    const unsigned L = bits_at(b, 17, 8);
+    const unsigned len = bframe ? 1 + L : wmb_tlg_length_format_a(L);
+    const unsigned P = 17 + 8 * len;
+    if (len < 12) return;
+
+    uint8_t pkt[292];
+    memset(pkt, 0, sizeof(pkt));
+    for (unsigned l = 0; l < len; l++) pkt[l] = (uint8_t)bits_at(b, 17 + 8 * l, 8);
+    int64_t n0 = 0, n1 = 0, s0 = 0, s1 = 0;
+    for (unsigned j = 17; j < P; j++) {
+        if (soft[j] == WMB_SOFT_NONE) continue;
+        if (WMB_BIT_DATA(b[j])) { n1++; s1 += soft[j]; } else { n0++; s0 += soft[j]; }
+    }
+    /* r of bit j; has[j] = 0 for a bit without a value */
+    static __thread int64_t r[8 * 292];
+    static __thread int has[8 * 292];
+    for (unsigned j = 17; j < P; j++) {
+        const int64_t sign = WMB_BIT_DATA(b[j]) ? 1 : -1, v = soft[j];
+        has[j - 17] = soft[j] != WMB_SOFT_NONE;
+        r[j - 17] = !has[j - 17] ? 0 : n0 * n1 == 0 ? sign * v : sign * (v * 2 * n0 * n1 - (s1 * n0 + s0 * n1));
+    }
+
+    const unsigned nblk = bframe ? wmb_nblk_b(len) : wmb_nblk_a(len);
+    unsigned flips = 0, blocks = 0;
+    for (unsigned k = 0; k < nblk; k++) {
+        const unsigned off = bframe ? wmb_blk_off_b(k) : wmb_blk_off_a(k), blk = bframe ? wmb_blk_len_b(len, k) : wmb_blk_len_a(len, k);
+        if (block_ok(pkt + off, blk)) continue;
+        /* the K least reliable flippable bits, by selection */
+        const unsigned lo = 17 + 8 * (off ? off : 1), hi = 17 + 8 * (off + blk);
+        const unsigned K = k_max < hi - lo ? k_max : hi - lo;
+        unsigned sel[WMB_SOFT_K_MAX];
+        for (unsigned t = 0; t < K; t++) {
+            int found = 0;
+            for (unsigned j = lo; j < hi; j++) {
+                int taken = 0;
+                for (unsigned u = 0; u < t; u++) taken |= sel[u] == j;
+                if (taken) continue;
+                if (!found || soft_before(has[j - 17], r[j - 17], j, has[sel[t] - 17], r[sel[t] - 17], sel[t])) { sel[t] = j; found = 1; }
+            }
+        }
+        unsigned pass = 0, first = 0;
+        for (unsigned x = 1; x < (1u << K); x++) {
+            uint8_t q[128];
+            memcpy(q, pkt + off, blk);
+            for (unsigned t = 0; t < K; t++)
+                if (x >> t & 1u) q[(sel[t] - 17) / 8 - off] ^= (uint8_t)(0x80u >> ((sel[t] - 17) % 8));
+            if (block_ok(q, blk)) { if (!pass) first = x; pass++; }
+        }
+        if (pass != 1) { out->outcome = pass ? WMB_REP_AMBIGUOUS : WMB_REP_UNREPAIRABLE; return; }
+        for (unsigned t = 0; t < K; t++)
+            if (first >> t & 1u) { pkt[(sel[t] - 17) / 8] ^= (uint8_t)(0x80u >> ((sel[t] - 17) % 8)); flips++; }
+        blocks++;
+    }
+    const cursor c = { f, P - 1, 0 };
+    finish(&c, &out->line, "C1", pkt, len, bframe, 0);
+    out->outcome = WMB_REP_REPAIRED;
+    out->erasures = flips;
+    out->blocks = blocks;
+}
+
+int wmb_frame_repair_soft(const wmb_frame *f, const int16_t *soft, uint32_t e_max, uint32_t k_max, wmb_repaired *out)
+{
+    if (k_max > WMB_SOFT_K_MAX || e_max > REP_MAX_ERASURES) { memset(out, 0, sizeof(*out)); return WMB_E_INVAL; }
+    if (k_max && soft && f->nbits && f->chain == WMB_CHAIN_T1C1) {
+        wmb_decoded d;
+        wmb_frame_decode(f, &d);
+        if (d.status == WMB_DEC_LINE && !d.crc_ok && d.mode[0] == 'C') {
+            memset(out, 0, sizeof(*out));
+            repair_soft_c1(f, soft, k_max, out);
+            return WMB_OK;
+        }
+    }
+    return wmb_frame_repair(f, e_max, out);
 }
 
 /* ---- output --------------------------------------------------------------------- */

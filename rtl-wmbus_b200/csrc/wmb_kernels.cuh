@@ -957,6 +957,7 @@ struct GatherDev {                  /* device-resident state of the gather, one 
     uint64_t n_cand_total[WMB_N_STREAMS]; /* access-code matches since the context was made (statistics) */
     uint32_t lanes_rerun;           /* statistics: refuted speculative lanes                */
     uint32_t rl_fallbacks;          /* statistics: batches redone with the monolithic run-length lanes */
+    uint64_t soft_from[WMB_N_STREAMS];    /* stream totals before the current batch: its events start here (k3_soft) */
 };
 
 struct BatchRec {                   /* what the host needs to know about one gathered batch; written last (k3_publish) */
@@ -979,6 +980,10 @@ struct K3Params {
     QualAcc *pend_qual[WMB_N_STREAMS];   /* carried candidates' class sums, same slots as pend   */
     QualAcc *qual_log;              /* one per candidate, parallel to hdr_log               */
     uint32_t qual_skip;             /* 1 (-a): the records hold zero sums                   */
+    /* soft values (wmb_set_soft_bits): null when off.  soft_ring[k] parallels ring[k] (T1/C1 streams only), soft_words
+     * parallels words */
+    int16_t *soft_ring[WMB_N_STREAMS];
+    int16_t *soft_words;
     uint32_t pend_cap, cand_cap;
     /* the carrier-offset windows of new matches are read from this batch's dphi set: [prefix | batch_m samples], batch
      * sample 0 = decimated sample m_first (40 bits); `clip` samples before it exist since the last reset / seek */
@@ -1017,6 +1022,7 @@ WMB_D void k3_plan(const K3Params &p)
         StreamDev &sd = *p.sd[k];
         if (sd.cand_overflow) { k3_flag(p.errors, 16u); sd.cand_overflow = 0; sd.n_cand = p.cand_cap; }
         g.n_cand_total[k] += sd.n_cand;
+        g.soft_from[k] = g.total_prev[k];
         uint32_t nk = g.n_pend[k] + sd.n_cand;
         /* ring overrun: the batch wrote more events into this stream's ring than it holds (a run-length tracker whose bit
          * length has collapsed, lane after lane): bits of its candidates may be overwritten -- none of THIS stream's
@@ -1212,6 +1218,42 @@ WMB_D void k3_cut(const K3Params &p, uint32_t i, int tid, int nthr)
     }
 }
 
+/* pass 1c (block per candidate, soft values on): the soft value (wmbus_b200_framer.h) of every event of a T1/C1 candidate
+ * that this batch produced, i.e. at a ring position >= the stream's total before the batch, into the soft ring beside the
+ * event.  A candidate exists in every batch that produces one of its events, so each shipped event gets its value here,
+ * with its dphi at hand in the batch's set; overlapping candidates write the same value.  The window ends at or before
+ * the event's own sample (D >= 2) and starts at most 8 * 63 + D + 2 samples before it, inside the set's history prefix. */
+WMB_D void k3_soft(const K3Params &p, uint32_t i, int tid, int nthr)
+{
+    const GatherDev &g = *p.gd;
+    if (i >= g.n || !p.soft_words) return;
+    const FrameHdr &h = p.hdr_log[g.base + i];
+    if (h.chain != WMB_CHAIN_T1C1) return;
+    const int k = h.algo;                                     /* stream k = chain * WMB_N_ALGOS + algo, chain 0 */
+    const uint64_t *ring = p.ring[k];
+    const uint64_t mask = p.ring_mask[k], total = p.sd[k]->total;
+    const bool rla = h.algo == WMB_ALGO_RLA;
+    const float *dphi = p.dphi[WMB_CHAIN_T1C1] + p.prefix;
+    const uint64_t from = g.soft_from[k] > h.ordinal ? g.soft_from[k] : h.ordinal;
+    /* every event k3_size found (the list before a reset cut, and before a frame-word overflow empties it) */
+    for (uint64_t o = from + (uint64_t)tid; o < h.ordinal + p.cut_n[i]; o += (uint64_t)nthr) {
+        const uint64_t m = EVG_M(ring[o & mask]);
+        uint32_t after = 0;                                   /* n - 1 - i: the run's later events at sample m */
+        if (rla)
+            while (after <= 63 && o + 1 + after < total && EVG_M(ring[(o + 1 + after) & mask]) == m) after++;
+        const int64_t c = (int64_t)((m - p.m_first) & EVG_M_MASK) - (rla ? WMB_SOFT_D_RL + 8 * (int64_t)after : WMB_SOFT_D_T2);
+        int16_t v = WMB_SOFT_NONE;
+        if (after <= 63 && c - 2 >= -(int64_t)p.clip) {
+            int64_t sum = 0;
+            for (int64_t q = c - 2; q < c + 3; q++) sum += wmb_ofs_x(dphi[q]);
+            int64_t x = sum >> 12;                            /* floor */
+            x = x > 32767 ? 32767 : x < -32767 ? -32767 : x;
+            v = (int16_t)x;
+        }
+        p.soft_ring[k][o & mask] = v;
+    }
+}
+
 /* pass 2: exclusive scan of nbits -> word offsets (three-phase block scan) */
 WMB_D void k3_offsets_a(const K3Params &p, uint32_t t)
 {
@@ -1267,6 +1309,7 @@ WMB_D void k3_copy(const K3Params &p, uint32_t i, int tid, int nthr)
         uint64_t off = (EVG_M(e) - h.sync_sample) & EVG_M_MASK;
         if (off >= (1u << 23)) off = (1u << 23) - 1;
         p.words[h.word_off + j] = ((uint32_t)off << 9) | (EVG_RSSI(e) << 1) | EVG_BIT(e);
+        if (p.soft_words && h.chain == WMB_CHAIN_T1C1) p.soft_words[h.word_off + j] = p.soft_ring[k][(h.ordinal + j) & mask];
     }
 }
 
@@ -1781,6 +1824,188 @@ WMB_D void k4r_repair(const K4RParams &p, uint32_t f, int tid, int nthr, K4RSmem
     }
 }
 
+/* =========================================================================== */
+/* K4S: soft repair of C1 candidates (definition in wmbus_b200_framer.h, host twin wmb_frame_repair_soft() in
+ * wmb_framer.c).  One warp per candidate, behind K4R: it reads K4's verdict from DecHdr and overwrites K4R's RepHdr of a C1
+ * line with CRC errors (K4R makes those UNREPAIRABLE); every other record stays as K4R wrote it.  The lanes reduce n0, n1,
+ * S0, S1; per failing block they pick the K least reliable bits by K rounds of warp argmin over a key that orders (has a
+ * value, r, bit index) -- unique, so the choice does not depend on the lanes -- compute the K single-bit CRC syndromes (the
+ * CRC is affine: a pattern's syndrome is the received one XOR its bits' syndromes) and test patterns lane and lane + 32.
+ * The passes are summed and the lowest passing pattern kept, whatever the lanes' order. */
+struct K4SParams {
+    const FrameHdr *hdr; const DecHdr *dec; uint32_t n;   /* gd == null: n candidates at hdr / dec / rep (test hook) */
+    const uint32_t *words;
+    const int16_t *soft;            /* parallel to words                                   */
+    const uint8_t *soft_ok;         /* test hook: 0 = this frame has no soft values (null: all have) */
+    RepHdr *rep;
+    uint8_t *pool; uint32_t pool_cap; uint32_t *pool_n;
+    uint32_t *errors;
+    uint32_t k_max;                 /* 1..WMB_SOFT_K_MAX */
+    const GatherDev *gd;
+};
+
+WMB_D uint32_t k4s_count(const K4SParams &p) { return p.gd ? p.gd->n : p.n; }
+
+struct K4SSmem {
+    uint8_t  pkt[296];
+    uint32_t s0;                    /* the current block's syndrome as received           */
+    uint32_t sel[WMB_SOFT_K_MAX];   /* its K least reliable bits                           */
+    uint32_t delta[WMB_SOFT_K_MAX]; /* their single-bit syndromes                          */
+    uint32_t data_off;
+};
+
+/* warp reductions; the CPU build runs a candidate on one simulated lane, which holds the whole result */
+WMB_D int64_t k4s_sum(int64_t x)
+{
+#ifndef WMB_HOSTSIM
+    for (int d = 16; d > 0; d >>= 1) x += __shfl_xor_sync(0xFFFFFFFFu, (long long)x, d);
+#endif
+    return x;
+}
+WMB_D uint64_t k4s_min(uint64_t x)
+{
+#ifndef WMB_HOSTSIM
+    for (int d = 16; d > 0; d >>= 1) {
+        const uint64_t y = __shfl_xor_sync(0xFFFFFFFFu, (unsigned long long)x, d);
+        x = y < x ? y : x;
+    }
+#endif
+    return x;
+}
+
+/* the linear part of the block CRC for one flipped bit: byte q (mask) of a block with nd data bytes, CRC bytes after them */
+WMB_HD uint32_t k4s_delta(uint32_t q, uint32_t mask, uint32_t nd)
+{
+    if (q == nd) return mask << 8;
+    if (q == nd + 1) return mask;
+    uint32_t crc = mask << 8;
+    for (uint32_t u = q; u < nd; u++) {
+        for (int k = 0; k < 8; k++) crc = (crc & 0x8000u) ? ((crc << 1) ^ 0x3D65u) : (crc << 1);
+        crc &= 0xFFFFu;
+    }
+    return crc;
+}
+
+WMB_D void k4s_repair(const K4SParams &p, uint32_t f, int tid, int nthr, K4SSmem &sm)
+{
+    if (f >= k4s_count(p)) return;
+    const uint32_t lb = p.gd ? p.gd->base : 0u;
+    const FrameHdr h = p.hdr[lb + f];
+    const DecHdr d = p.dec[lb + f];
+    if (h.nbits == 0 || d.status != K4_LINE || d.crc_ok || d.mode != 1) return;
+    if (p.soft_ok && !p.soft_ok[f]) return;
+    const uint32_t *b = p.words + h.word_off;
+    const int16_t *sv = p.soft + h.word_off;
+    RepHdr r;
+    r.consumed = 0; r.end_off = 0; r.serial = 0; r.data_off = 0; r.len = 0; r.outcome = K4R_UNREPAIRABLE;
+    r.erasures = 0; r.blocks = 0; r.had_line = 1; r.packet_rssi = 0; r.current_rssi = 0;
+    const bool bframe = k4_bits(b, 1, 12) == 0x543u;
+    const uint32_t L = k4_bits(b, 17, 8);
+    const uint32_t len = bframe ? 1 + L : wmb_tlg_len_a(L);
+    const uint32_t P = 17 + 8 * len;
+    r.consumed = P;
+    r.end_off = WMB_BIT_OFFSET(b[P - 1]);
+    if (len < 12) { if (tid == 0) p.rep[lb + f] = r; return; }
+
+    int64_t n0 = 0, n1 = 0, s0 = 0, s1 = 0;
+    for (uint32_t j = 17 + (uint32_t)tid; j < P; j += (uint32_t)nthr) {
+        const int16_t v = sv[j];
+        if (v == WMB_SOFT_NONE) continue;
+        if (WMB_BIT_DATA(b[j])) { n1++; s1 += v; } else { n0++; s0 += v; }
+    }
+    n0 = k4s_sum(n0); n1 = k4s_sum(n1); s0 = k4s_sum(s0); s1 = k4s_sum(s1);
+    const int64_t a = 2 * n0 * n1, t = s1 * n0 + s0 * n1;
+    /* search key of bit j: (has a value, r, j) in one integer; |r| < 2^38, j < 2^12 */
+    auto key = [&](uint32_t j) -> uint64_t {
+        const int16_t v = sv[j];
+        if (v == WMB_SOFT_NONE) return j;
+        const int64_t sign = WMB_BIT_DATA(b[j]) ? 1 : -1;
+        const int64_t rr = a == 0 ? sign * v : sign * ((int64_t)v * a - t);
+        return ((uint64_t)(rr + ((int64_t)1 << 40)) << 12) | j;
+    };
+    for (uint32_t l = (uint32_t)tid; l < len; l += (uint32_t)nthr) sm.pkt[l] = (uint8_t)k4_bits(b, 17 + 8 * l, 8);
+    K4_SYNC();
+
+    const uint32_t nblk = bframe ? wmb_nblk_b(len) : wmb_nblk_a(len);
+    uint32_t outcome = K4R_NONE, flips = 0, blocks = 0;
+    for (uint32_t k = 0; k < nblk && outcome == K4R_NONE; k++) {
+        const uint32_t off = bframe ? wmb_blk_off_b(k) : wmb_blk_off_a(k), blk = bframe ? wmb_blk_len_b(len, k) : wmb_blk_len_a(len, k);
+        if (blk < 2) { outcome = K4R_UNREPAIRABLE; break; }          /* no CRC: no pattern can pass */
+        if (tid == 0) sm.s0 = k4_crc16(sm.pkt + off, blk - 2) ^ (((uint32_t)sm.pkt[off + blk - 2] << 8) | sm.pkt[off + blk - 1]);
+        K4_SYNC();
+        const uint32_t syn = sm.s0;
+        K4_SYNC();
+        if (syn == 0) continue;
+        const uint32_t lo = 17 + 8 * (off ? off : 1), hi = 17 + 8 * (off + blk);
+        const uint32_t K = p.k_max < hi - lo ? p.k_max : hi - lo;
+        uint64_t prev = 0;
+        for (uint32_t u = 0; u < K; u++) {
+            uint64_t best = ~0ull;
+            for (uint32_t j = lo + (uint32_t)tid; j < hi; j += (uint32_t)nthr) {
+                const uint64_t kj = key(j);
+                if (kj > prev && kj < best) best = kj;
+            }
+            prev = k4s_min(best);
+            if (tid == 0) sm.sel[u] = (uint32_t)(prev & 4095u);
+        }
+        K4_SYNC();
+        for (uint32_t u = (uint32_t)tid; u < K; u += (uint32_t)nthr)
+            sm.delta[u] = k4s_delta((sm.sel[u] - 17) / 8 - off, 0x80u >> ((sm.sel[u] - 17) % 8), blk - 2);
+        K4_SYNC();
+        int64_t npass = 0;
+        uint64_t first = ~0ull;
+        for (uint32_t x = (uint32_t)tid; x < 64; x += (uint32_t)nthr) {
+            if (x == 0 || x >= (1u << K)) continue;
+            uint32_t s = syn;
+            for (uint32_t u = 0; u < K; u++) if (x >> u & 1u) s ^= sm.delta[u];
+            if (s == 0) { npass++; if (x < first) first = x; }
+        }
+        npass = k4s_sum(npass);
+        first = k4s_min(first);
+        if (npass != 1) { outcome = npass ? K4R_AMBIGUOUS : K4R_UNREPAIRABLE; break; }
+        if (tid == 0)
+            for (uint32_t u = 0; u < K; u++)
+                if (first >> u & 1u) sm.pkt[(sm.sel[u] - 17) / 8] ^= (uint8_t)(0x80u >> ((sm.sel[u] - 17) % 8));
+        flips += (uint32_t)wmb_popc((uint32_t)first);
+        blocks++;
+        K4_SYNC();
+    }
+    if (outcome == K4R_NONE) outcome = K4R_REPAIRED;
+    r.outcome = (uint8_t)outcome;
+    if (outcome != K4R_REPAIRED) { if (tid == 0) p.rep[lb + f] = r; return; }
+
+    /* the repaired telegram: CRC-stripped datagram (format A :551-592, format B :595-636) into the pool */
+    const uint32_t out_len = len - 2 * nblk;
+    if (tid == 0) {
+        const uint32_t room = (out_len + 3u) & ~3u;
+        uint32_t o = k4_gadd(p.pool_n, room);
+        if (o > p.pool_cap || room > p.pool_cap - o) {
+#ifdef WMB_HOSTSIM
+            *p.errors |= 8u;
+#else
+            atomicOr(p.errors, 8u);
+#endif
+            o = 0xFFFFFFFFu;
+        }
+        sm.data_off = o;
+    }
+    K4_SYNC();
+    const uint32_t data_off = sm.data_off;
+    if (data_off != 0xFFFFFFFFu)
+        for (uint32_t i = (uint32_t)tid; i < out_len; i += (uint32_t)nthr)
+            p.pool[data_off + i] = bframe ? (i == 0 ? (uint8_t)(sm.pkt[0] - 2 * nblk) : sm.pkt[wmb_strip_src_b(i)])
+                                          : sm.pkt[wmb_strip_src_a(i)];
+    if (tid == 0) {
+        r.serial = (uint32_t)sm.pkt[4] | ((uint32_t)sm.pkt[5] << 8) | ((uint32_t)sm.pkt[6] << 16) | ((uint32_t)sm.pkt[7] << 24);
+        r.data_off = data_off;
+        r.len = (uint16_t)(data_off == 0xFFFFFFFFu ? 0 : out_len);
+        r.erasures = (uint8_t)flips; r.blocks = (uint8_t)blocks;
+        r.packet_rssi = (uint8_t)WMB_BIT_RSSI(b[1]);
+        r.current_rssi = (uint8_t)WMB_BIT_RSSI(b[P - 1]);
+        p.rep[lb + f] = r;
+    }
+}
+
 /* wmb_reset: a new capture starts -- carried states, stream bookkeeping, gather state and error flags back to their
  * initial values, in stream order (no host copies, no synchronisation) */
 struct ResetParams {
@@ -2145,6 +2370,10 @@ __global__ void __launch_bounds__(SCAN_THREADS) k3_offsets_kernel(const K3Params
     __syncthreads();
     k3_offsets_c(p, threadIdx.x);
 }
+__global__ void k3_soft_kernel(const K3Params p)
+{
+    for (uint32_t i = blockIdx.x; i < p.gd->n; i += gridDim.x) k3_soft(p, i, threadIdx.x, blockDim.x);
+}
 __global__ void k3_copy_kernel(const K3Params p)
 {
     for (uint32_t i = blockIdx.x; i < p.gd->n; i += gridDim.x) k3_copy(p, i, threadIdx.x, blockDim.x);
@@ -2169,6 +2398,15 @@ __global__ void __launch_bounds__(K4_THREADS) k4r_repair_kernel(const K4RParams 
     const uint32_t n = k4r_count(p);
     for (uint32_t f = blockIdx.x; f < n; f += gridDim.x) {
         k4r_repair(p, f, threadIdx.x, blockDim.x, sm);
+        __syncthreads();
+    }
+}
+__global__ void __launch_bounds__(K4_THREADS) k4s_repair_kernel(const K4SParams p)
+{
+    __shared__ K4SSmem sm;
+    const uint32_t n = k4s_count(p);
+    for (uint32_t f = blockIdx.x; f < n; f += gridDim.x) {
+        k4s_repair(p, f, threadIdx.x, blockDim.x, sm);
         __syncthreads();
     }
 }

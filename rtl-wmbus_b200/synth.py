@@ -89,11 +89,14 @@ def chips_s1(wire: bytes, preamble_pairs: int = 40, post_pairs: int = 4) -> np.n
 
 
 def fsk_burst(chips: np.ndarray, chip_rate: float, fs: float, dev_hz: float, offset_hz: float,
-              amp: float) -> np.ndarray:
-    """Phase-continuous 2-FSK, chip 1 = +deviation.  Returns float32 array [n, 2] (I, Q)."""
+              amp: float, chip_dev: np.ndarray | None = None) -> np.ndarray:
+    """Phase-continuous 2-FSK, chip 1 = +deviation (chip_dev: a factor on chip i's deviation).  Returns float32 array
+    [n, 2] (I, Q)."""
     n = int(math.ceil(len(chips) * fs / chip_rate))
     idx = np.minimum((np.arange(n, dtype=np.float64) * (chip_rate / fs)).astype(np.int64), len(chips) - 1)
     f = offset_hz + dev_hz * (2.0 * chips[idx].astype(np.float64) - 1.0)
+    if chip_dev is not None:
+        f = offset_hz + (f - offset_hz) * np.asarray(chip_dev, np.float64)[idx]
     phase = 2.0 * math.pi * np.cumsum(f) / fs
     return np.stack([amp * np.cos(phase), amp * np.sin(phase)], axis=1).astype(np.float32)
 
@@ -112,6 +115,8 @@ class Emitter:
     seed: int = 1
     sync_flips: tuple = ()       # chips of the access code sent inverted in every telegram, counted back from its last chip
     data_flips: tuple = ()       # chips after the access code sent inverted in every telegram (0: the L-field's first chip)
+    weak_flips: tuple = ()       # chips after the access code sent on the wrong tone at weak_dev of the deviation (0: as data_flips)
+    weak_dev: float = 0.2        # the low-reliability error noise makes; data_flips is the full-swing one
     chip_rate: float = field(init=False)
 
     def __post_init__(self):
@@ -145,6 +150,15 @@ class Emitter:
             c = c.copy()
             c[end + np.asarray(self.data_flips)] ^= 1
         return c
+
+    def chip_dev(self):
+        """per chip, the fraction of dev_hz it is sent at (None: all at full deviation): -weak_dev at weak_flips"""
+        if not self.weak_flips:
+            return None
+        end = 2 * 40 + len(SYNC_S1) if self.mode == "S1" else 2 * 24 + len(SYNC_T1C1)
+        dev = np.ones(len(self._chips(0)))
+        dev[end + np.asarray(self.weak_flips)] = -self.weak_dev
+        return dev
 
     def _chips(self, k: int) -> np.ndarray:
         p = self.payload(k)
@@ -231,7 +245,7 @@ def synth_capture(n_bytes: int, fs: float = 1.6e6, emitters=None, seed: int = 0x
             if key not in burst_cache:
                 e = emitters[p.emitter]
                 shift = center_shift_hz if e.mode != "S1" else -center_shift_hz
-                b = fsk_burst(e.chips(p.k), e.chip_rate, fs, e.dev_hz, e.offset_hz + shift, e.amp)
+                b = fsk_burst(e.chips(p.k), e.chip_rate, fs, e.dev_hz, e.offset_hz + shift, e.amp, e.chip_dev())
                 burst_cache[key] = torch.from_numpy(b).to(dev)
             b = burst_cache[key]
             a0, a1 = max(s0, p.start_iq), min(s1, p.start_iq + b.shape[0])

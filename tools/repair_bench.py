@@ -1,6 +1,7 @@
-"""What erasure repair on the streaming path (wmb_set_repair) costs and what it gains.
-    python tools/repair_bench.py cost [steps]          GPU: step times, repair off against e_max 3
-    python tools/repair_bench.py gain [--cpu] [MiB]    the noise sweep (GPU library, or the CPU build with --cpu)
+"""What erasure repair on the streaming path (wmb_set_repair) and the C1 soft repair (wmb_set_repair_soft) cost and gain.
+    python tools/repair_bench.py cost [steps]              GPU: step times, repair off against e_max 3 and e_max 3 + k_max 6
+    python tools/repair_bench.py gain [--cpu] [MiB]        the noise sweep (GPU library, or the CPU build with --cpu)
+    python tools/repair_bench.py gain-soft [--cpu] [MiB]   the same for C1 telegrams and k_max 1 .. 6
 
 cost: the benchmark's default step -- 1 GiB of synthetic 1.6 MS/s cu8 with two T1 emitters, `-p S`, device-resident, one
 process_device per step -- then the same at clock lock 1 with T1/C1 access-code errors 3 (about 486 k matches per
@@ -9,7 +10,11 @@ CUDA events and the medians are printed, with kernel launches and D2H bytes per 
 
 gain: for each noise sigma, a capture with T1 and S1 emitters whose chips are all sent right (no data_flips), decoded
 at e_max 1, 2 and 3: the telegrams sent, those decoded CRC-ok by either algorithm, those recovered only by repair, and
-the wrong repairs (a REPAIRED datagram that was never sent).  The counts are exact: the GPU and the CPU build agree."""
+the wrong repairs (a REPAIRED datagram that was never sent).  The counts are exact: the GPU and the CPU build agree.
+
+gain-soft: the same sweep with one C1A (L = 0x29) and one C1B (L = 0x7F: a full 128-byte block) emitter, no planted
+errors, at k_max 1 .. 6: the C1 telegrams recovered only by the soft repair, and the wrong repairs, split by frame
+format (frame B's 128-byte block has code words of weight 2, DESIGN.md section 8)."""
 import importlib
 import os
 import subprocess
@@ -49,6 +54,7 @@ def cost(steps):
         # contexts agree without repair
         ctxs = {"off": pkg.WmbusB200("-p S", lib=lib, max_batch_mib=1024, **rx),
                 "e_max 3": pkg.WmbusB200("-p S", lib=lib, max_batch_mib=1024, repair=3, **rx),
+                "e3 k6": pkg.WmbusB200("-p S", lib=lib, max_batch_mib=1024, repair=3, repair_soft=6, **rx),
                 "off (2)": pkg.WmbusB200("-p S", lib=lib, max_batch_mib=1024, **rx)}
         times = {k: [] for k in ctxs}
         out = {}
@@ -112,10 +118,46 @@ def gain(cpu, mib):
               f"{row[7]:6d}")
 
 
+def gain_soft(cpu, mib):
+    if cpu:
+        from conftest import HOSTSIM_SO
+        lib = pkg.load_library(HOSTSIM_SO)
+    else:
+        import torch
+        lib = pkg.load_library()
+        print(f"device: {torch.cuda.get_device_name()}  power limit: {power_limit()}")
+    ems = [synth.Emitter("C1A", 0x20338739, amp=90.0, offset_hz=-5e3, l_field=0x29, period_s=0.10, start_s=0.004, seed=33),
+           synth.Emitter("C1B", 0x20210116, amp=90.0, offset_hz=4e3, l_field=0x7F, period_s=0.10, start_s=0.054, seed=34)]
+    print(f"{mib} MiB of 1.6 MS/s cu8 per sigma, one C1A (L = 0x29) and one C1B (L = 0x7F) emitter at amplitude 90, -v, "
+          f"e_max 1, {'CPU build' if cpu else 'GPU'}")
+    print("sigma  sent  crc_ok  " + "  ".join(f"+k{k}" for k in range(1, 7)) + "   wrong A/B at k 1..6")
+    for sigma in SIGMAS:
+        cu8, plan = synth.synth_capture(mib << 20, emitters=ems, seed=0xB2000200 + int(sigma), noise_sigma=sigma)
+        cu8 = np.ascontiguousarray(cu8.numpy())
+        sent = {ems[p.emitter].payload(p.k) for p in plan}
+        ok, gained, wrong = None, [], []
+        for k in range(1, 7):
+            with pkg.WmbusB200("-v", lib=lib, repair=1, repair_soft=k, max_batch_mib=min(mib, 1024)) as ctx:
+                lines = ctx.process(cu8.ctypes.data, len(cu8), flush=True)
+                recs = ctx.take_repairs()
+            if ok is None:
+                ok = {bytes.fromhex(l.split(";")[8][2:]) for l in lines if l.split(";")[2] == "1"} & sent
+            rep = {bytes(r.line.datagram[:r.line.len]) for r in recs
+                   if r.repair.outcome == 1 and bytes(r.line.mode[:2]) == b"C1"}
+            gained.append(len((rep & sent) - ok))
+            bad = rep - sent
+            nb = sum(1 for d in bad if len(d) > 1 and d[0] >= 0x7F - 8)           # by L: the C1B emitter's telegrams
+            wrong.append(f"{len(bad) - nb}/{nb}")
+        print(f"{sigma:5.1f}  {len(plan):4d}  {len(ok):6d}  " + "  ".join(f"{g:3d}" for g in gained) + "   " + " ".join(wrong))
+
+
 if __name__ == "__main__":
     what = sys.argv[1] if len(sys.argv) > 1 else "cost"
     if what == "cost":
         cost(int(sys.argv[2]) if len(sys.argv) > 2 else 8)
+    elif what == "gain-soft":
+        rest = [a for a in sys.argv[2:] if a != "--cpu"]
+        gain_soft("--cpu" in sys.argv[2:], int(rest[0]) if rest else 16)
     elif what == "gain":
         rest = [a for a in sys.argv[2:] if a != "--cpu"]
         gain("--cpu" in sys.argv[2:], int(rest[0]) if rest else 32)
