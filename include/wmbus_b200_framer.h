@@ -14,7 +14,8 @@
  * wmb_frame_decode_device() lets a test compare the two candidate by candidate.  wmb_frame_repair() repairs T1 / S1
  * candidates that lost a few chips (erasure decoding checked by the block CRCs), with the device twin
  * wmb_frame_repair_device(); wmb_frame_repair_soft() / wmb_frame_repair_soft_device() also repair C1 candidates from the
- * soft values of their bits (wmb_set_soft_bits, wmb_frame_soft).
+ * soft values of their bits (wmb_set_soft_bits, wmb_frame_soft), and wmb_frame_repair_t1_soft() /
+ * wmb_frame_repair_t1_soft_device() the T1 candidates that erasure repair gives up on.
  */
 #ifndef WMBUS_B200_FRAMER_H
 #define WMBUS_B200_FRAMER_H
@@ -107,7 +108,8 @@ typedef struct wmb_repair_record {
     uint64_t     sync_sample;   /* access-code match (decimated sample)                 */
     uint64_t     end_sample;    /* decimated sample of bit P - 1 (a C1 line: its last bit) */
     uint8_t      chain, algo;   /* WMB_CHAIN_*, WMB_ALGO_*                              */
-    uint8_t      reserved[6];
+    uint8_t      soft_t1;       /* 1: the T1 soft rule (wmb_set_repair_t1_soft) decided this record */
+    uint8_t      reserved[5];
     wmb_repaired repair;        /* outcome; REPAIRED: the repaired line                 */
 } wmb_repair_record;
 
@@ -173,6 +175,49 @@ int wmb_frame_repair_soft_device(wmb_ctx *ctx, const wmb_frame *frames, const in
  * UNREPAIRABLE; their record's end_sample is bit P - 1, the line's last bit, as before.  T1 and S1 candidates are
  * unchanged.  wmb_boundary_state appends k_max when it is not 0. */
 int wmb_set_repair_soft(wmb_ctx *ctx, uint32_t k_max);
+
+/* ---- T1 soft repair of one candidate --------------------------------------------------------------------------------
+ * The erasure rule gives up on a T1 block with more than e_max invalid symbols, on a symbol with no code word at distance
+ * 1, and on two wrong chips that made another valid code word.  The soft values decide all three.  T1 frame layout (as
+ * K4 reads it): bit 0 the flagged bit, byte l at bits [1 + 12 l, 13 + 12 l), its high-nibble symbol first, a symbol's
+ * first chip the MSB of its 6-bit word; len = wmb_tlg_len_a(L), P = 1 + 12 len; frame format A.  With s_max in
+ * 1..WMB_SOFT_K_MAX:
+ *   1. Candidates: a T1 frame whose decode is a line with crc_ok = 0 and len >= 12, whose bit list reaches P, with no bit
+ *      before P - 1 of rssi < 5 (a line implies both), with soft values, and for which wmb_frame_repair(f, e_max) ends
+ *      in TOO_MANY or UNREPAIRABLE.  The erasure rule runs first and its REPAIRED, AMBIGUOUS, TRUNCATED and NONE stand,
+ *      so the repairs with this rule on are a superset of those without it.  The L byte (bits [1, 13)) never changes.
+ *   2. Centring: over the chips [13, P) with a value, n1 and S1 are the count and the sum of v of the chips decided 1,
+ *      n0 and S0 those of the chips decided 0.  y_j = v_j 2 n0 n1 - (S1 n0 + S0 n1) in int64 (K4S's C1 centring); if
+ *      n0 n1 = 0, y_j = v_j; a chip without a value has y_j = 0.
+ *   3. Symbols: code word w (one of the 16) scores C(w) = sum over the symbol's six chips of (2 w_j - 1) y_j.  ML is
+ *      the argmax of C (ties: the lower nibble), the runner-up the argmax over the other 15 (same ties), and
+ *      delta = C(ML) - C(runner-up) >= 0.  A symbol with a chip without a value ranks before every symbol without one.
+ *   4. Blocks: frame A's (12 bytes, then 18).  A block that passes as received (every symbol valid, CRC passes) is left
+ *      alone.  In a failing block every searchable symbol takes its ML value and the K = min(s_max, searchable symbols)
+ *      of lowest delta (ties: lower symbol index) are searched; the first block's searchable symbols are those of bytes
+ *      1..11.  Exactly one of the 2^K patterns must pass the block's CRC: pattern 0 is pure ML, set bit u replaces
+ *      searched symbol u's ML value by its runner-up.  In block order, the first block where none does makes the frame
+ *      UNREPAIRABLE, where two or more do AMBIGUOUS.
+ *   5. REPAIRED: every block passes.  `line` is the line the reference would print for the corrected bytes (crc_ok =
+ *      ok_3of6 = 1, CRC-stripped datagram, consumed = P, end_sample = bit P - 1, packet_rssi / current_rssi at bits 1 and
+ *      P - 1); erasures = the symbols whose nibble differs from the hard decode (an invalid symbol differs; at most
+ *      255 are counted), blocks = the blocks changed, had_line = 1.
+ * When the rule ran, its outcome replaces the erasure rule's.  Any other frame, s_max = 0 or soft = NULL is repaired
+ * exactly as wmb_frame_repair(f, e_max) does.  All magnitudes fit int64: |y| < 2^39, |C| < 2^42.  Why a wrong repair
+ * stays rare: DESIGN.md section 8. */
+int wmb_frame_repair_t1_soft(const wmb_frame *f, const int16_t *soft, uint32_t e_max, uint32_t s_max, wmb_repaired *out);
+
+/* The same done on the device (K4, the erasure repair K4R, then K4S with k_max = 0), n frames at once; softs[i] is frame
+ * i's soft values (NULL: none). */
+int wmb_frame_repair_t1_soft_device(wmb_ctx *ctx, const wmb_frame *frames, const int16_t *const *softs, size_t n,
+                                    uint32_t e_max, uint32_t s_max, wmb_repaired *out);
+
+/* T1 soft repair on the streaming path.  wmb_set_repair_t1_soft(ctx, s_max), s_max 0 (off, the default) ..
+ * WMB_SOFT_K_MAX, else WMB_E_INVAL; WMB_E_INVAL on a manual_frames context; the state rules of wmb_set_repair_soft, the
+ * setting survives wmb_reset / wmb_seek and is independent of it.  While wmb_set_repair has repair on, the T1 candidates
+ * of the streaming repair follow the rule above with the soft values the gather computes; a record the rule decided has
+ * soft_t1 = 1.  Records become final at bit P - 1, as before.  wmb_boundary_state appends s_max when it is not 0. */
+int wmb_set_repair_t1_soft(wmb_ctx *ctx, uint32_t s_max);
 
 /* CRC-16, polynomial 0x3D65, complemented (t1_c1_packet_decoder.h:463-469) */
 uint16_t wmb_crc16(const uint8_t *data, size_t n);

@@ -45,7 +45,7 @@ REP_NONE, REP_REPAIRED, REP_AMBIGUOUS, REP_TOO_MANY, REP_UNREPAIRABLE, REP_TRUNC
 class WmbRepairRecord(C.Structure):
     """wmb_repair_record (include/wmbus_b200_framer.h): the repair of one candidate of the streaming framer"""
     _fields_ = [("sync_sample", C.c_uint64), ("end_sample", C.c_uint64), ("chain", C.c_uint8), ("algo", C.c_uint8),
-                ("reserved", C.c_uint8 * 6), ("repair", WmbRepaired)]
+                ("soft_t1", C.c_uint8), ("reserved", C.c_uint8 * 5), ("repair", WmbRepaired)]
 
     @property
     def line(self):
@@ -186,6 +186,10 @@ def _bind(lib):
     lib.wmb_take_repairs.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
     lib.wmb_set_soft_bits.argtypes = [C.c_void_p, C.c_int]
     lib.wmb_set_repair_soft.argtypes = [C.c_void_p, C.c_uint32]
+    lib.wmb_set_repair_t1_soft.argtypes = [C.c_void_p, C.c_uint32]
+    lib.wmb_frame_repair_t1_soft.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p]
+    lib.wmb_frame_repair_t1_soft_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint32,
+                                                    C.c_uint32, C.c_void_p]
     lib.wmb_frame_soft.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.POINTER(C.c_int16))]
     lib.wmb_frame_repair_soft.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p]
     lib.wmb_frame_repair_soft_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint32, C.c_uint32,
@@ -253,11 +257,14 @@ class WmbusB200:
     it survives reset() and seek().  take_repairs() hands out its records.
     repair_soft=k_max (1..6): with repair on, the C1 candidates are repaired from the soft values of their bits, see
     wmb_set_repair_soft() (0: off, the default); it survives reset() and seek().
+    repair_t1_soft=s_max (1..6): with repair on, the T1 candidates that erasure repair gives up on are repaired from the
+    soft values of their chips, see wmb_set_repair_t1_soft() (0: off, the default); it survives reset() and seek().
     soft_bits=True (manual_frames=1 only): the soft value of every T1/C1 bit, see wmb_set_soft_bits() (off by default); it
     survives reset() and seek().  frame_soft() returns a polled frame's values and repair_frames(k_max=...) uses them."""
 
     def __init__(self, flags: str = "", device: int = 0, lib=None, clock_lock=None, access_code_errors=None,
-                 burst_level=None, spectrum=None, quality=False, repair=0, repair_soft=0, soft_bits=False, **tuning):
+                 burst_level=None, spectrum=None, quality=False, repair=0, repair_soft=0, soft_bits=False,
+                 repair_t1_soft=0, **tuning):
         self.lib = lib or load_library()
         self.opts = opts_from_flags(self.lib, flags, **tuning)
         self._ctx = C.c_void_p()
@@ -302,6 +309,12 @@ class WmbusB200:
         if repair_soft:
             try:
                 self.set_repair_soft(repair_soft)
+            except Exception:
+                self.close()
+                raise
+        if repair_t1_soft:
+            try:
+                self.set_repair_t1_soft(repair_t1_soft)
             except Exception:
                 self.close()
                 raise
@@ -408,26 +421,30 @@ class WmbusB200:
     def decode_frames(self, arr, n):
         self._check(self.lib.wmb_decode_frames(self._ctx, arr, n))
 
-    def repair_frames(self, arr, n, e_max=2, device=True, k_max=0, soft=None):
+    def repair_frames(self, arr, n, e_max=2, device=True, k_max=0, soft=None, s_max=0):
         """Erasure repair (wmb_frame_repair_device, or the host twin wmb_frame_repair with device=False) of the first n
         frames of arr, e.g. what poll() returned with manual_frames=1.  Returns an array of n WmbRepaired; lines of the
         repaired ones format with repaired_line().
         k_max (1..6): C1 soft repair too (wmb_frame_repair_soft_device / wmb_frame_repair_soft), with soft[i] the int16
-        soft values of frame i (None: none); soft=None takes frame_soft() of every frame."""
+        soft values of frame i (None: none); soft=None takes frame_soft() of every frame.
+        s_max (1..6): T1 soft repair instead (wmb_frame_repair_t1_soft_device / wmb_frame_repair_t1_soft), with the same
+        soft; k_max and s_max cannot both be given."""
         out = (WmbRepaired * max(n, 1))()
-        if k_max:
+        if k_max and s_max:
+            raise ValueError("repair_frames: k_max (C1) and s_max (T1) are separate rules; give one of them")
+        if k_max or s_max:
             import numpy as np
             if soft is None:
                 soft = [self.frame_soft(arr[i]) for i in range(n)]
             soft = [None if v is None else np.ascontiguousarray(v, np.int16) for v in soft]
             ptrs = (C.c_void_p * max(n, 1))(*[None if v is None else v.ctypes.data for v in soft[:n]])
+            dev, host = ((self.lib.wmb_frame_repair_soft_device, self.lib.wmb_frame_repair_soft) if k_max else
+                         (self.lib.wmb_frame_repair_t1_soft_device, self.lib.wmb_frame_repair_t1_soft))
             if device:
-                self._check(self.lib.wmb_frame_repair_soft_device(self._ctx, C.addressof(arr), ptrs, n, e_max, k_max,
-                                                                  C.addressof(out)))
+                self._check(dev(self._ctx, C.addressof(arr), ptrs, n, e_max, k_max or s_max, C.addressof(out)))
             else:
                 for i in range(n):
-                    self._check(self.lib.wmb_frame_repair_soft(C.addressof(arr[i]), ptrs[i], e_max, k_max,
-                                                               C.addressof(out[i])))
+                    self._check(host(C.addressof(arr[i]), ptrs[i], e_max, k_max or s_max, C.addressof(out[i])))
             return out
         if device:
             self._check(self.lib.wmb_frame_repair_device(self._ctx, C.addressof(arr), n, e_max, C.addressof(out)))
@@ -534,6 +551,11 @@ class WmbusB200:
         """C1 soft repair of the streaming framer's candidates, k_max 1..6 (0 = off; before the first push, or after reset()
         / seek()); it acts while set_repair() has repair on"""
         self._check(self.lib.wmb_set_repair_soft(self._ctx, k_max))
+
+    def set_repair_t1_soft(self, s_max: int):
+        """T1 soft repair of the streaming framer's candidates, s_max 1..6 (0 = off; before the first push, or after
+        reset() / seek()); it acts while set_repair() has repair on"""
+        self._check(self.lib.wmb_set_repair_t1_soft(self._ctx, s_max))
 
     def set_soft_bits(self, on: bool):
         """soft values of the T1/C1 bits (before the first push, or after reset() / seek())"""

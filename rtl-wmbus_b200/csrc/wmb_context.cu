@@ -286,6 +286,7 @@ struct wmb_ctx {
      * wmb_reset).  Off: nothing is allocated or launched */
     bool soft = false;
     uint32_t repair_k = 0;                           /* wmb_set_repair_soft: k_max of the C1 soft repair K4S (0: off) */
+    uint32_t repair_s = 0;                           /* wmb_set_repair_t1_soft: s_max of the T1 soft repair K4S (0: off) */
     int16_t *d_soft_words = nullptr, *h_soft_words = nullptr;    /* parallel to d_words / h_words */
 
     /* band survey (wmb_set_spectrum; the setting survives wmb_reset).  Bins 0: off, nothing is allocated or launched */
@@ -1737,7 +1738,7 @@ static int enqueue_gather(wmb_ctx *c, bool final, bool after_batch)
     if (bursts) TRY(burst_alloc(c));
     if (quality) TRY(qual_alloc(c));
     const bool repair = c->repair_e && !c->manual;
-    const bool repair_soft = repair && c->repair_k;          /* C1 candidates: K4S behind K4R, on the soft values */
+    const bool repair_soft = repair && (c->repair_k || c->repair_s);     /* C1 / T1 candidates: K4S behind K4R */
     const bool soft = c->soft || repair_soft;
     if (repair && !c->rep.d) TRY(c->rep.alloc(c, 1, c->hdr.cap, c->hdr.prefix, 256));     /* first gather with repair on */
     if (soft) TRY(soft_alloc(c));
@@ -1780,7 +1781,8 @@ static int enqueue_gather(wmb_ctx *c, bool final, bool after_batch)
         K4SParams sp;
         memset(&sp, 0, sizeof(sp));
         sp.hdr = r.hdr; sp.dec = r.dec; sp.words = r.words; sp.soft = c->d_soft_words; sp.rep = r.rep; sp.pool = r.pool;
-        sp.pool_cap = r.pool_cap; sp.pool_n = r.pool_n; sp.errors = r.errors; sp.k_max = c->repair_k; sp.gd = r.gd;
+        sp.pool_cap = r.pool_cap; sp.pool_n = r.pool_n; sp.errors = r.errors; sp.k_max = c->repair_k; sp.s_max = c->repair_s;
+        sp.gd = r.gd;
         TRY(launch_k3_k4(c, p, c->manual ? nullptr : &q, repair ? &r : nullptr, repair_soft ? &sp : nullptr));
         /* results -> pinned host mirror: the record and a prefix of the arrays it describes (the rest, if a batch ever
          * produces more, is fetched when the record has been read) */
@@ -2310,7 +2312,7 @@ static void repaired_from(const RepHdr &h, uint64_t sync_sample, int mode, const
 {
     static const char modes[3][3] = { "T1", "C1", "S1" };
     memset(&o, 0, sizeof(o));
-    o.outcome = h.outcome; o.had_line = h.had_line;
+    o.outcome = h.outcome; o.had_line = h.had_line & 1u;             /* bit 1: K4S's T1 soft rule decided */
     if (h.outcome != K4R_REPAIRED) return;
     o.erasures = h.erasures; o.blocks = h.blocks;
     wmb_decoded &d = o.line;
@@ -2337,7 +2339,7 @@ static void book_repairs(wmb_ctx *c, const FrameHdr *hdr, const DecHdr *dec, con
         wmb_repair_record r;
         memset(&r, 0, sizeof(r));
         r.sync_sample = hdr[i].sync_sample; r.end_sample = hdr[i].sync_sample + h.end_off;
-        r.chain = hdr[i].chain; r.algo = hdr[i].algo;
+        r.chain = hdr[i].chain; r.algo = hdr[i].algo; r.soft_t1 = (uint8_t)(h.had_line >> 1);
         repaired_from(h, hdr[i].sync_sample, rep_mode(hdr[i].chain, dec[i]), pool, r.repair);
         fresh.push_back(r);
     };
@@ -2514,14 +2516,11 @@ static int launch_k4s(wmb_ctx *c, const K4SParams &p)
     return WMB_OK;
 }
 
-/* Test hook (wmbus_b200_framer.h): K4, the erasure repair K4R and the C1 soft repair K4S on caller-made frames, to compare
- * with the host twin wmb_frame_repair_soft() frame by frame. */
-extern "C" int wmb_frame_repair_soft_device(wmb_ctx *c, const wmb_frame *frames, const int16_t *const *softs, size_t n,
-                                            uint32_t e_max, uint32_t k_max, wmb_repaired *out)
+/* K4, the erasure repair K4R and the soft repair K4S (C1 with k_max, T1 with s_max, one of them non-zero) on caller-made
+ * frames */
+static int repair_soft_device(wmb_ctx *c, const wmb_frame *frames, const int16_t *const *softs, size_t n, uint32_t e_max,
+                              uint32_t k_max, uint32_t s_max, wmb_repaired *out)
 {
-    if (!c || !frames || !out || (!softs && n)) return set_err(WMB_E_INVAL, "null argument");
-    if (k_max > WMB_SOFT_K_MAX) return set_err(WMB_E_INVAL, "k_max %u out of range 0..%d", k_max, WMB_SOFT_K_MAX);
-    if (k_max == 0) return wmb_frame_repair_device(c, frames, n, e_max, out);
     if (e_max > K4R_MAX_ERASURES) return set_err(WMB_E_INVAL, "e_max %u out of range 0..%d", e_max, K4R_MAX_ERASURES);
     memset(out, 0, n * sizeof(*out));
     if (n == 0) return WMB_OK;
@@ -2554,6 +2553,7 @@ extern "C" int wmb_frame_repair_soft_device(wmb_ctx *c, const wmb_frame *frames,
     memset(&s, 0, sizeof(s));
     s.hdr = r.hdr; s.dec = r.dec; s.n = r.n; s.words = r.words; s.soft = d_soft; s.soft_ok = d_ok; s.rep = d_rep;
     s.pool = r.pool; s.pool_cap = r.pool_cap; s.pool_n = r.pool_n; s.errors = r.errors; s.k_max = k_max;
+    s.s_max = s_max;
     TRY(launch_k4s(c, s));
     std::vector<RepHdr> rep(n);
     CUDA_TRY(cudaMemcpyAsync(rep.data(), d_rep, n * sizeof(RepHdr), cudaMemcpyDeviceToHost, c->cs));
@@ -2568,6 +2568,26 @@ extern "C" int wmb_frame_repair_soft_device(wmb_ctx *c, const wmb_frame *frames,
         repaired_from(h, frames[i].sync_sample, rep_mode(frames[i].chain, c->dec.h[i]), c->pool.h, out[i]);
     }
     return WMB_OK;
+}
+
+/* Test hooks (wmbus_b200_framer.h): to compare with the host twins wmb_frame_repair_soft() / wmb_frame_repair_t1_soft()
+ * frame by frame. */
+extern "C" int wmb_frame_repair_soft_device(wmb_ctx *c, const wmb_frame *frames, const int16_t *const *softs, size_t n,
+                                            uint32_t e_max, uint32_t k_max, wmb_repaired *out)
+{
+    if (!c || !frames || !out || (!softs && n)) return set_err(WMB_E_INVAL, "null argument");
+    if (k_max > WMB_SOFT_K_MAX) return set_err(WMB_E_INVAL, "k_max %u out of range 0..%d", k_max, WMB_SOFT_K_MAX);
+    if (k_max == 0) return wmb_frame_repair_device(c, frames, n, e_max, out);
+    return repair_soft_device(c, frames, softs, n, e_max, k_max, 0, out);
+}
+
+extern "C" int wmb_frame_repair_t1_soft_device(wmb_ctx *c, const wmb_frame *frames, const int16_t *const *softs, size_t n,
+                                               uint32_t e_max, uint32_t s_max, wmb_repaired *out)
+{
+    if (!c || !frames || !out || (!softs && n)) return set_err(WMB_E_INVAL, "null argument");
+    if (s_max > WMB_SOFT_K_MAX) return set_err(WMB_E_INVAL, "s_max %u out of range 0..%d", s_max, WMB_SOFT_K_MAX);
+    if (s_max == 0) return wmb_frame_repair_device(c, frames, n, e_max, out);
+    return repair_soft_device(c, frames, softs, n, e_max, 0, s_max, out);
 }
 
 extern "C" int wmb_decode_frames(wmb_ctx *c, const wmb_frame *frames, size_t n)
@@ -2894,6 +2914,17 @@ extern "C" int wmb_set_repair_soft(wmb_ctx *c, uint32_t k_max)
     return WMB_OK;
 }
 
+extern "C" int wmb_set_repair_t1_soft(wmb_ctx *c, uint32_t s_max)
+{
+    if (!c) return set_err(WMB_E_INVAL, "null argument");
+    if (c->manual) return set_err(WMB_E_INVAL, "wmb_set_repair_t1_soft on a manual_frames context (repair the polled frames with wmb_frame_repair_t1_soft_device)");
+    if (s_max > WMB_SOFT_K_MAX) return set_err(WMB_E_INVAL, "s_max %u out of range 0 (off) .. %d", s_max, WMB_SOFT_K_MAX);
+    if (c->batch_no != 0 || !c->remainder.empty())
+        return set_err(WMB_E_STATE, "wmb_set_repair_t1_soft after samples were pushed (call it before the first push or after wmb_reset / wmb_seek)");
+    c->repair_s = s_max;
+    return WMB_OK;
+}
+
 extern "C" int wmb_frame_soft(wmb_ctx *c, const wmb_frame *f, const int16_t **soft)
 {
     if (!c || !f || !soft) return set_err(WMB_E_INVAL, "null argument");
@@ -3040,6 +3071,7 @@ extern "C" long wmb_boundary_state(wmb_ctx *c, uint8_t *buf, size_t cap)
     }
     if (c->repair_e) put(&c->repair_e, 4);             /* contexts that repair differently never agree */
     if (c->repair_k) put(&c->repair_k, 4);
+    if (c->repair_s) { const uint8_t tag = 'T'; put(&tag, 1); put(&c->repair_s, 4); }   /* never reads as a k_max */
     if (out.size() > cap) return set_err(WMB_E_INVAL, "buffer too small (%zu bytes needed)", out.size());
     memcpy(buf, out.data(), out.size());
     return (long)out.size();

@@ -478,6 +478,100 @@ int wmb_frame_repair_soft(const wmb_frame *f, const int16_t *soft, uint32_t e_ma
     return wmb_frame_repair(f, e_max, out);
 }
 
+/* ---- T1 soft repair (definition in wmbus_b200_framer.h; device twin: K4S, wmb_kernels.cuh) ------------------------ */
+
+static void repair_soft_t1(const wmb_frame *f, const int16_t *soft, uint32_t s_max, wmb_repaired *out)
+{
+    const wmb_bit *b = f->bits;
+    const unsigned L = (nibble_3of6(bits_at(b, 1, 6)) << 4) | nibble_3of6(bits_at(b, 7, 6));
+    const unsigned len = wmb_tlg_length_format_a(L), P = 1 + 12 * len, nsym = 2 * len;
+    int64_t n0 = 0, n1 = 0, s0 = 0, s1 = 0;
+    for (unsigned j = 13; j < P; j++) {
+        if (soft[j] == WMB_SOFT_NONE) continue;
+        if (WMB_BIT_DATA(b[j])) { n1++; s1 += soft[j]; } else { n0++; s0 += soft[j]; }
+    }
+    /* per symbol i (byte i / 2, the high nibble first): hard nibble (0xFF invalid), ML, runner-up, delta, has values */
+    static __thread uint8_t hard[2 * 292], ml[2 * 292], ru[2 * 292];
+    static __thread int64_t delta[2 * 292];
+    static __thread int has[2 * 292];
+    for (unsigned i = 2; i < nsym; i++) {
+        int64_t y[6];
+        has[i] = 1;
+        for (unsigned c = 0; c < 6; c++) {
+            const unsigned j = 1 + 6 * i + c;
+            const int64_t v = soft[j];
+            if (soft[j] == WMB_SOFT_NONE) { has[i] = 0; y[c] = 0; }
+            else y[c] = n0 * n1 == 0 ? v : v * 2 * n0 * n1 - (s1 * n0 + s0 * n1);
+        }
+        uint32_t m, r;
+        wmb_t1_sym_ml(y, &m, &r, &delta[i]);
+        ml[i] = (uint8_t)m; ru[i] = (uint8_t)r;
+        hard[i] = nibble_3of6(bits_at(b, 1 + 6 * i, 6));
+    }
+
+    uint8_t pkt[292];
+    memset(pkt, 0, sizeof(pkt));
+    pkt[0] = (uint8_t)L;
+    for (unsigned l = 1; l < len; l++) pkt[l] = (uint8_t)(((hard[2 * l] & 15u) << 4) | (hard[2 * l + 1] & 15u));
+    unsigned changed = 0, blocks = 0;
+    for (unsigned k = 0; k < wmb_nblk_a(len); k++) {
+        const unsigned off = wmb_blk_off_a(k), blk = wmb_blk_len_a(len, k);
+        const unsigned lo = 2 * (off ? off : 1), hi = 2 * (off + blk);    /* the block's searchable symbols */
+        int valid = 1;
+        for (unsigned i = lo; i < hi; i++) valid &= hard[i] != 0xFFu;
+        if (valid && block_ok(pkt + off, blk)) continue;
+        for (unsigned i = lo; i < hi; i++) pkt[i / 2] = (uint8_t)(i & 1u ? (pkt[i / 2] & 0xF0u) | ml[i] : (pkt[i / 2] & 0x0Fu) | ml[i] << 4);
+        /* the K symbols of lowest delta, by selection (a symbol with a chip without a value first, ties: lower index) */
+        const unsigned K = s_max < hi - lo ? s_max : hi - lo;
+        unsigned sel[WMB_SOFT_K_MAX];
+        for (unsigned t = 0; t < K; t++) {
+            int found = 0;
+            for (unsigned i = lo; i < hi; i++) {
+                int taken = 0;
+                for (unsigned u = 0; u < t; u++) taken |= sel[u] == i;
+                if (taken) continue;
+                if (!found || soft_before(has[i], delta[i], i, has[sel[t]], delta[sel[t]], sel[t])) { sel[t] = i; found = 1; }
+            }
+        }
+        unsigned pass = 0, first = 0;
+        for (unsigned x = 0; x < (1u << K); x++) {
+            uint8_t q[18];
+            memcpy(q, pkt + off, blk);
+            for (unsigned t = 0; t < K; t++)
+                if (x >> t & 1u) q[sel[t] / 2 - off] ^= (uint8_t)((ml[sel[t]] ^ ru[sel[t]]) << (sel[t] & 1u ? 0 : 4));
+            if (block_ok(q, blk)) { if (!pass) first = x; pass++; }
+        }
+        if (pass != 1) { out->outcome = pass ? WMB_REP_AMBIGUOUS : WMB_REP_UNREPAIRABLE; return; }
+        for (unsigned t = 0; t < K; t++)
+            if (first >> t & 1u) pkt[sel[t] / 2] ^= (uint8_t)((ml[sel[t]] ^ ru[sel[t]]) << (sel[t] & 1u ? 0 : 4));
+        for (unsigned i = lo; i < hi; i++) changed += hard[i] != (i & 1u ? pkt[i / 2] & 15u : pkt[i / 2] >> 4);
+        blocks++;
+    }
+    const cursor c = { f, P - 1, 0 };
+    finish(&c, &out->line, "T1", pkt, len, 0, 0);
+    out->outcome = WMB_REP_REPAIRED;
+    out->erasures = changed < 255 ? changed : 255;         /* the device record's byte */
+    out->blocks = blocks;
+}
+
+int wmb_frame_repair_t1_soft(const wmb_frame *f, const int16_t *soft, uint32_t e_max, uint32_t s_max, wmb_repaired *out)
+{
+    if (s_max > WMB_SOFT_K_MAX || e_max > REP_MAX_ERASURES) { memset(out, 0, sizeof(*out)); return WMB_E_INVAL; }
+    const int rc = wmb_frame_repair(f, e_max, out);
+    if (rc || !s_max || !soft || f->chain != WMB_CHAIN_T1C1) return rc;
+    if (out->outcome != WMB_REP_TOO_MANY && out->outcome != WMB_REP_UNREPAIRABLE) return rc;
+    wmb_decoded d;
+    wmb_frame_decode(f, &d);
+    if (d.status != WMB_DEC_LINE || d.crc_ok || d.mode[0] != 'T') return rc;
+    /* a line reaches P and has no rssi drop before P - 1; len >= 12 is the rule's own */
+    const unsigned L = (nibble_3of6(bits_at(f->bits, 1, 6)) << 4) | nibble_3of6(bits_at(f->bits, 7, 6));
+    if (wmb_tlg_length_format_a(L) < 12) return rc;
+    memset(out, 0, sizeof(*out));
+    out->had_line = 1;
+    repair_soft_t1(f, soft, s_max, out);
+    return WMB_OK;
+}
+
 /* ---- output --------------------------------------------------------------------- */
 
 void wmb_make_time_string(char *ts, size_t n)

@@ -1825,13 +1825,16 @@ WMB_D void k4r_repair(const K4RParams &p, uint32_t f, int tid, int nthr, K4RSmem
 }
 
 /* =========================================================================== */
-/* K4S: soft repair of C1 candidates (definition in wmbus_b200_framer.h, host twin wmb_frame_repair_soft() in
- * wmb_framer.c).  One warp per candidate, behind K4R: it reads K4's verdict from DecHdr and overwrites K4R's RepHdr of a C1
- * line with CRC errors (K4R makes those UNREPAIRABLE); every other record stays as K4R wrote it.  The lanes reduce n0, n1,
- * S0, S1; per failing block they pick the K least reliable bits by K rounds of warp argmin over a key that orders (has a
- * value, r, bit index) -- unique, so the choice does not depend on the lanes -- compute the K single-bit CRC syndromes (the
- * CRC is affine: a pattern's syndrome is the received one XOR its bits' syndromes) and test patterns lane and lane + 32.
- * The passes are summed and the lowest passing pattern kept, whatever the lanes' order. */
+/* K4S: soft repair of C1 and T1 candidates (definitions in wmbus_b200_framer.h, host twins wmb_frame_repair_soft() and
+ * wmb_frame_repair_t1_soft() in wmb_framer.c).  One warp per candidate, behind K4R: it reads K4's verdict from DecHdr and
+ * overwrites K4R's RepHdr of a C1 line with CRC errors (K4R makes those UNREPAIRABLE; k_max) and of a T1 line with CRC
+ * errors that K4R found TOO_MANY or UNREPAIRABLE (s_max; had_line = 3, bit 1 saying the T1 soft rule decided); every
+ * other record stays as K4R wrote it.  The lanes reduce n0, n1, S0, S1 (T1: and score every symbol into shared memory);
+ * per failing block they pick the K least reliable bits (T1: symbols) by K rounds of warp argmin over a key that orders
+ * (has a value, r or delta, index) -- unique, so the choice does not depend on the lanes -- compute the K single-bit CRC
+ * syndromes (T1: of the nibble mask ML ^ runner-up at its byte; the CRC is affine: a pattern's syndrome is the received
+ * one XOR its members' syndromes) and test patterns lane and lane + 32 (T1: pattern 0, pure ML, too).  The passes are
+ * summed and the lowest passing pattern kept, whatever the lanes' order. */
 struct K4SParams {
     const FrameHdr *hdr; const DecHdr *dec; uint32_t n;   /* gd == null: n candidates at hdr / dec / rep (test hook) */
     const uint32_t *words;
@@ -1840,7 +1843,8 @@ struct K4SParams {
     RepHdr *rep;
     uint8_t *pool; uint32_t pool_cap; uint32_t *pool_n;
     uint32_t *errors;
-    uint32_t k_max;                 /* 1..WMB_SOFT_K_MAX */
+    uint32_t k_max;                 /* C1: 1..WMB_SOFT_K_MAX, 0 = C1 lines are left alone    */
+    uint32_t s_max;                 /* T1: 1..WMB_SOFT_K_MAX, 0 = T1 lines are left alone    */
     const GatherDev *gd;
 };
 
@@ -1849,9 +1853,12 @@ WMB_D uint32_t k4s_count(const K4SParams &p) { return p.gd ? p.gd->n : p.n; }
 struct K4SSmem {
     uint8_t  pkt[296];
     uint32_t s0;                    /* the current block's syndrome as received           */
-    uint32_t sel[WMB_SOFT_K_MAX];   /* its K least reliable bits                           */
-    uint32_t delta[WMB_SOFT_K_MAX]; /* their single-bit syndromes                          */
+    uint32_t sel[WMB_SOFT_K_MAX];   /* its K least reliable bits (T1: symbols)             */
+    uint32_t delta[WMB_SOFT_K_MAX]; /* their single-bit (T1: substitution) syndromes       */
     uint32_t data_off;
+    /* T1, per symbol 2 l + s of byte l: hard nibble (0xFF invalid), ML << 4 | runner-up, search key */
+    uint8_t  hard[2 * 296], mr[2 * 296];
+    uint64_t key[2 * 296];
 };
 
 /* warp reductions; the CPU build runs a candidate on one simulated lane, which holds the whole result */
@@ -1892,30 +1899,38 @@ WMB_D void k4s_repair(const K4SParams &p, uint32_t f, int tid, int nthr, K4SSmem
     const uint32_t lb = p.gd ? p.gd->base : 0u;
     const FrameHdr h = p.hdr[lb + f];
     const DecHdr d = p.dec[lb + f];
-    if (h.nbits == 0 || d.status != K4_LINE || d.crc_ok || d.mode != 1) return;
+    if (h.nbits == 0 || d.status != K4_LINE || d.crc_ok) return;
+    /* C1 lines (k_max), and T1 lines whose erasure repair ended in TOO_MANY or UNREPAIRABLE (s_max) */
+    const bool t1 = d.mode == 0;
+    if (t1) {
+        if (!p.s_max) return;
+        const uint32_t prev = p.rep[lb + f].outcome;
+        if (prev != K4R_TOO_MANY && prev != K4R_UNREPAIRABLE) return;
+    } else if (d.mode != 1 || !p.k_max) return;
     if (p.soft_ok && !p.soft_ok[f]) return;
     const uint32_t *b = p.words + h.word_off;
     const int16_t *sv = p.soft + h.word_off;
     RepHdr r;
     r.consumed = 0; r.end_off = 0; r.serial = 0; r.data_off = 0; r.len = 0; r.outcome = K4R_UNREPAIRABLE;
-    r.erasures = 0; r.blocks = 0; r.had_line = 1; r.packet_rssi = 0; r.current_rssi = 0;
-    const bool bframe = k4_bits(b, 1, 12) == 0x543u;
-    const uint32_t L = k4_bits(b, 17, 8);
+    r.erasures = 0; r.blocks = 0; r.had_line = t1 ? 3 : 1; r.packet_rssi = 0; r.current_rssi = 0;
+    const bool bframe = !t1 && k4_bits(b, 1, 12) == 0x543u;
+    const uint32_t L = t1 ? (wmb_dec3of6(k4_bits(b, 1, 6)) << 4) | wmb_dec3of6(k4_bits(b, 7, 6)) : k4_bits(b, 17, 8);
     const uint32_t len = bframe ? 1 + L : wmb_tlg_len_a(L);
-    const uint32_t P = 17 + 8 * len;
+    const uint32_t d0 = t1 ? 13 : 17;                   /* the first chip / bit after the L byte */
+    const uint32_t P = t1 ? 1 + 12 * len : 17 + 8 * len;
     r.consumed = P;
     r.end_off = WMB_BIT_OFFSET(b[P - 1]);
-    if (len < 12) { if (tid == 0) p.rep[lb + f] = r; return; }
+    if (len < 12) { if (tid == 0 && !t1) p.rep[lb + f] = r; return; }     /* T1: not a candidate, K4R's record stands */
 
     int64_t n0 = 0, n1 = 0, s0 = 0, s1 = 0;
-    for (uint32_t j = 17 + (uint32_t)tid; j < P; j += (uint32_t)nthr) {
+    for (uint32_t j = d0 + (uint32_t)tid; j < P; j += (uint32_t)nthr) {
         const int16_t v = sv[j];
         if (v == WMB_SOFT_NONE) continue;
         if (WMB_BIT_DATA(b[j])) { n1++; s1 += v; } else { n0++; s0 += v; }
     }
     n0 = k4s_sum(n0); n1 = k4s_sum(n1); s0 = k4s_sum(s0); s1 = k4s_sum(s1);
     const int64_t a = 2 * n0 * n1, t = s1 * n0 + s0 * n1;
-    /* search key of bit j: (has a value, r, j) in one integer; |r| < 2^38, j < 2^12 */
+    /* C1 search key of bit j: (has a value, r, j) in one integer; |r| < 2^38, j < 2^12 */
     auto key = [&](uint32_t j) -> uint64_t {
         const int16_t v = sv[j];
         if (v == WMB_SOFT_NONE) return j;
@@ -1923,39 +1938,79 @@ WMB_D void k4s_repair(const K4SParams &p, uint32_t f, int tid, int nthr, K4SSmem
         const int64_t rr = a == 0 ? sign * v : sign * ((int64_t)v * a - t);
         return ((uint64_t)(rr + ((int64_t)1 << 40)) << 12) | j;
     };
-    for (uint32_t l = (uint32_t)tid; l < len; l += (uint32_t)nthr) sm.pkt[l] = (uint8_t)k4_bits(b, 17 + 8 * l, 8);
+    if (t1) {
+        /* per symbol i = 2 l + s: hard nibble, ML | runner-up, and the search key (all chips have values, delta, i);
+         * delta < 2^43, i < 2^10 */
+        for (uint32_t i = 2 + (uint32_t)tid; i < 2 * len; i += (uint32_t)nthr) {
+            int64_t y[6];
+            uint64_t has = 1;
+            for (uint32_t c = 0; c < 6; c++) {
+                const int16_t v = sv[1 + 6 * i + c];
+                if (v == WMB_SOFT_NONE) has = 0;
+                y[c] = v == WMB_SOFT_NONE ? 0 : a == 0 ? (int64_t)v : (int64_t)v * a - t;
+            }
+            uint32_t ml, ru;
+            int64_t delta;
+            wmb_t1_sym_ml(y, &ml, &ru, &delta);
+            sm.hard[i] = (uint8_t)wmb_dec3of6(k4_bits(b, 1 + 6 * i, 6));
+            sm.mr[i] = (uint8_t)(ml << 4 | ru);
+            sm.key[i] = has << 53 | (uint64_t)delta << 10 | i;
+        }
+        for (uint32_t l = (uint32_t)tid; l < len; l += (uint32_t)nthr)
+            sm.pkt[l] = l == 0 ? (uint8_t)L
+                               : (uint8_t)((wmb_dec3of6(k4_bits(b, 1 + 12 * l, 6)) & 15u) << 4 | (wmb_dec3of6(k4_bits(b, 7 + 12 * l, 6)) & 15u));
+    } else
+        for (uint32_t l = (uint32_t)tid; l < len; l += (uint32_t)nthr) sm.pkt[l] = (uint8_t)k4_bits(b, 17 + 8 * l, 8);
     K4_SYNC();
 
     const uint32_t nblk = bframe ? wmb_nblk_b(len) : wmb_nblk_a(len);
+    const uint32_t kk = t1 ? p.s_max : p.k_max;
     uint32_t outcome = K4R_NONE, flips = 0, blocks = 0;
     for (uint32_t k = 0; k < nblk && outcome == K4R_NONE; k++) {
         const uint32_t off = bframe ? wmb_blk_off_b(k) : wmb_blk_off_a(k), blk = bframe ? wmb_blk_len_b(len, k) : wmb_blk_len_a(len, k);
         if (blk < 2) { outcome = K4R_UNREPAIRABLE; break; }          /* no CRC: no pattern can pass */
+        /* the searchable bits (C1) or symbols (T1) of the block */
+        const uint32_t lo = t1 ? 2 * (off ? off : 1) : 17 + 8 * (off ? off : 1), hi = t1 ? 2 * (off + blk) : 17 + 8 * (off + blk);
+        int64_t invalid = 0;
+        if (t1)
+            for (uint32_t i = lo + (uint32_t)tid; i < hi; i += (uint32_t)nthr) invalid += sm.hard[i] == 0xFFu;
+        invalid = k4s_sum(invalid);
         if (tid == 0) sm.s0 = k4_crc16(sm.pkt + off, blk - 2) ^ (((uint32_t)sm.pkt[off + blk - 2] << 8) | sm.pkt[off + blk - 1]);
         K4_SYNC();
-        const uint32_t syn = sm.s0;
+        uint32_t syn = sm.s0;
         K4_SYNC();
-        if (syn == 0) continue;
-        const uint32_t lo = 17 + 8 * (off ? off : 1), hi = 17 + 8 * (off + blk);
-        const uint32_t K = p.k_max < hi - lo ? p.k_max : hi - lo;
+        if (syn == 0 && invalid == 0) continue;
+        if (t1) {                                               /* every searchable symbol takes its ML value */
+            for (uint32_t l = lo / 2 + (uint32_t)tid; l < hi / 2; l += (uint32_t)nthr)
+                sm.pkt[l] = (uint8_t)((sm.mr[2 * l] & 0xF0u) | sm.mr[2 * l + 1] >> 4);
+            K4_SYNC();
+            if (tid == 0) sm.s0 = k4_crc16(sm.pkt + off, blk - 2) ^ (((uint32_t)sm.pkt[off + blk - 2] << 8) | sm.pkt[off + blk - 1]);
+            K4_SYNC();
+            syn = sm.s0;
+        }
+        const uint32_t K = kk < hi - lo ? kk : hi - lo;
         uint64_t prev = 0;
         for (uint32_t u = 0; u < K; u++) {
             uint64_t best = ~0ull;
             for (uint32_t j = lo + (uint32_t)tid; j < hi; j += (uint32_t)nthr) {
-                const uint64_t kj = key(j);
+                const uint64_t kj = t1 ? sm.key[j] : key(j);
                 if (kj > prev && kj < best) best = kj;
             }
             prev = k4s_min(best);
-            if (tid == 0) sm.sel[u] = (uint32_t)(prev & 4095u);
+            if (tid == 0) sm.sel[u] = (uint32_t)(prev & (t1 ? 1023u : 4095u));
         }
         K4_SYNC();
-        for (uint32_t u = (uint32_t)tid; u < K; u += (uint32_t)nthr)
-            sm.delta[u] = k4s_delta((sm.sel[u] - 17) / 8 - off, 0x80u >> ((sm.sel[u] - 17) % 8), blk - 2);
+        /* a T1 substitution is the nibble mask ML ^ runner-up at its byte */
+        for (uint32_t u = (uint32_t)tid; u < K; u += (uint32_t)nthr) {
+            const uint32_t j = sm.sel[u];
+            sm.delta[u] = t1 ? k4s_delta(j / 2 - off, (uint32_t)((sm.mr[j] >> 4) ^ (sm.mr[j] & 15u)) << (j & 1u ? 0 : 4), blk - 2)
+                             : k4s_delta((j - 17) / 8 - off, 0x80u >> ((j - 17) % 8), blk - 2);
+        }
         K4_SYNC();
         int64_t npass = 0;
         uint64_t first = ~0ull;
         for (uint32_t x = (uint32_t)tid; x < 64; x += (uint32_t)nthr) {
-            if (x == 0 || x >= (1u << K)) continue;
+            if ((x == 0 && !t1) || x >= (1u << K)) continue;        /* T1: pattern 0 is pure ML */
             uint32_t s = syn;
             for (uint32_t u = 0; u < K; u++) if (x >> u & 1u) s ^= sm.delta[u];
             if (s == 0) { npass++; if (x < first) first = x; }
@@ -1964,9 +2019,19 @@ WMB_D void k4s_repair(const K4SParams &p, uint32_t f, int tid, int nthr, K4SSmem
         first = k4s_min(first);
         if (npass != 1) { outcome = npass ? K4R_AMBIGUOUS : K4R_UNREPAIRABLE; break; }
         if (tid == 0)
-            for (uint32_t u = 0; u < K; u++)
-                if (first >> u & 1u) sm.pkt[(sm.sel[u] - 17) / 8] ^= (uint8_t)(0x80u >> ((sm.sel[u] - 17) % 8));
-        flips += (uint32_t)wmb_popc((uint32_t)first);
+            for (uint32_t u = 0; u < K; u++) {
+                if (!(first >> u & 1u)) continue;
+                const uint32_t j = sm.sel[u];
+                if (t1) sm.pkt[j / 2] ^= (uint8_t)(((sm.mr[j] >> 4) ^ (sm.mr[j] & 15u)) << (j & 1u ? 0 : 4));
+                else sm.pkt[(j - 17) / 8] ^= (uint8_t)(0x80u >> ((j - 17) % 8));
+            }
+        K4_SYNC();
+        if (t1) {                                               /* the symbols whose nibble differs from the hard decode */
+            int64_t changed = 0;
+            for (uint32_t i = lo + (uint32_t)tid; i < hi; i += (uint32_t)nthr)
+                changed += sm.hard[i] != (i & 1u ? sm.pkt[i / 2] & 15u : sm.pkt[i / 2] >> 4);
+            flips += (uint32_t)k4s_sum(changed);
+        } else flips += (uint32_t)wmb_popc((uint32_t)first);
         blocks++;
         K4_SYNC();
     }
@@ -1999,7 +2064,7 @@ WMB_D void k4s_repair(const K4SParams &p, uint32_t f, int tid, int nthr, K4SSmem
         r.serial = (uint32_t)sm.pkt[4] | ((uint32_t)sm.pkt[5] << 8) | ((uint32_t)sm.pkt[6] << 16) | ((uint32_t)sm.pkt[7] << 24);
         r.data_off = data_off;
         r.len = (uint16_t)(data_off == 0xFFFFFFFFu ? 0 : out_len);
-        r.erasures = (uint8_t)flips; r.blocks = (uint8_t)blocks;
+        r.erasures = (uint8_t)(flips < 255 ? flips : 255); r.blocks = (uint8_t)blocks;
         r.packet_rssi = (uint8_t)WMB_BIT_RSSI(b[1]);
         r.current_rssi = (uint8_t)WMB_BIT_RSSI(b[P - 1]);
         p.rep[lb + f] = r;
