@@ -15,7 +15,8 @@
  * candidates that lost a few chips (erasure decoding checked by the block CRCs), with the device twin
  * wmb_frame_repair_device(); wmb_frame_repair_soft() / wmb_frame_repair_soft_device() also repair C1 candidates from the
  * soft values of their bits (wmb_set_soft_bits, wmb_frame_soft), and wmb_frame_repair_t1_soft() /
- * wmb_frame_repair_t1_soft_device() the T1 candidates that erasure repair gives up on.
+ * wmb_frame_repair_t1_soft_device() the T1 candidates that erasure repair gives up on, and wmb_frame_repair_s1_soft() /
+ * wmb_frame_repair_s1_soft_device() the S1 ones, from the soft values of their chips (wmb_set_soft_bits_s1).
  */
 #ifndef WMBUS_B200_FRAMER_H
 #define WMBUS_B200_FRAMER_H
@@ -109,7 +110,8 @@ typedef struct wmb_repair_record {
     uint64_t     end_sample;    /* decimated sample of bit P - 1 (a C1 line: its last bit) */
     uint8_t      chain, algo;   /* WMB_CHAIN_*, WMB_ALGO_*                              */
     uint8_t      soft_t1;       /* 1: the T1 soft rule (wmb_set_repair_t1_soft) decided this record */
-    uint8_t      reserved[5];
+    uint8_t      soft_s1;       /* 1: the S1 soft rule (wmb_set_repair_s1_soft) decided this record */
+    uint8_t      reserved[4];
     wmb_repaired repair;        /* outcome; REPAIRED: the repaired line                 */
 } wmb_repair_record;
 
@@ -133,7 +135,7 @@ int wmb_take_repairs(wmb_ctx *ctx, wmb_repair_record *out, size_t cap, size_t *n
  * wmb_set_soft_bits(ctx, on) makes the device gather of a manual_frames context compute them (WMB_E_INVAL on any other
  * context: its soft values serve wmb_set_repair_soft below); the setter follows wmb_set_line_quality's state rules and
  * the setting survives wmb_reset / wmb_seek.  wmb_frame_soft() returns them for a frame of the last wmb_poll: parallel to
- * f->bits, valid as long as f->bits; NULL for S1 frames or when soft values are off. */
+ * f->bits, valid as long as f->bits; NULL for S1 frames (unless wmb_set_soft_bits_s1 is on) or when soft values are off. */
 #define WMB_SOFT_NONE  (-32768)
 #define WMB_SOFT_D_T2  2
 #define WMB_SOFT_D_RL  7
@@ -218,6 +220,68 @@ int wmb_frame_repair_t1_soft_device(wmb_ctx *ctx, const wmb_frame *frames, const
  * of the streaming repair follow the rule above with the soft values the gather computes; a record the rule decided has
  * soft_t1 = 1.  Records become final at bit P - 1, as before.  wmb_boundary_state appends s_max when it is not 0. */
 int wmb_set_repair_t1_soft(wmb_ctx *ctx, uint32_t s_max);
+
+/* ---- soft values of the S1 chain's chips --------------------------------------------------------------------------
+ * How sure the slicer was of an S1 chip.  Bit event e of an S1 stream lies at decimated sample m.  Its chip centre is
+ *   t2a:  c = m - WMB_SOFT_S1_D_T2;
+ *   rla:  c = m - WMB_SOFT_S1_D_RL - 24 (n - 1 - i), e being the i-th of the n events that share sample m.  24 is the
+ *         nominal samples per chip (runlength_algorithm_reset_s1); a valid Manchester run is at most 2 chips long, so
+ *         the nominal spacing is off by less than a sample.
+ * v = clamp(floor(sum over q in [c - 8, c + 8) of rint(dphi[q] * 2^24) / 2^WMB_SOFT_S1_SHIFT), -32767, 32767), as an
+ * int16, over the same post-FIR, pre-DC-block dphi as the T1/C1 values.  WMB_SOFT_NONE: the window starts before the
+ * first sample pushed since the last reset / seek, or n - 1 - i > 31 (so the window stays inside the dphi history).
+ * Both windows end at or before the event's own sample, which the event's batch holds: the delays are >= 7.  The delays
+ * maximise the mean of (2 chip - 1) v over clean S1 telegrams (DESIGN.md section 8).
+ * wmb_set_soft_bits_s1(ctx, on) makes the device gather of a manual_frames context compute them (WMB_E_INVAL on any
+ * other context: its S1 values serve wmb_set_repair_s1_soft below), with wmb_set_soft_bits' state rules; the setting
+ * survives wmb_reset / wmb_seek and is independent of wmb_set_soft_bits.  With it on, wmb_frame_soft() returns the values
+ * of S1 frames; with it off (the default) it returns NULL for them. */
+#define WMB_SOFT_S1_D_T2   7
+#define WMB_SOFT_S1_D_RL   13
+#define WMB_SOFT_S1_SHIFT  14
+
+int wmb_set_soft_bits_s1(wmb_ctx *ctx, int on);
+
+/* ---- S1 soft repair of one candidate --------------------------------------------------------------------------------
+ * Manchester sends every bit as one chip on each tone, so d = v(second chip) - v(first chip) decides a bit without an
+ * estimate of the tone means.  S1 frame layout (as K4 reads it): bit 0 the flagged bit, byte l at bits
+ * [1 + 16 l, 17 + 16 l), data bit b of the byte (MSB first) the pair (1 + 16 l + 2 b, 2 + 16 l + 2 b): "01" = 1,
+ * "10" = 0; pair index 8 l + b; len = wmb_tlg_len_a(L), P = 1 + 16 len; frame format A.  With s_max in
+ * 1..WMB_SOFT_K_MAX:
+ *   1. Candidates: an S1 frame whose decode is a line with crc_ok = 0 or an abort on a Manchester violation after the L
+ *      byte, with len >= 12, whose bit list reaches P, with no bit before P - 1 of rssi < 5 (an RSSI abort stays one),
+ *      with soft values, and for which wmb_frame_repair(f, e_max) ends in TOO_MANY or UNREPAIRABLE.  Its REPAIRED,
+ *      AMBIGUOUS, TRUNCATED and NONE stand, so the repairs with this rule on are a superset of those without it.  The L
+ *      byte never changes.
+ *   2. Pairs: d = v2 - v1 in int32 (v1 the first chip's value); a pair with a chip without a value has d = 0 and ranks
+ *      before every pair with values.  The ML bit is 1 if d > 0, 0 if d < 0, and if d = 0 the received bit when the pair
+ *      is valid, else 0.  Its reliability is |d|.
+ *   3. Blocks: frame A's (12 bytes, then 18).  A block without a violation that passes its CRC as received is left
+ *      alone.  In a failing block every searchable pair (all of the block's, but the L byte's in the first block) takes
+ *      its ML bit, and the K = min(s_max, searchable pairs) of lowest key (has a value, |d|, pair index) are searched.
+ *      Exactly one of the 2^K patterns must pass the block's CRC: pattern 0 is pure ML, set bit u flips searched pair
+ *      u.  In block order, the first block where none does makes the frame UNREPAIRABLE, where two or more do
+ *      AMBIGUOUS.
+ *   4. REPAIRED: every block passes.  `line` is the line the reference would print for the corrected bytes (crc_ok =
+ *      ok_3of6 = 1, CRC-stripped datagram, consumed = P, end_sample = bit P - 1, packet_rssi / current_rssi at bits 1 and
+ *      P - 1); erasures = the bits that differ from the hard decode (a violation differs; at most 255 are counted),
+ *      blocks = the blocks changed, had_line = 1 for a line and 0 for an abort.
+ * When the rule ran, its outcome replaces the erasure rule's.  Any other frame, s_max = 0 or soft = NULL is repaired
+ * exactly as wmb_frame_repair(f, e_max) does.  Why a wrong repair stays rare: DESIGN.md section 8. */
+int wmb_frame_repair_s1_soft(const wmb_frame *f, const int16_t *soft, uint32_t e_max, uint32_t s_max, wmb_repaired *out);
+
+/* The same done on the device (K4, the erasure repair K4R, then K4S), n frames at once; softs[i] is frame i's soft values
+ * (NULL: none). */
+int wmb_frame_repair_s1_soft_device(wmb_ctx *ctx, const wmb_frame *frames, const int16_t *const *softs, size_t n,
+                                    uint32_t e_max, uint32_t s_max, wmb_repaired *out);
+
+/* S1 soft repair on the streaming path.  wmb_set_repair_s1_soft(ctx, s_max), s_max 0 (off, the default) ..
+ * WMB_SOFT_K_MAX, else WMB_E_INVAL; WMB_E_INVAL on a manual_frames context; the state rules of wmb_set_repair_t1_soft,
+ * the setting survives wmb_reset / wmb_seek and is independent of the C1 and T1 settings.  While wmb_set_repair has
+ * repair on, the S1 candidates of the streaming repair follow the rule above with the soft values the gather computes; a
+ * record the rule decided has soft_s1 = 1.  Records become final at bit P - 1, as before.  wmb_boundary_state appends a
+ * tag and s_max when s_max is not 0. */
+int wmb_set_repair_s1_soft(wmb_ctx *ctx, uint32_t s_max);
 
 /* CRC-16, polynomial 0x3D65, complemented (t1_c1_packet_decoder.h:463-469) */
 uint16_t wmb_crc16(const uint8_t *data, size_t n);

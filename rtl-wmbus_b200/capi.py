@@ -45,7 +45,7 @@ REP_NONE, REP_REPAIRED, REP_AMBIGUOUS, REP_TOO_MANY, REP_UNREPAIRABLE, REP_TRUNC
 class WmbRepairRecord(C.Structure):
     """wmb_repair_record (include/wmbus_b200_framer.h): the repair of one candidate of the streaming framer"""
     _fields_ = [("sync_sample", C.c_uint64), ("end_sample", C.c_uint64), ("chain", C.c_uint8), ("algo", C.c_uint8),
-                ("soft_t1", C.c_uint8), ("reserved", C.c_uint8 * 5), ("repair", WmbRepaired)]
+                ("soft_t1", C.c_uint8), ("soft_s1", C.c_uint8), ("reserved", C.c_uint8 * 4), ("repair", WmbRepaired)]
 
     @property
     def line(self):
@@ -187,6 +187,11 @@ def _bind(lib):
     lib.wmb_set_soft_bits.argtypes = [C.c_void_p, C.c_int]
     lib.wmb_set_repair_soft.argtypes = [C.c_void_p, C.c_uint32]
     lib.wmb_set_repair_t1_soft.argtypes = [C.c_void_p, C.c_uint32]
+    lib.wmb_set_repair_s1_soft.argtypes = [C.c_void_p, C.c_uint32]
+    lib.wmb_set_soft_bits_s1.argtypes = [C.c_void_p, C.c_int]
+    lib.wmb_frame_repair_s1_soft.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p]
+    lib.wmb_frame_repair_s1_soft_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint32,
+                                                    C.c_uint32, C.c_void_p]
     lib.wmb_frame_repair_t1_soft.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p]
     lib.wmb_frame_repair_t1_soft_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint32,
                                                     C.c_uint32, C.c_void_p]
@@ -259,12 +264,15 @@ class WmbusB200:
     wmb_set_repair_soft() (0: off, the default); it survives reset() and seek().
     repair_t1_soft=s_max (1..6): with repair on, the T1 candidates that erasure repair gives up on are repaired from the
     soft values of their chips, see wmb_set_repair_t1_soft() (0: off, the default); it survives reset() and seek().
+    repair_s1_soft=s_max (1..6): with repair on, the S1 candidates that erasure repair gives up on are repaired from the
+    soft values of their chips, see wmb_set_repair_s1_soft() (0: off, the default); it survives reset() and seek().
     soft_bits=True (manual_frames=1 only): the soft value of every T1/C1 bit, see wmb_set_soft_bits() (off by default); it
-    survives reset() and seek().  frame_soft() returns a polled frame's values and repair_frames(k_max=...) uses them."""
+    survives reset() and seek().  frame_soft() returns a polled frame's values and repair_frames(k_max=...) uses them.
+    soft_bits_s1=True (manual_frames=1 only): the soft value of every S1 chip too, see wmb_set_soft_bits_s1()."""
 
     def __init__(self, flags: str = "", device: int = 0, lib=None, clock_lock=None, access_code_errors=None,
                  burst_level=None, spectrum=None, quality=False, repair=0, repair_soft=0, soft_bits=False,
-                 repair_t1_soft=0, **tuning):
+                 repair_t1_soft=0, repair_s1_soft=0, soft_bits_s1=False, **tuning):
         self.lib = lib or load_library()
         self.opts = opts_from_flags(self.lib, flags, **tuning)
         self._ctx = C.c_void_p()
@@ -315,6 +323,18 @@ class WmbusB200:
         if repair_t1_soft:
             try:
                 self.set_repair_t1_soft(repair_t1_soft)
+            except Exception:
+                self.close()
+                raise
+        if repair_s1_soft:
+            try:
+                self.set_repair_s1_soft(repair_s1_soft)
+            except Exception:
+                self.close()
+                raise
+        if soft_bits_s1:
+            try:
+                self.set_soft_bits_s1(True)
             except Exception:
                 self.close()
                 raise
@@ -421,30 +441,33 @@ class WmbusB200:
     def decode_frames(self, arr, n):
         self._check(self.lib.wmb_decode_frames(self._ctx, arr, n))
 
-    def repair_frames(self, arr, n, e_max=2, device=True, k_max=0, soft=None, s_max=0):
+    def repair_frames(self, arr, n, e_max=2, device=True, k_max=0, soft=None, s_max=0, s1_max=0):
         """Erasure repair (wmb_frame_repair_device, or the host twin wmb_frame_repair with device=False) of the first n
         frames of arr, e.g. what poll() returned with manual_frames=1.  Returns an array of n WmbRepaired; lines of the
         repaired ones format with repaired_line().
         k_max (1..6): C1 soft repair too (wmb_frame_repair_soft_device / wmb_frame_repair_soft), with soft[i] the int16
         soft values of frame i (None: none); soft=None takes frame_soft() of every frame.
         s_max (1..6): T1 soft repair instead (wmb_frame_repair_t1_soft_device / wmb_frame_repair_t1_soft), with the same
-        soft; k_max and s_max cannot both be given."""
+        soft; s1_max (1..6): S1 soft repair instead (wmb_frame_repair_s1_soft_device / wmb_frame_repair_s1_soft).  At most
+        one of k_max, s_max and s1_max can be given."""
         out = (WmbRepaired * max(n, 1))()
-        if k_max and s_max:
-            raise ValueError("repair_frames: k_max (C1) and s_max (T1) are separate rules; give one of them")
-        if k_max or s_max:
+        if sum(1 for x in (k_max, s_max, s1_max) if x) > 1:
+            raise ValueError("repair_frames: k_max (C1), s_max (T1) and s1_max (S1) are separate rules; give one of them")
+        if k_max or s_max or s1_max:
             import numpy as np
             if soft is None:
                 soft = [self.frame_soft(arr[i]) for i in range(n)]
             soft = [None if v is None else np.ascontiguousarray(v, np.int16) for v in soft]
             ptrs = (C.c_void_p * max(n, 1))(*[None if v is None else v.ctypes.data for v in soft[:n]])
             dev, host = ((self.lib.wmb_frame_repair_soft_device, self.lib.wmb_frame_repair_soft) if k_max else
-                         (self.lib.wmb_frame_repair_t1_soft_device, self.lib.wmb_frame_repair_t1_soft))
+                         (self.lib.wmb_frame_repair_t1_soft_device, self.lib.wmb_frame_repair_t1_soft) if s_max else
+                         (self.lib.wmb_frame_repair_s1_soft_device, self.lib.wmb_frame_repair_s1_soft))
+            kk = k_max or s_max or s1_max
             if device:
-                self._check(dev(self._ctx, C.addressof(arr), ptrs, n, e_max, k_max or s_max, C.addressof(out)))
+                self._check(dev(self._ctx, C.addressof(arr), ptrs, n, e_max, kk, C.addressof(out)))
             else:
                 for i in range(n):
-                    self._check(host(C.addressof(arr[i]), ptrs[i], e_max, k_max or s_max, C.addressof(out[i])))
+                    self._check(host(C.addressof(arr[i]), ptrs[i], e_max, kk, C.addressof(out[i])))
             return out
         if device:
             self._check(self.lib.wmb_frame_repair_device(self._ctx, C.addressof(arr), n, e_max, C.addressof(out)))
@@ -557,13 +580,22 @@ class WmbusB200:
         reset() / seek()); it acts while set_repair() has repair on"""
         self._check(self.lib.wmb_set_repair_t1_soft(self._ctx, s_max))
 
+    def set_repair_s1_soft(self, s_max: int):
+        """S1 soft repair of the streaming framer's candidates, s_max 1..6 (0 = off; before the first push, or after
+        reset() / seek()); it acts while set_repair() has repair on"""
+        self._check(self.lib.wmb_set_repair_s1_soft(self._ctx, s_max))
+
+    def set_soft_bits_s1(self, on: bool):
+        """soft values of the S1 chips (manual_frames=1; before the first push, or after reset() / seek())"""
+        self._check(self.lib.wmb_set_soft_bits_s1(self._ctx, int(bool(on))))
+
     def set_soft_bits(self, on: bool):
         """soft values of the T1/C1 bits (before the first push, or after reset() / seek())"""
         self._check(self.lib.wmb_set_soft_bits(self._ctx, int(bool(on))))
 
     def frame_soft(self, frame):
-        """the int16 soft values of a frame of the last poll(), parallel to its bits (a copy); None for S1 frames or
-        when soft values are off"""
+        """the int16 soft values of a frame of the last poll(), parallel to its bits (a copy); None for S1 frames
+        (unless soft_bits_s1 is on) or when soft values are off"""
         import numpy as np
         p = C.POINTER(C.c_int16)()
         self._check(self.lib.wmb_frame_soft(self._ctx, C.addressof(frame), C.byref(p)))

@@ -54,6 +54,11 @@
  *                              symbols of each failing CRC block (wmb_set_repair_t1_soft; DESIGN.md 8).  Unset: T1 is
  *                              repaired from hard decisions only.  A bad value, or this variable without
  *                              WMBUS_B200_REPAIRED, is an error at start-up.  stdout does not change.
+ *   WMBUS_B200_REPAIR_S1_SOFT_BITS=<s>  also repair S1 telegrams that erasure repair gives up on, from the soft values
+ *                              of their chips: maximum-likelihood bits and a search over the s (1..6) least reliable
+ *                              Manchester pairs of each failing CRC block (wmb_set_repair_s1_soft; DESIGN.md 8).  Unset: S1
+ *                              is repaired from hard decisions only.  A bad value, or this variable without
+ *                              WMBUS_B200_REPAIRED, is an error at start-up.  stdout does not change.
  */
 #define _GNU_SOURCE
 #include <errno.h>
@@ -471,6 +476,19 @@ int main(int argc, char *argv[])
             return EXIT_FAILURE;
         }
     }
+    unsigned long repair_s1 = 0;
+    if ((e = getenv("WMBUS_B200_REPAIR_S1_SOFT_BITS")) != NULL) {
+        char *end = NULL;
+        repair_s1 = strtoul(e, &end, 10);
+        if (!getenv("WMBUS_B200_REPAIRED")) {
+            fprintf(stderr, "rtl_wmbus_b200: WMBUS_B200_REPAIR_S1_SOFT_BITS needs WMBUS_B200_REPAIRED\n");
+            return EXIT_FAILURE;
+        }
+        if (e[0] < '0' || e[0] > '9' || *end || repair_s1 < 1 || repair_s1 > WMB_SOFT_K_MAX) {
+            fprintf(stderr, "rtl_wmbus_b200: WMBUS_B200_REPAIR_S1_SOFT_BITS=%s: expected 1 .. %d\n", e, WMB_SOFT_K_MAX);
+            return EXIT_FAILURE;
+        }
+    }
     if ((e = getenv("WMBUS_B200_REPAIRED")) != NULL && (g_rep_file = fopen(e, "w")) == NULL) {
         fprintf(stderr, "rtl_wmbus_b200: WMBUS_B200_REPAIRED=%s: %s\n", e, strerror(errno));
         return EXIT_FAILURE;
@@ -497,7 +515,8 @@ int main(int argc, char *argv[])
         return EXIT_FAILURE;
     }
     if (g_rep_file && (wmb_set_repair(ctx, (uint32_t)repair_e) != WMB_OK || wmb_set_repair_soft(ctx, (uint32_t)repair_k) != WMB_OK ||
-                       wmb_set_repair_t1_soft(ctx, (uint32_t)repair_s) != WMB_OK)) {
+                       wmb_set_repair_t1_soft(ctx, (uint32_t)repair_s) != WMB_OK ||
+                       wmb_set_repair_s1_soft(ctx, (uint32_t)repair_s1) != WMB_OK)) {
         fprintf(stderr, "rtl_wmbus_b200: %s\n", wmb_last_error());
         return EXIT_FAILURE;
     }

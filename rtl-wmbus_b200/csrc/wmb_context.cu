@@ -79,7 +79,7 @@ struct Stream {                     /* one (chain, algo) bit stream */
     uint64_t *pend = nullptr;       /* device: candidates waiting for more bits   */
     OfsAcc *pend_ofs = nullptr;     /* device: their carrier-offset sums          */
     QualAcc *pend_qual = nullptr;   /* device: their quality sums (quality on)    */
-    int16_t *soft_ring = nullptr;   /* device: soft values beside ring (soft values on, T1/C1 only) */
+    int16_t *soft_ring = nullptr;   /* device: soft values beside ring (soft values on; S1: its values on) */
     uint64_t *agg = nullptr;        /* scan scratch [tiles]                       */
     uint64_t total = 0;             /* host mirror of sd->total at the last read  */
     uint64_t total_prev = 0;        /* ... before the last batch read (stage tap) */
@@ -287,6 +287,8 @@ struct wmb_ctx {
     bool soft = false;
     uint32_t repair_k = 0;                           /* wmb_set_repair_soft: k_max of the C1 soft repair K4S (0: off) */
     uint32_t repair_s = 0;                           /* wmb_set_repair_t1_soft: s_max of the T1 soft repair K4S (0: off) */
+    bool soft_s1 = false;                            /* wmb_set_soft_bits_s1 (manual_frames): S1 soft values too */
+    uint32_t repair_s1 = 0;                          /* wmb_set_repair_s1_soft: s_max of the S1 soft repair K4S (0: off) */
     int16_t *d_soft_words = nullptr, *h_soft_words = nullptr;    /* parallel to d_words / h_words */
 
     /* band survey (wmb_set_spectrum; the setting survives wmb_reset).  Bins 0: off, nothing is allocated or launched */
@@ -351,9 +353,13 @@ static int launch_k3_k4(wmb_ctx *c, const K3Params &p, const K4Params *q, const 
      * it writes are the same again) */
     if (p.soft_words) {
         const uint32_t n = p.gd->n;
-        hs_for(n, [&](uint32_t i) { hs_for(4, [&](uint32_t t) { k3_soft(p, i, t, 4); }); });
-        hs_for(n, [&](uint32_t i) { hs_for(4, [&](uint32_t t) { k3_copy(p, i, t, 4); }); });
+        hs_for(n, [&](uint32_t i) { hs_for(4, [&](uint32_t t) { k3_soft<false>(p, i, t, 4); }); });
         c->st.kernel_launches += 1;
+        if (p.soft_ring[WMB_CHAIN_S1 * WMB_N_ALGOS + WMB_ALGO_RLA] || p.soft_ring[WMB_CHAIN_S1 * WMB_N_ALGOS + WMB_ALGO_T2A]) {
+            hs_for(n, [&](uint32_t i) { hs_for(4, [&](uint32_t t) { k3_soft<true>(p, i, t, 4); }); });
+            c->st.kernel_launches += 1;
+        }
+        hs_for(n, [&](uint32_t i) { hs_for(4, [&](uint32_t t) { k3_copy(p, i, t, 4); }); });
     }
     if (!r) return WMB_OK;
     static K4RSmem sm;                  /* the block's phases need real barriers: one simulated thread */
@@ -361,8 +367,14 @@ static int launch_k3_k4(wmb_ctx *c, const K3Params &p, const K4Params *q, const 
     c->st.kernel_launches += 1;
     if (sp) {
         static K4SSmem ss;
-        hs_for(p.gd->n, [&](uint32_t i) { k4s_repair(*sp, i, 0, 1, ss); });
-        c->st.kernel_launches += 1;
+        if (sp->k_max || sp->s_max) {
+            hs_for(p.gd->n, [&](uint32_t i) { k4s_repair<false>(*sp, i, 0, 1, ss); });
+            c->st.kernel_launches += 1;
+        }
+        if (sp->s1_max) {
+            hs_for(p.gd->n, [&](uint32_t i) { k4s_repair<true>(*sp, i, 0, 1, ss); });
+            c->st.kernel_launches += 1;
+        }
     }
     *p.errors |= p.rec->errors & K3_SOFT_ERRORS;
     k3_publish(p);
@@ -568,6 +580,10 @@ static int launch_k3_k4(wmb_ctx *c, const K3Params &p, const K4Params *q, const 
         k3_soft_kernel<<<sms * 32, 64, 0, c->cs>>>(p);
         c->st.kernel_launches += 1;
     }
+    if (p.soft_ring[WMB_CHAIN_S1 * WMB_N_ALGOS + WMB_ALGO_RLA] || p.soft_ring[WMB_CHAIN_S1 * WMB_N_ALGOS + WMB_ALGO_T2A]) {
+        k3_soft_s1_kernel<<<sms * 32, 64, 0, c->cs>>>(p);     /* the S1 streams' values */
+        c->st.kernel_launches += 1;
+    }
     k3_offsets_kernel<<<1, SCAN_THREADS, 0, c->cs>>>(p);
     k3_copy_kernel<<<sms * 32, 128, 0, c->cs>>>(p);
     k3_carry_kernel<<<sms, 128, 0, c->cs>>>(p);
@@ -580,8 +596,12 @@ static int launch_k3_k4(wmb_ctx *c, const K3Params &p, const K4Params *q, const 
         k4r_repair_kernel<<<sms * 64, K4_THREADS, 0, c->cs>>>(*r);
         c->st.kernel_launches += 1;
     }
-    if (sp) {                                /* C1 soft repair: overwrites K4R's record of a C1 line with CRC errors */
+    if (sp && (sp->k_max || sp->s_max)) {    /* C1 / T1 soft repair: overwrites K4R's record of such a candidate */
         k4s_repair_kernel<<<sms * 64, K4_THREADS, 0, c->cs>>>(*sp);
+        c->st.kernel_launches += 1;
+    }
+    if (sp && sp->s1_max) {                  /* S1 soft repair: K4S's S1 instance */
+        k4s_s1_repair_kernel<<<sms * 64, K4_THREADS, 0, c->cs>>>(*sp);
         c->st.kernel_launches += 1;
     }
     k3_publish_kernel<<<1, 32, 0, c->cs>>>(p);
@@ -1032,14 +1052,18 @@ static int qual_alloc(wmb_ctx *c)
     return WMB_OK;
 }
 
-/* soft values: a ring beside each T1/C1 stream's ring, the frame words' twin, and its host mirror for manual mode */
-static int soft_alloc(wmb_ctx *c)
+/* soft values: a ring beside each T1/C1 stream's ring (and, with S1 values on, each S1 stream's), the frame words' twin,
+ * and its host mirror for manual mode */
+static int soft_alloc(wmb_ctx *c, bool s1)
 {
-    if (c->d_soft_words) return WMB_OK;
-    for (int a = 0; a < WMB_N_ALGOS; a++) {
-        Stream &s = c->cb[WMB_CHAIN_T1C1].s[a];
-        if (s.ring) TRY(dev_alloc(c, &s.soft_ring, s.ring_cap));
+    for (int ch = 0; ch < WMB_N_CHAINS; ch++) {
+        if (ch == WMB_CHAIN_S1 && !s1) continue;
+        for (int a = 0; a < WMB_N_ALGOS; a++) {
+            Stream &s = c->cb[ch].s[a];
+            if (s.ring && !s.soft_ring) TRY(dev_alloc(c, &s.soft_ring, s.ring_cap));
+        }
     }
+    if (c->d_soft_words) return WMB_OK;
     TRY(dev_alloc(c, &c->d_soft_words, c->frame_words_cap));
     if (c->manual) TRY(host_alloc(c, &c->h_soft_words, c->frame_words_cap));
     return WMB_OK;
@@ -1738,10 +1762,11 @@ static int enqueue_gather(wmb_ctx *c, bool final, bool after_batch)
     if (bursts) TRY(burst_alloc(c));
     if (quality) TRY(qual_alloc(c));
     const bool repair = c->repair_e && !c->manual;
-    const bool repair_soft = repair && (c->repair_k || c->repair_s);     /* C1 / T1 candidates: K4S behind K4R */
-    const bool soft = c->soft || repair_soft;
+    const bool repair_soft = repair && (c->repair_k || c->repair_s || c->repair_s1);   /* K4S behind K4R */
+    const bool soft_s1 = c->soft_s1 || (repair && c->repair_s1);        /* the S1 streams' values too */
+    const bool soft = c->soft || soft_s1 || repair_soft;
     if (repair && !c->rep.d) TRY(c->rep.alloc(c, 1, c->hdr.cap, c->hdr.prefix, 256));     /* first gather with repair on */
-    if (soft) TRY(soft_alloc(c));
+    if (soft) TRY(soft_alloc(c, soft_s1));
     if (any_sync) {
         K3Params p;
         memset(&p, 0, sizeof(p));
@@ -1754,7 +1779,7 @@ static int enqueue_gather(wmb_ctx *c, bool final, bool after_batch)
                 p.ring[k] = s.ring; p.ring_mask[k] = s.ring_cap - 1; p.sd[k] = s.sd; p.cand[k] = s.cand; p.pend[k] = s.pend;
                 p.pend_ofs[k] = s.pend_ofs;
                 if (quality) p.pend_qual[k] = s.pend_qual;
-                if (soft) p.soft_ring[k] = s.soft_ring;
+                if (soft && (ch != WMB_CHAIN_S1 || soft_s1)) p.soft_ring[k] = s.soft_ring;
             }
             p.dphi[ch] = c->cb[ch].set[c->last_set].dphi;
         }
@@ -1782,7 +1807,7 @@ static int enqueue_gather(wmb_ctx *c, bool final, bool after_batch)
         memset(&sp, 0, sizeof(sp));
         sp.hdr = r.hdr; sp.dec = r.dec; sp.words = r.words; sp.soft = c->d_soft_words; sp.rep = r.rep; sp.pool = r.pool;
         sp.pool_cap = r.pool_cap; sp.pool_n = r.pool_n; sp.errors = r.errors; sp.k_max = c->repair_k; sp.s_max = c->repair_s;
-        sp.gd = r.gd;
+        sp.s1_max = c->repair_s1; sp.gd = r.gd;
         TRY(launch_k3_k4(c, p, c->manual ? nullptr : &q, repair ? &r : nullptr, repair_soft ? &sp : nullptr));
         /* results -> pinned host mirror: the record and a prefix of the arrays it describes (the rest, if a batch ever
          * produces more, is fetched when the record has been read) */
@@ -1916,7 +1941,7 @@ static int consume_oldest(wmb_ctx *c)
     if (!f.dec && r.n_words) {               /* manual mode reads after every batch: the frame words are this batch's */
         CUDA_TRY(cudaMemcpyAsync(c->h_words, c->d_words, (size_t)r.n_words * 4, cudaMemcpyDeviceToHost, c->xs));
         c->st.d2h_bytes += (uint64_t)r.n_words * 4;
-        if (c->soft) {
+        if (c->soft || c->soft_s1) {
             CUDA_TRY(cudaMemcpyAsync(c->h_soft_words, c->d_soft_words, (size_t)r.n_words * 2, cudaMemcpyDeviceToHost, c->xs));
             c->st.d2h_bytes += (uint64_t)r.n_words * 2;
         }
@@ -1986,7 +2011,7 @@ static int consume_oldest(wmb_ctx *c)
             if (!slot) { c->held.emplace_back(); slot = &c->held.back(); }
             slot->f = fr;
             slot->words.assign(c->h_words + h.word_off, c->h_words + h.word_off + h.nbits);
-            if (c->soft && h.chain == WMB_CHAIN_T1C1) slot->soft.assign(c->h_soft_words + h.word_off, c->h_soft_words + h.word_off + h.nbits);
+            if (h.chain == WMB_CHAIN_T1C1 ? c->soft : c->soft_s1) slot->soft.assign(c->h_soft_words + h.word_off, c->h_soft_words + h.word_off + h.nbits);
             else slot->soft.clear();
         }
     }
@@ -2312,7 +2337,7 @@ static void repaired_from(const RepHdr &h, uint64_t sync_sample, int mode, const
 {
     static const char modes[3][3] = { "T1", "C1", "S1" };
     memset(&o, 0, sizeof(o));
-    o.outcome = h.outcome; o.had_line = h.had_line & 1u;             /* bit 1: K4S's T1 soft rule decided */
+    o.outcome = h.outcome; o.had_line = h.had_line & 1u;             /* bits 1, 2: K4S's T1 / S1 soft rule decided */
     if (h.outcome != K4R_REPAIRED) return;
     o.erasures = h.erasures; o.blocks = h.blocks;
     wmb_decoded &d = o.line;
@@ -2339,7 +2364,8 @@ static void book_repairs(wmb_ctx *c, const FrameHdr *hdr, const DecHdr *dec, con
         wmb_repair_record r;
         memset(&r, 0, sizeof(r));
         r.sync_sample = hdr[i].sync_sample; r.end_sample = hdr[i].sync_sample + h.end_off;
-        r.chain = hdr[i].chain; r.algo = hdr[i].algo; r.soft_t1 = (uint8_t)(h.had_line >> 1);
+        r.chain = hdr[i].chain; r.algo = hdr[i].algo; r.soft_t1 = (uint8_t)(h.had_line >> 1 & 1u);
+        r.soft_s1 = (uint8_t)(h.had_line >> 2 & 1u);
         repaired_from(h, hdr[i].sync_sample, rep_mode(hdr[i].chain, dec[i]), pool, r.repair);
         fresh.push_back(r);
     };
@@ -2507,19 +2533,21 @@ static int launch_k4s(wmb_ctx *c, const K4SParams &p)
 {
 #ifdef WMB_HOSTSIM
     static K4SSmem sm;                  /* the block's phases need real barriers: one simulated thread */
-    hs_for(p.n, [&](uint32_t i) { k4s_repair(p, i, 0, 1, sm); });
+    if (p.s1_max) hs_for(p.n, [&](uint32_t i) { k4s_repair<true>(p, i, 0, 1, sm); });
+    else hs_for(p.n, [&](uint32_t i) { k4s_repair<false>(p, i, 0, 1, sm); });
 #else
-    k4s_repair_kernel<<<p.n ? p.n : 1, K4_THREADS, 0, c->cs>>>(p);
+    if (p.s1_max) k4s_s1_repair_kernel<<<p.n ? p.n : 1, K4_THREADS, 0, c->cs>>>(p);
+    else k4s_repair_kernel<<<p.n ? p.n : 1, K4_THREADS, 0, c->cs>>>(p);
     CUDA_TRY(cudaGetLastError());
 #endif
     c->st.kernel_launches += 1;
     return WMB_OK;
 }
 
-/* K4, the erasure repair K4R and the soft repair K4S (C1 with k_max, T1 with s_max, one of them non-zero) on caller-made
- * frames */
+/* K4, the erasure repair K4R and the soft repair K4S (C1 with k_max, T1 with s_max, S1 with s1_max, one of them non-zero)
+ * on caller-made frames */
 static int repair_soft_device(wmb_ctx *c, const wmb_frame *frames, const int16_t *const *softs, size_t n, uint32_t e_max,
-                              uint32_t k_max, uint32_t s_max, wmb_repaired *out)
+                              uint32_t k_max, uint32_t s_max, uint32_t s1_max, wmb_repaired *out)
 {
     if (e_max > K4R_MAX_ERASURES) return set_err(WMB_E_INVAL, "e_max %u out of range 0..%d", e_max, K4R_MAX_ERASURES);
     memset(out, 0, n * sizeof(*out));
@@ -2553,7 +2581,7 @@ static int repair_soft_device(wmb_ctx *c, const wmb_frame *frames, const int16_t
     memset(&s, 0, sizeof(s));
     s.hdr = r.hdr; s.dec = r.dec; s.n = r.n; s.words = r.words; s.soft = d_soft; s.soft_ok = d_ok; s.rep = d_rep;
     s.pool = r.pool; s.pool_cap = r.pool_cap; s.pool_n = r.pool_n; s.errors = r.errors; s.k_max = k_max;
-    s.s_max = s_max;
+    s.s_max = s_max; s.s1_max = s1_max;
     TRY(launch_k4s(c, s));
     std::vector<RepHdr> rep(n);
     CUDA_TRY(cudaMemcpyAsync(rep.data(), d_rep, n * sizeof(RepHdr), cudaMemcpyDeviceToHost, c->cs));
@@ -2578,7 +2606,7 @@ extern "C" int wmb_frame_repair_soft_device(wmb_ctx *c, const wmb_frame *frames,
     if (!c || !frames || !out || (!softs && n)) return set_err(WMB_E_INVAL, "null argument");
     if (k_max > WMB_SOFT_K_MAX) return set_err(WMB_E_INVAL, "k_max %u out of range 0..%d", k_max, WMB_SOFT_K_MAX);
     if (k_max == 0) return wmb_frame_repair_device(c, frames, n, e_max, out);
-    return repair_soft_device(c, frames, softs, n, e_max, k_max, 0, out);
+    return repair_soft_device(c, frames, softs, n, e_max, k_max, 0, 0, out);
 }
 
 extern "C" int wmb_frame_repair_t1_soft_device(wmb_ctx *c, const wmb_frame *frames, const int16_t *const *softs, size_t n,
@@ -2587,7 +2615,16 @@ extern "C" int wmb_frame_repair_t1_soft_device(wmb_ctx *c, const wmb_frame *fram
     if (!c || !frames || !out || (!softs && n)) return set_err(WMB_E_INVAL, "null argument");
     if (s_max > WMB_SOFT_K_MAX) return set_err(WMB_E_INVAL, "s_max %u out of range 0..%d", s_max, WMB_SOFT_K_MAX);
     if (s_max == 0) return wmb_frame_repair_device(c, frames, n, e_max, out);
-    return repair_soft_device(c, frames, softs, n, e_max, 0, s_max, out);
+    return repair_soft_device(c, frames, softs, n, e_max, 0, s_max, 0, out);
+}
+
+extern "C" int wmb_frame_repair_s1_soft_device(wmb_ctx *c, const wmb_frame *frames, const int16_t *const *softs, size_t n,
+                                               uint32_t e_max, uint32_t s_max, wmb_repaired *out)
+{
+    if (!c || !frames || !out || (!softs && n)) return set_err(WMB_E_INVAL, "null argument");
+    if (s_max > WMB_SOFT_K_MAX) return set_err(WMB_E_INVAL, "s_max %u out of range 0..%d", s_max, WMB_SOFT_K_MAX);
+    if (s_max == 0) return wmb_frame_repair_device(c, frames, n, e_max, out);
+    return repair_soft_device(c, frames, softs, n, e_max, 0, 0, s_max, out);
 }
 
 extern "C" int wmb_decode_frames(wmb_ctx *c, const wmb_frame *frames, size_t n)
@@ -2925,6 +2962,28 @@ extern "C" int wmb_set_repair_t1_soft(wmb_ctx *c, uint32_t s_max)
     return WMB_OK;
 }
 
+extern "C" int wmb_set_soft_bits_s1(wmb_ctx *c, int on)
+{
+    if (!c) return set_err(WMB_E_INVAL, "null argument");
+    if (on != 0 && on != 1) return set_err(WMB_E_INVAL, "S1 soft bits %d: 0 (off) or 1 (on)", on);
+    if (!c->manual) return set_err(WMB_E_INVAL, "wmb_set_soft_bits_s1 needs a manual_frames context (the streaming framer's S1 soft repair: wmb_set_repair_s1_soft)");
+    if (c->batch_no != 0 || !c->remainder.empty())
+        return set_err(WMB_E_STATE, "wmb_set_soft_bits_s1 after samples were pushed (call it before the first push or after wmb_reset / wmb_seek)");
+    c->soft_s1 = on != 0;
+    return WMB_OK;
+}
+
+extern "C" int wmb_set_repair_s1_soft(wmb_ctx *c, uint32_t s_max)
+{
+    if (!c) return set_err(WMB_E_INVAL, "null argument");
+    if (c->manual) return set_err(WMB_E_INVAL, "wmb_set_repair_s1_soft on a manual_frames context (repair the polled frames with wmb_frame_repair_s1_soft_device)");
+    if (s_max > WMB_SOFT_K_MAX) return set_err(WMB_E_INVAL, "s_max %u out of range 0 (off) .. %d", s_max, WMB_SOFT_K_MAX);
+    if (c->batch_no != 0 || !c->remainder.empty())
+        return set_err(WMB_E_STATE, "wmb_set_repair_s1_soft after samples were pushed (call it before the first push or after wmb_reset / wmb_seek)");
+    c->repair_s1 = s_max;
+    return WMB_OK;
+}
+
 extern "C" int wmb_frame_soft(wmb_ctx *c, const wmb_frame *f, const int16_t **soft)
 {
     if (!c || !f || !soft) return set_err(WMB_E_INVAL, "null argument");
@@ -3072,6 +3131,7 @@ extern "C" long wmb_boundary_state(wmb_ctx *c, uint8_t *buf, size_t cap)
     if (c->repair_e) put(&c->repair_e, 4);             /* contexts that repair differently never agree */
     if (c->repair_k) put(&c->repair_k, 4);
     if (c->repair_s) { const uint8_t tag = 'T'; put(&tag, 1); put(&c->repair_s, 4); }   /* never reads as a k_max */
+    if (c->repair_s1) { const uint8_t tag = 'S'; put(&tag, 1); put(&c->repair_s1, 4); }
     if (out.size() > cap) return set_err(WMB_E_INVAL, "buffer too small (%zu bytes needed)", out.size());
     memcpy(buf, out.data(), out.size());
     return (long)out.size();

@@ -1,7 +1,8 @@
 /*
  * wmb_frame_a.h -- the CRC block layout of frame format A (t1_c1_packet_decoder.h:471-506, CRC strip :551-592), shared
  * by the device repair K4R (wmb_kernels.cuh) and its host twin wmb_frame_repair() (wmb_framer.c), so that the two cannot
- * drift apart (and, below, the T1 soft repair's symbol scoring, for K4S and wmb_frame_repair_t1_soft()).  A telegram
+ * drift apart (and, below, the T1 soft repair's symbol scoring and the S1 soft repair's pair scoring, for K4S and
+ * wmb_frame_repair_t1_soft() / wmb_frame_repair_s1_soft()).  A telegram
  * of len >= 12 bytes has a 12-byte first block and 18-byte blocks after it, the last one
  * shorter; each block ends in its two CRC bytes.
  */
@@ -61,6 +62,17 @@ WMB_FA void wmb_t1_sym_ml(const int64_t *y, uint32_t *ml, uint32_t *ru, int64_t 
         else if (s == 16 || c > second) { s = n; second = c; }
     }
     *ml = b; *ru = s; *delta = 2 * (best - second);
+}
+
+/* S1 soft repair (wmbus_b200_framer.h), shared by K4S and its host twin wmb_frame_repair_s1_soft(): Manchester pair p
+ * from its chips' soft values v1, v2 (-32768: none) and hard chips a, c.  *ml is its ML bit; the result its search key
+ * (has a value, |d|, p) as one integer, has << 29 | |d| << 12 | p: |d| <= 65534 < 2^17, p < 8 * 296 < 2^12. */
+WMB_FA uint32_t wmb_s1_pair(int32_t v1, int32_t v2, uint32_t a, uint32_t c, uint32_t p, uint32_t *ml)
+{
+    const int none = v1 == -32768 || v2 == -32768;
+    const int32_t d = none ? 0 : v2 - v1;
+    *ml = d > 0 ? 1u : d < 0 ? 0u : (a != c ? c : 0u);
+    return (none ? 0u : 1u << 29) | (uint32_t)(d < 0 ? -d : d) << 12 | p;
 }
 
 #endif

@@ -572,6 +572,88 @@ int wmb_frame_repair_t1_soft(const wmb_frame *f, const int16_t *soft, uint32_t e
     return WMB_OK;
 }
 
+/* ---- S1 soft repair (definition in wmbus_b200_framer.h; device twin: K4S, wmb_kernels.cuh) ------------------------ */
+
+static unsigned s1_bit(const uint8_t *pkt, unsigned p) { return pkt[p / 8] >> (7 - p % 8) & 1u; }
+
+static void repair_soft_s1(const wmb_frame *f, const int16_t *soft, unsigned L, uint32_t s_max, wmb_repaired *out)
+{
+    const wmb_bit *b = f->bits;
+    const unsigned len = wmb_tlg_length_format_a(L), npair = 8 * len;
+    /* per pair p = 8 l + bit: hard bit (2: a violation), ML bit, search key */
+    static __thread uint8_t hard[8 * 292], ml[8 * 292];
+    static __thread uint32_t key[8 * 292];
+    for (unsigned p = 8; p < npair; p++) {
+        const unsigned a = WMB_BIT_DATA(b[1 + 2 * p]), c = WMB_BIT_DATA(b[2 + 2 * p]);
+        uint32_t m;
+        key[p] = wmb_s1_pair(soft[1 + 2 * p], soft[2 + 2 * p], a, c, p, &m);
+        ml[p] = (uint8_t)m;
+        hard[p] = (uint8_t)(a != c ? c : 2u);
+    }
+
+    uint8_t pkt[292];
+    memset(pkt, 0, sizeof(pkt));
+    pkt[0] = (uint8_t)L;
+    for (unsigned p = 8; p < npair; p++) pkt[p / 8] |= (uint8_t)((hard[p] & 1u) << (7 - p % 8));
+    unsigned changed = 0, blocks = 0;
+    for (unsigned k = 0; k < wmb_nblk_a(len); k++) {
+        const unsigned off = wmb_blk_off_a(k), blk = wmb_blk_len_a(len, k);
+        const unsigned lo = 8 * (off ? off : 1), hi = 8 * (off + blk);    /* the block's searchable pairs */
+        int valid = 1;
+        for (unsigned p = lo; p < hi; p++) valid &= hard[p] != 2u;
+        if (valid && block_ok(pkt + off, blk)) continue;
+        for (unsigned p = lo; p < hi; p++) pkt[p / 8] = (uint8_t)((pkt[p / 8] & ~(0x80u >> p % 8)) | ml[p] << (7 - p % 8));
+        /* the K pairs of lowest key, by selection (keys are unique) */
+        const unsigned K = s_max < hi - lo ? s_max : hi - lo;
+        unsigned sel[WMB_SOFT_K_MAX];
+        for (unsigned t = 0; t < K; t++) {
+            uint32_t best = 0xFFFFFFFFu;
+            for (unsigned p = lo; p < hi; p++)
+                if (key[p] < best && (t == 0 || key[p] > key[sel[t - 1]])) { best = key[p]; sel[t] = p; }
+        }
+        unsigned pass = 0, first = 0;
+        for (unsigned x = 0; x < (1u << K); x++) {
+            uint8_t q[18];
+            memcpy(q, pkt + off, blk);
+            for (unsigned t = 0; t < K; t++)
+                if (x >> t & 1u) q[sel[t] / 8 - off] ^= (uint8_t)(0x80u >> sel[t] % 8);
+            if (block_ok(q, blk)) { if (!pass) first = x; pass++; }
+        }
+        if (pass != 1) { out->outcome = pass ? WMB_REP_AMBIGUOUS : WMB_REP_UNREPAIRABLE; return; }
+        for (unsigned t = 0; t < K; t++)
+            if (first >> t & 1u) pkt[sel[t] / 8] ^= (uint8_t)(0x80u >> sel[t] % 8);
+        for (unsigned p = lo; p < hi; p++) changed += hard[p] != s1_bit(pkt, p);
+        blocks++;
+    }
+    const cursor c = { f, 16 * len, 0 };
+    finish(&c, &out->line, "S1", pkt, len, 0, 0);
+    out->outcome = WMB_REP_REPAIRED;
+    out->erasures = changed < 255 ? changed : 255;         /* the device record's byte */
+    out->blocks = blocks;
+}
+
+int wmb_frame_repair_s1_soft(const wmb_frame *f, const int16_t *soft, uint32_t e_max, uint32_t s_max, wmb_repaired *out)
+{
+    if (s_max > WMB_SOFT_K_MAX || e_max > REP_MAX_ERASURES) { memset(out, 0, sizeof(*out)); return WMB_E_INVAL; }
+    const int rc = wmb_frame_repair(f, e_max, out);
+    if (rc || !s_max || !soft || f->chain != WMB_CHAIN_S1) return rc;
+    /* TOO_MANY / UNREPAIRABLE: a candidate of the erasure rule (a line with crc_ok = 0 or a violation abort) whose list
+     * reaches P; UNREPAIRABLE also stands for len < 12 and an rssi drop, which stay so */
+    if (out->outcome != WMB_REP_TOO_MANY && out->outcome != WMB_REP_UNREPAIRABLE) return rc;
+    unsigned L = 0;
+    for (unsigned k = 0; k < 8; k++) L = (L << 1) | WMB_BIT_DATA(f->bits[2 + 2 * k]);
+    const unsigned len = wmb_tlg_length_format_a(L), P = 1 + 16 * len;
+    if (len < 12) return rc;
+    for (unsigned i = 0; i + 1 < P; i++)
+        if (WMB_BIT_RSSI(f->bits[i]) < CAPTURE_THRESHOLD) return rc;
+    const uint32_t had_line = out->had_line;
+    memset(out, 0, sizeof(*out));
+    out->had_line = had_line;
+    out->outcome = WMB_REP_UNREPAIRABLE;
+    repair_soft_s1(f, soft, L, s_max, out);
+    return WMB_OK;
+}
+
 /* ---- output --------------------------------------------------------------------- */
 
 void wmb_make_time_string(char *ts, size_t n)

@@ -980,8 +980,8 @@ struct K3Params {
     QualAcc *pend_qual[WMB_N_STREAMS];   /* carried candidates' class sums, same slots as pend   */
     QualAcc *qual_log;              /* one per candidate, parallel to hdr_log               */
     uint32_t qual_skip;             /* 1 (-a): the records hold zero sums                   */
-    /* soft values (wmb_set_soft_bits): null when off.  soft_ring[k] parallels ring[k] (T1/C1 streams only), soft_words
-     * parallels words */
+    /* soft values (wmb_set_soft_bits): null when off.  soft_ring[k] parallels ring[k] (T1/C1 streams, and the S1 streams
+     * when their values are on; null: no values for the stream), soft_words parallels words */
     int16_t *soft_ring[WMB_N_STREAMS];
     int16_t *soft_words;
     uint32_t pend_cap, cand_cap;
@@ -1218,35 +1218,51 @@ WMB_D void k3_cut(const K3Params &p, uint32_t i, int tid, int nthr)
     }
 }
 
-/* pass 1c (block per candidate, soft values on): the soft value (wmbus_b200_framer.h) of every event of a T1/C1 candidate
- * that this batch produced, i.e. at a ring position >= the stream's total before the batch, into the soft ring beside the
- * event.  A candidate exists in every batch that produces one of its events, so each shipped event gets its value here,
- * with its dphi at hand in the batch's set; overlapping candidates write the same value.  The window ends at or before
- * the event's own sample (D >= 2) and starts at most 8 * 63 + D + 2 samples before it, inside the set's history prefix. */
+/* pass 1c (block per candidate, soft values on): the soft value (wmbus_b200_framer.h) of every event of a T1/C1 candidate,
+ * and with S1 values on (the S1 streams have soft rings) of an S1 candidate, that this batch produced, i.e. at a ring
+ * position >= the stream's total before the batch, into the soft ring beside the event.  A candidate exists in every
+ * batch that produces one of its events, so each shipped event gets its value here, with its dphi at hand in the batch's
+ * set; overlapping candidates write the same value.  The window ends at or before the event's own sample (T1/C1: D >= 2,
+ * S1: D >= 7) and starts at most 8 * 63 + D + 2 (S1: 24 * 31 + D + 8) samples before it, inside the set's history
+ * prefix. */
+/* One instance per chain (k3_soft_kernel, and k3_soft_s1_kernel when the S1 streams have soft rings): the chain's
+ * constants are compile-time, which keeps the T1/C1 instance at its registers. */
+static_assert(WMB_SOFT_D_T2 >= 2 && WMB_SOFT_D_RL >= 2 && WMB_SOFT_S1_D_T2 >= 7 && WMB_SOFT_S1_D_RL >= 7,
+              "a soft value's window must end at or before its event's sample");
+static_assert(8 * 63 + WMB_SOFT_D_RL + 2 <= WMB_OFS_HIST && 24 * 31 + WMB_SOFT_S1_D_RL + 8 <= WMB_OFS_HIST &&
+              WMB_SOFT_S1_D_T2 + 8 <= WMB_OFS_HIST, "a soft value's window must lie inside the dphi history");
+template <bool S1>
 WMB_D void k3_soft(const K3Params &p, uint32_t i, int tid, int nthr)
 {
     const GatherDev &g = *p.gd;
     if (i >= g.n || !p.soft_words) return;
     const FrameHdr &h = p.hdr_log[g.base + i];
-    if (h.chain != WMB_CHAIN_T1C1) return;
-    const int k = h.algo;                                     /* stream k = chain * WMB_N_ALGOS + algo, chain 0 */
+    const bool s1 = S1;
+    const int chain = S1 ? WMB_CHAIN_S1 : WMB_CHAIN_T1C1;
+    if (h.chain != chain) return;
+    const int k = chain * WMB_N_ALGOS + h.algo;
+    if (S1 && !p.soft_ring[k]) return;
     const uint64_t *ring = p.ring[k];
     const uint64_t mask = p.ring_mask[k], total = p.sd[k]->total;
     const bool rla = h.algo == WMB_ALGO_RLA;
-    const float *dphi = p.dphi[WMB_CHAIN_T1C1] + p.prefix;
+    const float *dphi = p.dphi[chain] + p.prefix;
     const uint64_t from = g.soft_from[k] > h.ordinal ? g.soft_from[k] : h.ordinal;
+    /* window [c - lo, c + hi), run cap, samples per chip, delays and scale of the chain */
+    const uint32_t cap = s1 ? 31 : 63, spc = s1 ? 24 : 8, shift = s1 ? WMB_SOFT_S1_SHIFT : 12;
+    const int64_t lo = s1 ? 8 : 2, hi = s1 ? 8 : 3;
+    const int64_t d_rl = s1 ? WMB_SOFT_S1_D_RL : WMB_SOFT_D_RL, d_t2 = s1 ? WMB_SOFT_S1_D_T2 : WMB_SOFT_D_T2;
     /* every event k3_size found (the list before a reset cut, and before a frame-word overflow empties it) */
     for (uint64_t o = from + (uint64_t)tid; o < h.ordinal + p.cut_n[i]; o += (uint64_t)nthr) {
         const uint64_t m = EVG_M(ring[o & mask]);
         uint32_t after = 0;                                   /* n - 1 - i: the run's later events at sample m */
         if (rla)
-            while (after <= 63 && o + 1 + after < total && EVG_M(ring[(o + 1 + after) & mask]) == m) after++;
-        const int64_t c = (int64_t)((m - p.m_first) & EVG_M_MASK) - (rla ? WMB_SOFT_D_RL + 8 * (int64_t)after : WMB_SOFT_D_T2);
+            while (after <= cap && o + 1 + after < total && EVG_M(ring[(o + 1 + after) & mask]) == m) after++;
+        const int64_t c = (int64_t)((m - p.m_first) & EVG_M_MASK) - (rla ? d_rl + (int64_t)spc * after : d_t2);
         int16_t v = WMB_SOFT_NONE;
-        if (after <= 63 && c - 2 >= -(int64_t)p.clip) {
+        if (after <= cap && c - lo >= -(int64_t)p.clip) {
             int64_t sum = 0;
-            for (int64_t q = c - 2; q < c + 3; q++) sum += wmb_ofs_x(dphi[q]);
-            int64_t x = sum >> 12;                            /* floor */
+            for (int64_t q = c - lo; q < c + hi; q++) sum += wmb_ofs_x(dphi[q]);
+            int64_t x = sum >> shift;                         /* floor */
             x = x > 32767 ? 32767 : x < -32767 ? -32767 : x;
             v = (int16_t)x;
         }
@@ -1309,7 +1325,7 @@ WMB_D void k3_copy(const K3Params &p, uint32_t i, int tid, int nthr)
         uint64_t off = (EVG_M(e) - h.sync_sample) & EVG_M_MASK;
         if (off >= (1u << 23)) off = (1u << 23) - 1;
         p.words[h.word_off + j] = ((uint32_t)off << 9) | (EVG_RSSI(e) << 1) | EVG_BIT(e);
-        if (p.soft_words && h.chain == WMB_CHAIN_T1C1) p.soft_words[h.word_off + j] = p.soft_ring[k][(h.ordinal + j) & mask];
+        if (p.soft_words && p.soft_ring[k]) p.soft_words[h.word_off + j] = p.soft_ring[k][(h.ordinal + j) & mask];
     }
 }
 
@@ -1825,11 +1841,12 @@ WMB_D void k4r_repair(const K4RParams &p, uint32_t f, int tid, int nthr, K4RSmem
 }
 
 /* =========================================================================== */
-/* K4S: soft repair of C1 and T1 candidates (definitions in wmbus_b200_framer.h, host twins wmb_frame_repair_soft() and
- * wmb_frame_repair_t1_soft() in wmb_framer.c).  One warp per candidate, behind K4R: it reads K4's verdict from DecHdr and
- * overwrites K4R's RepHdr of a C1 line with CRC errors (K4R makes those UNREPAIRABLE; k_max) and of a T1 line with CRC
- * errors that K4R found TOO_MANY or UNREPAIRABLE (s_max; had_line = 3, bit 1 saying the T1 soft rule decided); every
- * other record stays as K4R wrote it.  The lanes reduce n0, n1, S0, S1 (T1: and score every symbol into shared memory);
+/* K4S: soft repair of C1, T1 and S1 candidates (definitions in wmbus_b200_framer.h, host twins wmb_frame_repair_soft(),
+ * wmb_frame_repair_t1_soft() and wmb_frame_repair_s1_soft() in wmb_framer.c).  One warp per candidate, behind K4R: it
+ * reads K4's verdict from DecHdr and overwrites K4R's RepHdr of a C1 line with CRC errors (K4R makes those UNREPAIRABLE;
+ * k_max), of a T1 line with CRC errors that K4R found TOO_MANY or UNREPAIRABLE (s_max; had_line = 3, bit 1 saying the
+ * T1 soft rule decided) and of an S1 candidate that K4R found so (s1_max; had_line bit 2 set, bit 0 kept: S1 pairs are
+ * scored on the fly from their two chips, pattern 0 is pure ML as for T1); every other record stays as K4R wrote it.  The lanes reduce n0, n1, S0, S1 (T1: and score every symbol into shared memory);
  * per failing block they pick the K least reliable bits (T1: symbols) by K rounds of warp argmin over a key that orders
  * (has a value, r or delta, index) -- unique, so the choice does not depend on the lanes -- compute the K single-bit CRC
  * syndromes (T1: of the nibble mask ML ^ runner-up at its byte; the CRC is affine: a pattern's syndrome is the received
@@ -1845,6 +1862,7 @@ struct K4SParams {
     uint32_t *errors;
     uint32_t k_max;                 /* C1: 1..WMB_SOFT_K_MAX, 0 = C1 lines are left alone    */
     uint32_t s_max;                 /* T1: 1..WMB_SOFT_K_MAX, 0 = T1 lines are left alone    */
+    uint32_t s1_max;                /* S1: 1..WMB_SOFT_K_MAX, 0 = S1 candidates are left alone */
     const GatherDev *gd;
 };
 
@@ -1893,17 +1911,24 @@ WMB_HD uint32_t k4s_delta(uint32_t q, uint32_t mask, uint32_t nd)
     return crc;
 }
 
+/* two instances: S1 = false repairs C1 and T1 candidates, S1 = true S1 ones.  The S1 branch in one instance with the
+ * others took K4S from 64 to 80 registers (sm_90a) and so from 32 to 25 resident blocks per SM; apart, each instance
+ * keeps its own count, and the C1 / T1 instance is the code it was */
+template <bool S1>
 WMB_D void k4s_repair(const K4SParams &p, uint32_t f, int tid, int nthr, K4SSmem &sm)
 {
     if (f >= k4s_count(p)) return;
     const uint32_t lb = p.gd ? p.gd->base : 0u;
     const FrameHdr h = p.hdr[lb + f];
     const DecHdr d = p.dec[lb + f];
-    if (h.nbits == 0 || d.status != K4_LINE || d.crc_ok) return;
-    /* C1 lines (k_max), and T1 lines whose erasure repair ended in TOO_MANY or UNREPAIRABLE (s_max) */
-    const bool t1 = d.mode == 0;
-    if (t1) {
-        if (!p.s_max) return;
+    const bool s1 = S1;
+    if (S1 != (h.chain == WMB_CHAIN_S1)) return;
+    if (h.nbits == 0 || (!s1 && (d.status != K4_LINE || d.crc_ok))) return;
+    /* C1 lines (k_max), T1 lines (s_max) and S1 candidates (s1_max) whose erasure repair ended in TOO_MANY or
+     * UNREPAIRABLE; an S1 one is a line with CRC errors or a violation abort whose list reaches P */
+    const bool t1 = !s1 && d.mode == 0;
+    if (t1 || s1) {
+        if (!(t1 ? p.s_max : p.s1_max)) return;
         const uint32_t prev = p.rep[lb + f].outcome;
         if (prev != K4R_TOO_MANY && prev != K4R_UNREPAIRABLE) return;
     } else if (d.mode != 1 || !p.k_max) return;
@@ -1912,24 +1937,38 @@ WMB_D void k4s_repair(const K4SParams &p, uint32_t f, int tid, int nthr, K4SSmem
     const int16_t *sv = p.soft + h.word_off;
     RepHdr r;
     r.consumed = 0; r.end_off = 0; r.serial = 0; r.data_off = 0; r.len = 0; r.outcome = K4R_UNREPAIRABLE;
-    r.erasures = 0; r.blocks = 0; r.had_line = t1 ? 3 : 1; r.packet_rssi = 0; r.current_rssi = 0;
-    const bool bframe = !t1 && k4_bits(b, 1, 12) == 0x543u;
-    const uint32_t L = t1 ? (wmb_dec3of6(k4_bits(b, 1, 6)) << 4) | wmb_dec3of6(k4_bits(b, 7, 6)) : k4_bits(b, 17, 8);
+    /* had_line: bit 1 the T1 soft rule decided, bit 2 the S1 one (bit 0 of an S1 candidate: K4R's, 0 for an abort) */
+    r.erasures = 0; r.blocks = 0; r.had_line = t1 ? 3 : s1 ? (uint8_t)(p.rep[lb + f].had_line | 4u) : 1;
+    r.packet_rssi = 0; r.current_rssi = 0;
+    const bool bframe = !t1 && !s1 && k4_bits(b, 1, 12) == 0x543u;
+    uint32_t L = 0;
+    if (s1) for (uint32_t k = 0; k < 8; k++) L = (L << 1) | WMB_BIT_DATA(b[2 + 2 * k]);
+    else L = t1 ? (wmb_dec3of6(k4_bits(b, 1, 6)) << 4) | wmb_dec3of6(k4_bits(b, 7, 6)) : k4_bits(b, 17, 8);
     const uint32_t len = bframe ? 1 + L : wmb_tlg_len_a(L);
     const uint32_t d0 = t1 ? 13 : 17;                   /* the first chip / bit after the L byte */
-    const uint32_t P = t1 ? 1 + 12 * len : 17 + 8 * len;
+    const uint32_t P = s1 ? 1 + 16 * len : t1 ? 1 + 12 * len : 17 + 8 * len;
     r.consumed = P;
     r.end_off = WMB_BIT_OFFSET(b[P - 1]);
-    if (len < 12) { if (tid == 0 && !t1) p.rep[lb + f] = r; return; }     /* T1: not a candidate, K4R's record stands */
+    /* T1, S1: not a candidate, K4R's record stands */
+    if (len < 12) { if (tid == 0 && !t1 && !s1) p.rep[lb + f] = r; return; }
+    if (s1) {                                           /* an rssi drop before P - 1 stays an abort */
+        int64_t low = 0;
+        for (uint32_t j = (uint32_t)tid; j + 1 < P; j += (uint32_t)nthr) low += WMB_BIT_RSSI(b[j]) < K4_CAPTURE_THRESHOLD;
+        if (k4s_sum(low)) return;
+    }
 
-    int64_t n0 = 0, n1 = 0, s0 = 0, s1 = 0;
-    for (uint32_t j = d0 + (uint32_t)tid; j < P; j += (uint32_t)nthr) {
+    int64_t n0 = 0, n1 = 0, s0 = 0, s1s = 0;
+    for (uint32_t j = d0 + (uint32_t)tid; j < P && !s1; j += (uint32_t)nthr) {
         const int16_t v = sv[j];
         if (v == WMB_SOFT_NONE) continue;
-        if (WMB_BIT_DATA(b[j])) { n1++; s1 += v; } else { n0++; s0 += v; }
+        if (WMB_BIT_DATA(b[j])) { n1++; s1s += v; } else { n0++; s0 += v; }
     }
-    n0 = k4s_sum(n0); n1 = k4s_sum(n1); s0 = k4s_sum(s0); s1 = k4s_sum(s1);
-    const int64_t a = 2 * n0 * n1, t = s1 * n0 + s0 * n1;
+    n0 = k4s_sum(n0); n1 = k4s_sum(n1); s0 = k4s_sum(s0); s1s = k4s_sum(s1s);
+    const int64_t a = 2 * n0 * n1, t = s1s * n0 + s0 * n1;
+    /* S1 pair q: its ML bit and search key (wmb_frame_a.h) */
+    auto s1_pair = [&](uint32_t q, uint32_t *ml) -> uint32_t {
+        return wmb_s1_pair(sv[1 + 2 * q], sv[2 + 2 * q], WMB_BIT_DATA(b[1 + 2 * q]), WMB_BIT_DATA(b[2 + 2 * q]), q, ml);
+    };
     /* C1 search key of bit j: (has a value, r, j) in one integer; |r| < 2^38, j < 2^12 */
     auto key = [&](uint32_t j) -> uint64_t {
         const int16_t v = sv[j];
@@ -1959,30 +1998,53 @@ WMB_D void k4s_repair(const K4SParams &p, uint32_t f, int tid, int nthr, K4SSmem
         for (uint32_t l = (uint32_t)tid; l < len; l += (uint32_t)nthr)
             sm.pkt[l] = l == 0 ? (uint8_t)L
                                : (uint8_t)((wmb_dec3of6(k4_bits(b, 1 + 12 * l, 6)) & 15u) << 4 | (wmb_dec3of6(k4_bits(b, 7 + 12 * l, 6)) & 15u));
+    } else if (s1) {                                    /* the hard decode, a violation's bit 0 */
+        for (uint32_t l = (uint32_t)tid; l < len; l += (uint32_t)nthr) {
+            uint32_t v = L;
+            if (l) {
+                v = 0;
+                for (uint32_t k = 0; k < 8; k++) {
+                    const uint32_t x = WMB_BIT_DATA(b[1 + 16 * l + 2 * k]), c = WMB_BIT_DATA(b[2 + 16 * l + 2 * k]);
+                    v |= (x != c ? c : 0u) << (7 - k);
+                }
+            }
+            sm.pkt[l] = (uint8_t)v;
+        }
     } else
         for (uint32_t l = (uint32_t)tid; l < len; l += (uint32_t)nthr) sm.pkt[l] = (uint8_t)k4_bits(b, 17 + 8 * l, 8);
     K4_SYNC();
 
     const uint32_t nblk = bframe ? wmb_nblk_b(len) : wmb_nblk_a(len);
-    const uint32_t kk = t1 ? p.s_max : p.k_max;
+    const uint32_t kk = t1 ? p.s_max : s1 ? p.s1_max : p.k_max;
     uint32_t outcome = K4R_NONE, flips = 0, blocks = 0;
     for (uint32_t k = 0; k < nblk && outcome == K4R_NONE; k++) {
         const uint32_t off = bframe ? wmb_blk_off_b(k) : wmb_blk_off_a(k), blk = bframe ? wmb_blk_len_b(len, k) : wmb_blk_len_a(len, k);
         if (blk < 2) { outcome = K4R_UNREPAIRABLE; break; }          /* no CRC: no pattern can pass */
-        /* the searchable bits (C1) or symbols (T1) of the block */
-        const uint32_t lo = t1 ? 2 * (off ? off : 1) : 17 + 8 * (off ? off : 1), hi = t1 ? 2 * (off + blk) : 17 + 8 * (off + blk);
+        /* the searchable bits (C1), symbols (T1) or pairs (S1) of the block */
+        const uint32_t g0 = off ? off : 1;
+        const uint32_t lo = t1 ? 2 * g0 : s1 ? 8 * g0 : 17 + 8 * g0, hi = t1 ? 2 * (off + blk) : s1 ? 8 * (off + blk) : 17 + 8 * (off + blk);
         int64_t invalid = 0;
         if (t1)
             for (uint32_t i = lo + (uint32_t)tid; i < hi; i += (uint32_t)nthr) invalid += sm.hard[i] == 0xFFu;
+        else if (s1)
+            for (uint32_t q = lo + (uint32_t)tid; q < hi; q += (uint32_t)nthr)
+                invalid += WMB_BIT_DATA(b[1 + 2 * q]) == WMB_BIT_DATA(b[2 + 2 * q]);
         invalid = k4s_sum(invalid);
         if (tid == 0) sm.s0 = k4_crc16(sm.pkt + off, blk - 2) ^ (((uint32_t)sm.pkt[off + blk - 2] << 8) | sm.pkt[off + blk - 1]);
         K4_SYNC();
         uint32_t syn = sm.s0;
         K4_SYNC();
         if (syn == 0 && invalid == 0) continue;
-        if (t1) {                                               /* every searchable symbol takes its ML value */
-            for (uint32_t l = lo / 2 + (uint32_t)tid; l < hi / 2; l += (uint32_t)nthr)
-                sm.pkt[l] = (uint8_t)((sm.mr[2 * l] & 0xF0u) | sm.mr[2 * l + 1] >> 4);
+        if (t1 || s1) {                                         /* every searchable symbol / pair takes its ML value */
+            if (t1)
+                for (uint32_t l = lo / 2 + (uint32_t)tid; l < hi / 2; l += (uint32_t)nthr)
+                    sm.pkt[l] = (uint8_t)((sm.mr[2 * l] & 0xF0u) | sm.mr[2 * l + 1] >> 4);
+            else
+                for (uint32_t l = lo / 8 + (uint32_t)tid; l < hi / 8; l += (uint32_t)nthr) {
+                    uint32_t v = 0, ml;
+                    for (uint32_t k = 0; k < 8; k++) { s1_pair(8 * l + k, &ml); v |= ml << (7 - k); }
+                    sm.pkt[l] = (uint8_t)v;
+                }
             K4_SYNC();
             if (tid == 0) sm.s0 = k4_crc16(sm.pkt + off, blk - 2) ^ (((uint32_t)sm.pkt[off + blk - 2] << 8) | sm.pkt[off + blk - 1]);
             K4_SYNC();
@@ -1993,7 +2055,8 @@ WMB_D void k4s_repair(const K4SParams &p, uint32_t f, int tid, int nthr, K4SSmem
         for (uint32_t u = 0; u < K; u++) {
             uint64_t best = ~0ull;
             for (uint32_t j = lo + (uint32_t)tid; j < hi; j += (uint32_t)nthr) {
-                const uint64_t kj = t1 ? sm.key[j] : key(j);
+                uint32_t ml;
+                const uint64_t kj = t1 ? sm.key[j] : s1 ? (uint64_t)s1_pair(j, &ml) : key(j);
                 if (kj > prev && kj < best) best = kj;
             }
             prev = k4s_min(best);
@@ -2004,13 +2067,14 @@ WMB_D void k4s_repair(const K4SParams &p, uint32_t f, int tid, int nthr, K4SSmem
         for (uint32_t u = (uint32_t)tid; u < K; u += (uint32_t)nthr) {
             const uint32_t j = sm.sel[u];
             sm.delta[u] = t1 ? k4s_delta(j / 2 - off, (uint32_t)((sm.mr[j] >> 4) ^ (sm.mr[j] & 15u)) << (j & 1u ? 0 : 4), blk - 2)
+                        : s1 ? k4s_delta(j / 8 - off, 0x80u >> (j % 8), blk - 2)
                              : k4s_delta((j - 17) / 8 - off, 0x80u >> ((j - 17) % 8), blk - 2);
         }
         K4_SYNC();
         int64_t npass = 0;
         uint64_t first = ~0ull;
         for (uint32_t x = (uint32_t)tid; x < 64; x += (uint32_t)nthr) {
-            if ((x == 0 && !t1) || x >= (1u << K)) continue;        /* T1: pattern 0 is pure ML */
+            if ((x == 0 && !t1 && !s1) || x >= (1u << K)) continue;     /* T1, S1: pattern 0 is pure ML */
             uint32_t s = syn;
             for (uint32_t u = 0; u < K; u++) if (x >> u & 1u) s ^= sm.delta[u];
             if (s == 0) { npass++; if (x < first) first = x; }
@@ -2023,6 +2087,7 @@ WMB_D void k4s_repair(const K4SParams &p, uint32_t f, int tid, int nthr, K4SSmem
                 if (!(first >> u & 1u)) continue;
                 const uint32_t j = sm.sel[u];
                 if (t1) sm.pkt[j / 2] ^= (uint8_t)(((sm.mr[j] >> 4) ^ (sm.mr[j] & 15u)) << (j & 1u ? 0 : 4));
+                else if (s1) sm.pkt[j / 8] ^= (uint8_t)(0x80u >> (j % 8));
                 else sm.pkt[(j - 17) / 8] ^= (uint8_t)(0x80u >> ((j - 17) % 8));
             }
         K4_SYNC();
@@ -2030,6 +2095,13 @@ WMB_D void k4s_repair(const K4SParams &p, uint32_t f, int tid, int nthr, K4SSmem
             int64_t changed = 0;
             for (uint32_t i = lo + (uint32_t)tid; i < hi; i += (uint32_t)nthr)
                 changed += sm.hard[i] != (i & 1u ? sm.pkt[i / 2] & 15u : sm.pkt[i / 2] >> 4);
+            flips += (uint32_t)k4s_sum(changed);
+        } else if (s1) {                                        /* the bits that differ from the hard decode */
+            int64_t changed = 0;
+            for (uint32_t q = lo + (uint32_t)tid; q < hi; q += (uint32_t)nthr) {
+                const uint32_t x = WMB_BIT_DATA(b[1 + 2 * q]), c = WMB_BIT_DATA(b[2 + 2 * q]);
+                changed += x == c || c != (uint32_t)(sm.pkt[q / 8] >> (7 - q % 8) & 1u);
+            }
             flips += (uint32_t)k4s_sum(changed);
         } else flips += (uint32_t)wmb_popc((uint32_t)first);
         blocks++;
@@ -2437,7 +2509,11 @@ __global__ void __launch_bounds__(SCAN_THREADS) k3_offsets_kernel(const K3Params
 }
 __global__ void k3_soft_kernel(const K3Params p)
 {
-    for (uint32_t i = blockIdx.x; i < p.gd->n; i += gridDim.x) k3_soft(p, i, threadIdx.x, blockDim.x);
+    for (uint32_t i = blockIdx.x; i < p.gd->n; i += gridDim.x) k3_soft<false>(p, i, threadIdx.x, blockDim.x);
+}
+__global__ void k3_soft_s1_kernel(const K3Params p)
+{
+    for (uint32_t i = blockIdx.x; i < p.gd->n; i += gridDim.x) k3_soft<true>(p, i, threadIdx.x, blockDim.x);
 }
 __global__ void k3_copy_kernel(const K3Params p)
 {
@@ -2471,7 +2547,16 @@ __global__ void __launch_bounds__(K4_THREADS) k4s_repair_kernel(const K4SParams 
     __shared__ K4SSmem sm;
     const uint32_t n = k4s_count(p);
     for (uint32_t f = blockIdx.x; f < n; f += gridDim.x) {
-        k4s_repair(p, f, threadIdx.x, blockDim.x, sm);
+        k4s_repair<false>(p, f, threadIdx.x, blockDim.x, sm);
+        __syncthreads();
+    }
+}
+__global__ void __launch_bounds__(K4_THREADS) k4s_s1_repair_kernel(const K4SParams p)
+{
+    __shared__ K4SSmem sm;
+    const uint32_t n = k4s_count(p);
+    for (uint32_t f = blockIdx.x; f < n; f += gridDim.x) {
+        k4s_repair<true>(p, f, threadIdx.x, blockDim.x, sm);
         __syncthreads();
     }
 }

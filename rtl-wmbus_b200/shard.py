@@ -202,8 +202,8 @@ def decode_time_chunk(ctx, push, n_bytes: int, d: int, rank: int, world: int, ha
     quality=True (ctx made with quality=True): the lines' wmb_line_quality records follow the line records, and with
     bursts=True the bursts' wmb_burst_quality records follow the bursts: (lines[, records], quality[, bursts,
     burst_quality][, spectrum]).  Their windows are the offset windows, so they are the sequential run's as well.
-    repairs=True (ctx made with repair=e_max, repair_soft=k_max for the C1 and repair_t1_soft=s_max for the T1 soft
-    repair; the setting survives the chunk's seek): the repair records (take_repairs()) of the candidates matched in the chunk
+    repairs=True (ctx made with repair=e_max, repair_soft=k_max for the C1, repair_t1_soft=s_max for the T1 and
+    repair_s1_soft=s_max for the S1 soft repair; the settings survive the chunk's seek): the repair records (take_repairs()) of the candidates matched in the chunk
     come last; merge_repairs() over the chunks gives the sequential records.  A candidate that waits for its repair
     counts in pending_before(), so the right halo goes on until its record is made."""
     import hashlib
