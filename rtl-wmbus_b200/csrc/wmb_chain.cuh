@@ -15,10 +15,20 @@
 /* ---- geometry of the demod kernel (K1) ---- */
 #define K1_THREADS   256       /* threads that convert, filter and demodulate a tile                            */
 #define K1_BLOCK     (K1_THREADS + 32)   /* ... plus one warp that only runs the RSSI recurrences, one tile behind */
-#define K1_TILE      960       /* decimated samples produced per tile: TILE + HALO = 4 rows per thread exactly */
-#define K1_HALO      64        /* decimated samples recomputed left of each tile */
-#define K1_RSSI_SEG  32        /* outputs per RSSI recurrence segment (one thread of the RSSI warp)  */
+#define K1_HALO      64        /* decimated samples recomputed left of each tile (the S1 FIR's 45 and the RSSI warm-up's 48,
+                                  rounded up so that the tile is whole 32-sample slicer words) */
 #define K1_RSSI_WARM 48        /* warm-up steps before each segment (contraction 0.32 per step) */
+#define K1_RPT_WIDE   8        /* rows per producer thread on d = 1 and the d = 2 fast path: the block still fits 4 per SM */
+#define K1_RPT_NARROW 4        /* ... on every other geometry (the tile of decimation 25 must fit one block)               */
+/* tile geometry of a kernel instance: RPT rows per producer thread, TILE + HALO = RPT * K1_THREADS rows, TILE outputs
+ * (960 or 1984); the RSSI warp runs one segment of SEG outputs per thread (30 of 32 or 31 of 64) */
+template <int RPT> struct K1Geo {
+    static constexpr int ROWS = RPT * K1_THREADS;
+    static constexpr int TILE = ROWS - K1_HALO;
+    static constexpr int SEG = 8 * RPT;
+    static_assert(TILE % 32 == 0 && TILE % SEG == 0 && TILE / SEG <= 32, "whole slicer words, one RSSI segment per lane");
+};
+#define K1_TILE      (K1Geo<K1_RPT_NARROW>::TILE)   /* 960: the tile of the separate box / discriminator phases */
 #define K1_BOX_MAX   16
 
 /* ---- bit-sync lanes (K2) ---- */

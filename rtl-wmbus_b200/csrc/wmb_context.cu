@@ -332,6 +332,45 @@ static uint32_t *gd_field(wmb_ctx *c, size_t off) { return (uint32_t *)((uint8_t
 
 #ifdef WMB_HOSTSIM
 #include "hostsim_launch.inl"
+/* The demod kernel's wide tile (k1_rows_per_thread(): d = 1 or the d = 2 fast path, so neither the prefilter nor the
+ * separate box / discriminator phases occur) in the CPU build, with the narrow tile's structure: each barrier-separated
+ * phase over all producer threads, then the RSSI warp's lanes.  Narrow tiles go through launch_k1 of hostsim_launch.inl. */
+template <class CH>
+static void hostsim_k1_wide_chain(const K1Params &p, K1Smem &sm, const uint8_t *raw, int64_t tile, bool need_convert)
+{
+    const bool fast = p.d == 2u;
+    if (need_convert) hs_for(K1_THREADS, [&](uint32_t t) {
+        if (fast) k1_convert_fast(p, sm, raw, tile, t); else k1_convert<CH::ID>(p, sm, raw, tile, t);
+    });
+    if (fast) hs_for(K1_THREADS, [&](uint32_t t) { k1_box_disc<CH, 1, true, K1_RPT_WIDE>(p, sm, t); });
+    else hs_for(K1_THREADS, [&](uint32_t t) { k1_box_disc<CH, 1, false, K1_RPT_WIDE>(p, sm, t); });
+    hs_for(K1_THREADS, [&](uint32_t t) { k1_fir<CH, K1_RPT_WIDE>(p, sm, tile, t); });
+    hs_for(32, [&](uint32_t t) { k1_rssi<CH, K1_RPT_WIDE>(p, sm.mag, tile, t); });      /* the block's RSSI warp */
+}
+
+static int launch_demod(wmb_ctx *c, const K1Params &p, cudaStream_t st)
+{
+    if (p.rpt != K1_RPT_WIDE) return launch_k1(c, p, st);
+    const int64_t ntiles = (p.M + K1Geo<K1_RPT_WIDE>::TILE - 1) / K1Geo<K1_RPT_WIDE>::TILE;
+    std::vector<uint8_t> smem(k1_smem_bytes(p.d, p.prefilter, p.rpt) + 256, 0xA5);   /* garbage-filled like real smem */
+    K1Smem sm;
+    uint8_t *base = smem.data();
+    base += (128 - ((uintptr_t)base & 127)) & 127;
+    k1_carve(sm, base, p.d, p.prefilter, p.rpt);
+    hs_for(WMB_ATAN_TAB_ELEMS, [&](uint32_t i) { wmb_atan_tab_fill((WmbAtanTab *)base, i); });
+    int rc = WMB_OK;
+    hs_for((uint32_t)ntiles, [&](uint32_t tile) {
+        const K1Load L = k1_plan_load(p, tile);
+        if (L.n0) memcpy(sm.bytes[0], L.src0, (size_t)L.n0);
+        if (L.n1) memcpy(sm.bytes[0] + L.off1, L.src1, (size_t)L.n1);
+        if ((L.n0 | L.n1 | L.off1) & 15) { rc = set_err(WMB_E_STATE, "hostsim: unaligned bulk copy"); return; }
+        const uint8_t *raw = sm.bytes[0];
+        if (p.chains & 1u) hostsim_k1_wide_chain<ChainT1C1>(p, sm, raw, tile, true);
+        if (p.chains & 2u) hostsim_k1_wide_chain<ChainS1>(p, sm, raw, tile, p.mix || !(p.chains & 1u));
+    });
+    c->st.kernel_launches++;
+    return rc;
+}
 /* the CPU build runs every launch when it is enqueued, in the order of the calls: the stream is not needed */
 static int launch_k2p1(wmb_ctx *c, const K2p1Params &p, cudaStream_t) { return launch_k2p1(c, p); }
 static int launch_k2p_rest(wmb_ctx *c, const K2pcParams &pc, const K2p2Params &p2, cudaStream_t) { return launch_k2p_rest(c, pc, p2); }
@@ -383,18 +422,23 @@ static int launch_k3_k4(wmb_ctx *c, const K3Params &p, const K4Params *q, const 
 #else
 static int g_k1_ctas = 0;                /* WMBUS_B200_K1_CTAS: resident demod blocks per SM (0: as many as fit) */
 
-static int launch_k1(wmb_ctx *c, const K1Params &p, cudaStream_t st)
+static int launch_demod(wmb_ctx *c, const K1Params &p, cudaStream_t st)
 {
-    const int64_t ntiles = (p.M + K1_TILE - 1) / K1_TILE;
+    const int64_t tile = k1_tile_len(p.rpt);
+    const int64_t ntiles = (p.M + tile - 1) / tile;
     /* `-p S -p T` turns both chains off: no chain buffer exists, and there is nothing to demodulate */
     if (ntiles <= 0 || p.chains == 0u) return WMB_OK;
     static int sm_count = 0, blocks_per_sm = 0;
-    const size_t smem = k1_smem_bytes(p.d, p.prefilter);
+    const size_t smem = k1_smem_bytes(p.d, p.prefilter, p.rpt);
     if (!sm_count) {
         cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, c->device);
     }
+    const bool wide = p.rpt == K1_RPT_WIDE;
     auto kern = p.prefilter ? (p.chains == 1u ? k1_demod_pre_kernel<1u> : p.chains == 2u ? k1_demod_pre_kernel<2u> : k1_demod_pre_kernel<3u>)
-                            : (p.chains == 1u ? k1_demod_kernel<1u> : p.chains == 2u ? k1_demod_kernel<2u> : k1_demod_kernel<3u>);
+              : wide ? (p.chains == 1u ? k1_demod_kernel<1u, K1_RPT_WIDE> : p.chains == 2u ? k1_demod_kernel<2u, K1_RPT_WIDE>
+                                                                            : k1_demod_kernel<3u, K1_RPT_WIDE>)
+                     : (p.chains == 1u ? k1_demod_kernel<1u, K1_RPT_NARROW> : p.chains == 2u ? k1_demod_kernel<2u, K1_RPT_NARROW>
+                                                                              : k1_demod_kernel<3u, K1_RPT_NARROW>);
     CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm, kern, K1_BLOCK, smem));
     if (blocks_per_sm < 1) return set_err(WMB_E_INVAL, "decimation %u needs %zu B shared memory per CTA", p.d, smem);
@@ -1448,6 +1492,7 @@ static int run_batch(wmb_ctx *c, const uint8_t *src, size_t nbytes, cudaEvent_t 
     k1.M = M; k1.d = d; k1.chains = c->chains;
     k1.accurate = c->o.accurate_atan; k1.mix = c->o.simultaneous ? 1u : 0u;
     k1.prefilter = c->o.prefilter;
+    k1.rpt = k1_rows_per_thread(d, k1.mix, k1.prefilter);
     k1.lut_n = c->o.simultaneous ? (c->o.decimation * 800u) / 25u : 1u;
     k1.mix_k0 = (uint32_t)(c->iq_consumed % k1.lut_n);
     for (int ch = 0; ch < WMB_N_CHAINS; ch++) {
@@ -1464,7 +1509,7 @@ static int run_batch(wmb_ctx *c, const uint8_t *src, size_t nbytes, cudaEvent_t 
         k1.rssi[ch] = c->cb[ch].set[set].rssi ? c->cb[ch].set[set].rssi + c->W : nullptr;
         k1.dbits[ch] = k1_bits && c->cb[ch].set[set].dbits ? c->cb[ch].set[set].dbits + c->W / 32 : nullptr;
     }
-    TRY(launch_k1(c, k1, sk));
+    TRY(launch_demod(c, k1, sk));
     CUDA_TRY(cudaEventRecord(evt[1], sk));
     CUDA_TRY(cudaEventRecord(c->ev_k1[set], sk));
     /* keep the last k1_hist_bytes() of the stream for the next batch's tile 0 */
