@@ -139,6 +139,29 @@ static int parse_pair(const char *e, unsigned long v[2])
     return *end == 0 && v[0] <= 0xFFFFFFFFul && v[1] <= 0xFFFFFFFFul;
 }
 
+#define STR_(x) #x
+#define STR(x) STR_(x)
+#define SOFT_K_MAX_STR STR(WMB_SOFT_K_MAX)
+
+/* a WMBUS_B200_REPAIR_* variable: when set, it needs WMBUS_B200_REPAIRED and a decimal in 1 .. hi (expected says which)
+ * goes to *v; returns 1 after printing why it does not */
+static int repair_setting(const char *name, unsigned long hi, const char *expected, unsigned long *v)
+{
+    const char *e = getenv(name);
+    if (!e) return 0;
+    char *end = NULL;
+    *v = strtoul(e, &end, 10);
+    if (!getenv("WMBUS_B200_REPAIRED")) {
+        fprintf(stderr, "rtl_wmbus_b200: %s needs WMBUS_B200_REPAIRED\n", name);
+        return 1;
+    }
+    if (e[0] < '0' || e[0] > '9' || *end || *v < 1 || *v > hi) {
+        fprintf(stderr, "rtl_wmbus_b200: %s=%s: expected %s\n", name, e, expected);
+        return 1;
+    }
+    return 0;
+}
+
 /* WMBUS_B200_LINE_INFO / WMBUS_B200_LINE_QUALITY: one record per stdout line, in the same order */
 static FILE *g_info_file = NULL, *g_qual_file = NULL;
 #define INFO_CAP 4096
@@ -437,58 +460,12 @@ int main(int argc, char *argv[])
         }
     }
 
-    unsigned long repair_e = 1;
-    if ((e = getenv("WMBUS_B200_REPAIR_ERASURES")) != NULL) {
-        char *end = NULL;
-        repair_e = strtoul(e, &end, 10);
-        if (!getenv("WMBUS_B200_REPAIRED")) {
-            fprintf(stderr, "rtl_wmbus_b200: WMBUS_B200_REPAIR_ERASURES needs WMBUS_B200_REPAIRED\n");
-            return EXIT_FAILURE;
-        }
-        if (e[0] < '0' || e[0] > '9' || *end || repair_e < 1 || repair_e > 3) {
-            fprintf(stderr, "rtl_wmbus_b200: WMBUS_B200_REPAIR_ERASURES=%s: expected 1, 2 or 3\n", e);
-            return EXIT_FAILURE;
-        }
-    }
-    unsigned long repair_k = 0;
-    if ((e = getenv("WMBUS_B200_REPAIR_SOFT_BITS")) != NULL) {
-        char *end = NULL;
-        repair_k = strtoul(e, &end, 10);
-        if (!getenv("WMBUS_B200_REPAIRED")) {
-            fprintf(stderr, "rtl_wmbus_b200: WMBUS_B200_REPAIR_SOFT_BITS needs WMBUS_B200_REPAIRED\n");
-            return EXIT_FAILURE;
-        }
-        if (e[0] < '0' || e[0] > '9' || *end || repair_k < 1 || repair_k > WMB_SOFT_K_MAX) {
-            fprintf(stderr, "rtl_wmbus_b200: WMBUS_B200_REPAIR_SOFT_BITS=%s: expected 1 .. %d\n", e, WMB_SOFT_K_MAX);
-            return EXIT_FAILURE;
-        }
-    }
-    unsigned long repair_s = 0;
-    if ((e = getenv("WMBUS_B200_REPAIR_T1_SOFT_SYMBOLS")) != NULL) {
-        char *end = NULL;
-        repair_s = strtoul(e, &end, 10);
-        if (!getenv("WMBUS_B200_REPAIRED")) {
-            fprintf(stderr, "rtl_wmbus_b200: WMBUS_B200_REPAIR_T1_SOFT_SYMBOLS needs WMBUS_B200_REPAIRED\n");
-            return EXIT_FAILURE;
-        }
-        if (e[0] < '0' || e[0] > '9' || *end || repair_s < 1 || repair_s > WMB_SOFT_K_MAX) {
-            fprintf(stderr, "rtl_wmbus_b200: WMBUS_B200_REPAIR_T1_SOFT_SYMBOLS=%s: expected 1 .. %d\n", e, WMB_SOFT_K_MAX);
-            return EXIT_FAILURE;
-        }
-    }
-    unsigned long repair_s1 = 0;
-    if ((e = getenv("WMBUS_B200_REPAIR_S1_SOFT_BITS")) != NULL) {
-        char *end = NULL;
-        repair_s1 = strtoul(e, &end, 10);
-        if (!getenv("WMBUS_B200_REPAIRED")) {
-            fprintf(stderr, "rtl_wmbus_b200: WMBUS_B200_REPAIR_S1_SOFT_BITS needs WMBUS_B200_REPAIRED\n");
-            return EXIT_FAILURE;
-        }
-        if (e[0] < '0' || e[0] > '9' || *end || repair_s1 < 1 || repair_s1 > WMB_SOFT_K_MAX) {
-            fprintf(stderr, "rtl_wmbus_b200: WMBUS_B200_REPAIR_S1_SOFT_BITS=%s: expected 1 .. %d\n", e, WMB_SOFT_K_MAX);
-            return EXIT_FAILURE;
-        }
-    }
+    unsigned long repair_e = 1, repair_k = 0, repair_s = 0, repair_s1 = 0;
+    if (repair_setting("WMBUS_B200_REPAIR_ERASURES", 3, "1, 2 or 3", &repair_e) ||
+        repair_setting("WMBUS_B200_REPAIR_SOFT_BITS", WMB_SOFT_K_MAX, "1 .. " SOFT_K_MAX_STR, &repair_k) ||
+        repair_setting("WMBUS_B200_REPAIR_T1_SOFT_SYMBOLS", WMB_SOFT_K_MAX, "1 .. " SOFT_K_MAX_STR, &repair_s) ||
+        repair_setting("WMBUS_B200_REPAIR_S1_SOFT_BITS", WMB_SOFT_K_MAX, "1 .. " SOFT_K_MAX_STR, &repair_s1))
+        return EXIT_FAILURE;
     if ((e = getenv("WMBUS_B200_REPAIRED")) != NULL && (g_rep_file = fopen(e, "w")) == NULL) {
         fprintf(stderr, "rtl_wmbus_b200: WMBUS_B200_REPAIRED=%s: %s\n", e, strerror(errno));
         return EXIT_FAILURE;

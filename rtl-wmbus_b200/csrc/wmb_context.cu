@@ -2589,11 +2589,14 @@ static int launch_k4s(wmb_ctx *c, const K4SParams &p)
     return WMB_OK;
 }
 
-/* K4, the erasure repair K4R and the soft repair K4S (C1 with k_max, T1 with s_max, S1 with s1_max, one of them non-zero)
- * on caller-made frames */
+/* K4, the erasure repair K4R and the soft repair K4S on caller-made frames, with one of K4S's limits (k_max: C1, s_max: T1,
+ * s1_max: S1) set to k, named name in the messages; k = 0: wmb_frame_repair_device */
 static int repair_soft_device(wmb_ctx *c, const wmb_frame *frames, const int16_t *const *softs, size_t n, uint32_t e_max,
-                              uint32_t k_max, uint32_t s_max, uint32_t s1_max, wmb_repaired *out)
+                              uint32_t K4SParams::*limit, const char *name, uint32_t k, wmb_repaired *out)
 {
+    if (!c || !frames || !out || (!softs && n)) return set_err(WMB_E_INVAL, "null argument");
+    if (k > WMB_SOFT_K_MAX) return set_err(WMB_E_INVAL, "%s %u out of range 0..%d", name, k, WMB_SOFT_K_MAX);
+    if (k == 0) return wmb_frame_repair_device(c, frames, n, e_max, out);
     if (e_max > K4R_MAX_ERASURES) return set_err(WMB_E_INVAL, "e_max %u out of range 0..%d", e_max, K4R_MAX_ERASURES);
     memset(out, 0, n * sizeof(*out));
     if (n == 0) return WMB_OK;
@@ -2625,8 +2628,8 @@ static int repair_soft_device(wmb_ctx *c, const wmb_frame *frames, const int16_t
     K4SParams s;
     memset(&s, 0, sizeof(s));
     s.hdr = r.hdr; s.dec = r.dec; s.n = r.n; s.words = r.words; s.soft = d_soft; s.soft_ok = d_ok; s.rep = d_rep;
-    s.pool = r.pool; s.pool_cap = r.pool_cap; s.pool_n = r.pool_n; s.errors = r.errors; s.k_max = k_max;
-    s.s_max = s_max; s.s1_max = s1_max;
+    s.pool = r.pool; s.pool_cap = r.pool_cap; s.pool_n = r.pool_n; s.errors = r.errors;
+    s.*limit = k;
     TRY(launch_k4s(c, s));
     std::vector<RepHdr> rep(n);
     CUDA_TRY(cudaMemcpyAsync(rep.data(), d_rep, n * sizeof(RepHdr), cudaMemcpyDeviceToHost, c->cs));
@@ -2648,28 +2651,19 @@ static int repair_soft_device(wmb_ctx *c, const wmb_frame *frames, const int16_t
 extern "C" int wmb_frame_repair_soft_device(wmb_ctx *c, const wmb_frame *frames, const int16_t *const *softs, size_t n,
                                             uint32_t e_max, uint32_t k_max, wmb_repaired *out)
 {
-    if (!c || !frames || !out || (!softs && n)) return set_err(WMB_E_INVAL, "null argument");
-    if (k_max > WMB_SOFT_K_MAX) return set_err(WMB_E_INVAL, "k_max %u out of range 0..%d", k_max, WMB_SOFT_K_MAX);
-    if (k_max == 0) return wmb_frame_repair_device(c, frames, n, e_max, out);
-    return repair_soft_device(c, frames, softs, n, e_max, k_max, 0, 0, out);
+    return repair_soft_device(c, frames, softs, n, e_max, &K4SParams::k_max, "k_max", k_max, out);
 }
 
 extern "C" int wmb_frame_repair_t1_soft_device(wmb_ctx *c, const wmb_frame *frames, const int16_t *const *softs, size_t n,
                                                uint32_t e_max, uint32_t s_max, wmb_repaired *out)
 {
-    if (!c || !frames || !out || (!softs && n)) return set_err(WMB_E_INVAL, "null argument");
-    if (s_max > WMB_SOFT_K_MAX) return set_err(WMB_E_INVAL, "s_max %u out of range 0..%d", s_max, WMB_SOFT_K_MAX);
-    if (s_max == 0) return wmb_frame_repair_device(c, frames, n, e_max, out);
-    return repair_soft_device(c, frames, softs, n, e_max, 0, s_max, 0, out);
+    return repair_soft_device(c, frames, softs, n, e_max, &K4SParams::s_max, "s_max", s_max, out);
 }
 
 extern "C" int wmb_frame_repair_s1_soft_device(wmb_ctx *c, const wmb_frame *frames, const int16_t *const *softs, size_t n,
                                                uint32_t e_max, uint32_t s_max, wmb_repaired *out)
 {
-    if (!c || !frames || !out || (!softs && n)) return set_err(WMB_E_INVAL, "null argument");
-    if (s_max > WMB_SOFT_K_MAX) return set_err(WMB_E_INVAL, "s_max %u out of range 0..%d", s_max, WMB_SOFT_K_MAX);
-    if (s_max == 0) return wmb_frame_repair_device(c, frames, n, e_max, out);
-    return repair_soft_device(c, frames, softs, n, e_max, 0, 0, s_max, out);
+    return repair_soft_device(c, frames, softs, n, e_max, &K4SParams::s1_max, "s_max", s_max, out);
 }
 
 extern "C" int wmb_decode_frames(wmb_ctx *c, const wmb_frame *frames, size_t n)
@@ -2963,13 +2957,24 @@ extern "C" int wmb_set_line_quality(wmb_ctx *c, int on)
     return WMB_OK;
 }
 
-extern "C" int wmb_set_repair(wmb_ctx *c, uint32_t e_max)
+/* What the repair and soft-value setters check alike: a context of the right kind (streaming for a repair setter, where
+ * instead names the hook for polled frames; manual_frames for a soft-value setter, where instead names the streaming
+ * setter), v in 0 (off) .. hi (what == null: the caller checked its value), and no sample pushed yet. */
+static int repair_setter_check(wmb_ctx *c, const char *name, bool manual, const char *instead, const char *what, uint32_t v,
+                               uint32_t hi)
 {
     if (!c) return set_err(WMB_E_INVAL, "null argument");
-    if (c->manual) return set_err(WMB_E_INVAL, "wmb_set_repair on a manual_frames context (repair the polled frames with wmb_frame_repair_device)");
-    if (e_max > K4R_MAX_ERASURES) return set_err(WMB_E_INVAL, "e_max %u out of range 0 (off) .. %d", e_max, K4R_MAX_ERASURES);
+    if (c->manual && !manual) return set_err(WMB_E_INVAL, "%s on a manual_frames context (repair the polled frames with %s)", name, instead);
+    if (!c->manual && manual) return set_err(WMB_E_INVAL, "%s needs a manual_frames context (the streaming framer's %s)", name, instead);
+    if (what && v > hi) return set_err(WMB_E_INVAL, "%s %u out of range 0 (off) .. %u", what, v, hi);
     if (c->batch_no != 0 || !c->remainder.empty())
-        return set_err(WMB_E_STATE, "wmb_set_repair after samples were pushed (call it before the first push or after wmb_reset / wmb_seek)");
+        return set_err(WMB_E_STATE, "%s after samples were pushed (call it before the first push or after wmb_reset / wmb_seek)", name);
+    return WMB_OK;
+}
+
+extern "C" int wmb_set_repair(wmb_ctx *c, uint32_t e_max)
+{
+    TRY(repair_setter_check(c, "wmb_set_repair", false, "wmb_frame_repair_device", "e_max", e_max, K4R_MAX_ERASURES));
     c->repair_e = e_max;
     return WMB_OK;
 }
@@ -2978,31 +2983,21 @@ extern "C" int wmb_set_soft_bits(wmb_ctx *c, int on)
 {
     if (!c) return set_err(WMB_E_INVAL, "null argument");
     if (on != 0 && on != 1) return set_err(WMB_E_INVAL, "soft bits %d: 0 (off) or 1 (on)", on);
-    if (!c->manual) return set_err(WMB_E_INVAL, "wmb_set_soft_bits needs a manual_frames context (the streaming framer's soft repair: wmb_set_repair_soft)");
-    if (c->batch_no != 0 || !c->remainder.empty())
-        return set_err(WMB_E_STATE, "wmb_set_soft_bits after samples were pushed (call it before the first push or after wmb_reset / wmb_seek)");
+    TRY(repair_setter_check(c, "wmb_set_soft_bits", true, "soft repair: wmb_set_repair_soft", nullptr, 0, 0));
     c->soft = on != 0;
     return WMB_OK;
 }
 
 extern "C" int wmb_set_repair_soft(wmb_ctx *c, uint32_t k_max)
 {
-    if (!c) return set_err(WMB_E_INVAL, "null argument");
-    if (c->manual) return set_err(WMB_E_INVAL, "wmb_set_repair_soft on a manual_frames context (repair the polled frames with wmb_frame_repair_soft_device)");
-    if (k_max > WMB_SOFT_K_MAX) return set_err(WMB_E_INVAL, "k_max %u out of range 0 (off) .. %d", k_max, WMB_SOFT_K_MAX);
-    if (c->batch_no != 0 || !c->remainder.empty())
-        return set_err(WMB_E_STATE, "wmb_set_repair_soft after samples were pushed (call it before the first push or after wmb_reset / wmb_seek)");
+    TRY(repair_setter_check(c, "wmb_set_repair_soft", false, "wmb_frame_repair_soft_device", "k_max", k_max, WMB_SOFT_K_MAX));
     c->repair_k = k_max;
     return WMB_OK;
 }
 
 extern "C" int wmb_set_repair_t1_soft(wmb_ctx *c, uint32_t s_max)
 {
-    if (!c) return set_err(WMB_E_INVAL, "null argument");
-    if (c->manual) return set_err(WMB_E_INVAL, "wmb_set_repair_t1_soft on a manual_frames context (repair the polled frames with wmb_frame_repair_t1_soft_device)");
-    if (s_max > WMB_SOFT_K_MAX) return set_err(WMB_E_INVAL, "s_max %u out of range 0 (off) .. %d", s_max, WMB_SOFT_K_MAX);
-    if (c->batch_no != 0 || !c->remainder.empty())
-        return set_err(WMB_E_STATE, "wmb_set_repair_t1_soft after samples were pushed (call it before the first push or after wmb_reset / wmb_seek)");
+    TRY(repair_setter_check(c, "wmb_set_repair_t1_soft", false, "wmb_frame_repair_t1_soft_device", "s_max", s_max, WMB_SOFT_K_MAX));
     c->repair_s = s_max;
     return WMB_OK;
 }
@@ -3011,20 +3006,14 @@ extern "C" int wmb_set_soft_bits_s1(wmb_ctx *c, int on)
 {
     if (!c) return set_err(WMB_E_INVAL, "null argument");
     if (on != 0 && on != 1) return set_err(WMB_E_INVAL, "S1 soft bits %d: 0 (off) or 1 (on)", on);
-    if (!c->manual) return set_err(WMB_E_INVAL, "wmb_set_soft_bits_s1 needs a manual_frames context (the streaming framer's S1 soft repair: wmb_set_repair_s1_soft)");
-    if (c->batch_no != 0 || !c->remainder.empty())
-        return set_err(WMB_E_STATE, "wmb_set_soft_bits_s1 after samples were pushed (call it before the first push or after wmb_reset / wmb_seek)");
+    TRY(repair_setter_check(c, "wmb_set_soft_bits_s1", true, "S1 soft repair: wmb_set_repair_s1_soft", nullptr, 0, 0));
     c->soft_s1 = on != 0;
     return WMB_OK;
 }
 
 extern "C" int wmb_set_repair_s1_soft(wmb_ctx *c, uint32_t s_max)
 {
-    if (!c) return set_err(WMB_E_INVAL, "null argument");
-    if (c->manual) return set_err(WMB_E_INVAL, "wmb_set_repair_s1_soft on a manual_frames context (repair the polled frames with wmb_frame_repair_s1_soft_device)");
-    if (s_max > WMB_SOFT_K_MAX) return set_err(WMB_E_INVAL, "s_max %u out of range 0 (off) .. %d", s_max, WMB_SOFT_K_MAX);
-    if (c->batch_no != 0 || !c->remainder.empty())
-        return set_err(WMB_E_STATE, "wmb_set_repair_s1_soft after samples were pushed (call it before the first push or after wmb_reset / wmb_seek)");
+    TRY(repair_setter_check(c, "wmb_set_repair_s1_soft", false, "wmb_frame_repair_s1_soft_device", "s_max", s_max, WMB_SOFT_K_MAX));
     c->repair_s1 = s_max;
     return WMB_OK;
 }

@@ -387,271 +387,196 @@ int wmb_frame_repair(const wmb_frame *f, uint32_t e_max, wmb_repaired *out)
     return WMB_OK;
 }
 
-/* ---- C1 soft repair (definition in wmbus_b200_framer.h; device twin: K4S, wmb_kernels.cuh) ------------------------ */
+/* ---- soft repair of C1, T1 and S1 (definitions in wmbus_b200_framer.h; device twin: K4S, wmb_kernels.cuh) ------------ */
 
-/* a before b in the search order: a bit without a value first, then lower r, then lower index */
-static int soft_before(int sa, int64_t ra, unsigned ja, int sb, int64_t rb, unsigned jb)
+/* One searchable unit: a C1 bit, a T1 symbol or an S1 pair.  Unit i of a code with W units per byte lies in byte i / W;
+ * its value is (pkt[byte] >> shift) & mask. */
+typedef struct soft_unit {
+    uint64_t key;                /* the rule's search order as one integer, packed as K4S packs it: unique, lowest first */
+    uint16_t byte;
+    uint8_t  shift, mask;
+    uint8_t  hard, ml, flip;     /* hard value (0xFF: invalid), ML value, ML ^ the alternative */
+} soft_unit;
+
+static __thread soft_unit g_units[8 * 292];
+
+/* the centring of the soft values of chips [j0, P): y = v 2 n0 n1 - (S1 n0 + S0 n1), or v when one side is empty */
+static void centring(const wmb_frame *f, const int16_t *soft, unsigned j0, unsigned P, int64_t *a, int64_t *t)
 {
-    if (sa != sb) return sa < sb;
-    if (ra != rb) return ra < rb;
-    return ja < jb;
-}
-
-static void repair_soft_c1(const wmb_frame *f, const int16_t *soft, uint32_t k_max, wmb_repaired *out)
-{
-    const wmb_bit *b = f->bits;
-    out->had_line = 1;
-    out->outcome = WMB_REP_UNREPAIRABLE;
-    const int bframe = bits_at(b, 1, 12) == 0x543u;
-    const unsigned L = bits_at(b, 17, 8);
-    const unsigned len = bframe ? 1 + L : wmb_tlg_length_format_a(L);
-    const unsigned P = 17 + 8 * len;
-    if (len < 12) return;
-
-    uint8_t pkt[292];
-    memset(pkt, 0, sizeof(pkt));
-    for (unsigned l = 0; l < len; l++) pkt[l] = (uint8_t)bits_at(b, 17 + 8 * l, 8);
     int64_t n0 = 0, n1 = 0, s0 = 0, s1 = 0;
-    for (unsigned j = 17; j < P; j++) {
+    for (unsigned j = j0; j < P; j++) {
         if (soft[j] == WMB_SOFT_NONE) continue;
-        if (WMB_BIT_DATA(b[j])) { n1++; s1 += soft[j]; } else { n0++; s0 += soft[j]; }
+        if (WMB_BIT_DATA(f->bits[j])) { n1++; s1 += soft[j]; } else { n0++; s0 += soft[j]; }
     }
-    /* r of bit j; has[j] = 0 for a bit without a value */
-    static __thread int64_t r[8 * 292];
-    static __thread int has[8 * 292];
-    for (unsigned j = 17; j < P; j++) {
-        const int64_t sign = WMB_BIT_DATA(b[j]) ? 1 : -1, v = soft[j];
-        has[j - 17] = soft[j] != WMB_SOFT_NONE;
-        r[j - 17] = !has[j - 17] ? 0 : n0 * n1 == 0 ? sign * v : sign * (v * 2 * n0 * n1 - (s1 * n0 + s0 * n1));
-    }
-
-    const unsigned nblk = bframe ? wmb_nblk_b(len) : wmb_nblk_a(len);
-    unsigned flips = 0, blocks = 0;
-    for (unsigned k = 0; k < nblk; k++) {
-        const unsigned off = bframe ? wmb_blk_off_b(k) : wmb_blk_off_a(k), blk = bframe ? wmb_blk_len_b(len, k) : wmb_blk_len_a(len, k);
-        if (block_ok(pkt + off, blk)) continue;
-        /* the K least reliable flippable bits, by selection */
-        const unsigned lo = 17 + 8 * (off ? off : 1), hi = 17 + 8 * (off + blk);
-        const unsigned K = k_max < hi - lo ? k_max : hi - lo;
-        unsigned sel[WMB_SOFT_K_MAX];
-        for (unsigned t = 0; t < K; t++) {
-            int found = 0;
-            for (unsigned j = lo; j < hi; j++) {
-                int taken = 0;
-                for (unsigned u = 0; u < t; u++) taken |= sel[u] == j;
-                if (taken) continue;
-                if (!found || soft_before(has[j - 17], r[j - 17], j, has[sel[t] - 17], r[sel[t] - 17], sel[t])) { sel[t] = j; found = 1; }
-            }
-        }
-        unsigned pass = 0, first = 0;
-        for (unsigned x = 1; x < (1u << K); x++) {
-            uint8_t q[128];
-            memcpy(q, pkt + off, blk);
-            for (unsigned t = 0; t < K; t++)
-                if (x >> t & 1u) q[(sel[t] - 17) / 8 - off] ^= (uint8_t)(0x80u >> ((sel[t] - 17) % 8));
-            if (block_ok(q, blk)) { if (!pass) first = x; pass++; }
-        }
-        if (pass != 1) { out->outcome = pass ? WMB_REP_AMBIGUOUS : WMB_REP_UNREPAIRABLE; return; }
-        for (unsigned t = 0; t < K; t++)
-            if (first >> t & 1u) { pkt[(sel[t] - 17) / 8] ^= (uint8_t)(0x80u >> ((sel[t] - 17) % 8)); flips++; }
-        blocks++;
-    }
-    const cursor c = { f, P - 1, 0 };
-    finish(&c, &out->line, "C1", pkt, len, bframe, 0);
-    out->outcome = WMB_REP_REPAIRED;
-    out->erasures = flips;
-    out->blocks = blocks;
+    *a = 2 * n0 * n1;
+    *t = s1 * n0 + s0 * n1;
 }
 
-int wmb_frame_repair_soft(const wmb_frame *f, const int16_t *soft, uint32_t e_max, uint32_t k_max, wmb_repaired *out)
+/* C1 bit i = 8 l + k is frame bit 17 + i; key (has a value, r, 17 + i): |r| < 2^38 */
+static void units_c1(const wmb_frame *f, const int16_t *soft, unsigned len, soft_unit *u)
 {
-    if (k_max > WMB_SOFT_K_MAX || e_max > REP_MAX_ERASURES) { memset(out, 0, sizeof(*out)); return WMB_E_INVAL; }
-    if (k_max && soft && f->nbits && f->chain == WMB_CHAIN_T1C1) {
-        wmb_decoded d;
-        wmb_frame_decode(f, &d);
-        if (d.status == WMB_DEC_LINE && !d.crc_ok && d.mode[0] == 'C') {
-            memset(out, 0, sizeof(*out));
-            repair_soft_c1(f, soft, k_max, out);
-            return WMB_OK;
-        }
+    int64_t a, t;
+    centring(f, soft, 17, 17 + 8 * len, &a, &t);
+    for (unsigned i = 8; i < 8 * len; i++) {
+        const unsigned j = 17 + i, bit = WMB_BIT_DATA(f->bits[j]);
+        const int64_t v = soft[j], r = (bit ? 1 : -1) * (a == 0 ? v : v * a - t);
+        const uint64_t key = v == WMB_SOFT_NONE ? j : (uint64_t)(r + ((int64_t)1 << 40)) << 12 | j;
+        u[i] = (soft_unit){ key, (uint16_t)(i / 8), (uint8_t)(7 - i % 8), 1, (uint8_t)bit, (uint8_t)bit, 1 };
     }
-    return wmb_frame_repair(f, e_max, out);
 }
 
-/* ---- T1 soft repair (definition in wmbus_b200_framer.h; device twin: K4S, wmb_kernels.cuh) ------------------------ */
-
-static void repair_soft_t1(const wmb_frame *f, const int16_t *soft, uint32_t s_max, wmb_repaired *out)
+/* T1 symbol i = 2 l + s (the high nibble first), chips 1 + 6 i ..; key (all chips have values, delta, i): delta < 2^43 */
+static void units_t1(const wmb_frame *f, const int16_t *soft, unsigned len, soft_unit *u)
 {
-    const wmb_bit *b = f->bits;
-    const unsigned L = (nibble_3of6(bits_at(b, 1, 6)) << 4) | nibble_3of6(bits_at(b, 7, 6));
-    const unsigned len = wmb_tlg_length_format_a(L), P = 1 + 12 * len, nsym = 2 * len;
-    int64_t n0 = 0, n1 = 0, s0 = 0, s1 = 0;
-    for (unsigned j = 13; j < P; j++) {
-        if (soft[j] == WMB_SOFT_NONE) continue;
-        if (WMB_BIT_DATA(b[j])) { n1++; s1 += soft[j]; } else { n0++; s0 += soft[j]; }
-    }
-    /* per symbol i (byte i / 2, the high nibble first): hard nibble (0xFF invalid), ML, runner-up, delta, has values */
-    static __thread uint8_t hard[2 * 292], ml[2 * 292], ru[2 * 292];
-    static __thread int64_t delta[2 * 292];
-    static __thread int has[2 * 292];
-    for (unsigned i = 2; i < nsym; i++) {
-        int64_t y[6];
-        has[i] = 1;
+    int64_t a, t;
+    centring(f, soft, 13, 1 + 12 * len, &a, &t);
+    for (unsigned i = 2; i < 2 * len; i++) {
+        int64_t y[6], delta;
+        uint64_t has = 1;
         for (unsigned c = 0; c < 6; c++) {
-            const unsigned j = 1 + 6 * i + c;
-            const int64_t v = soft[j];
-            if (soft[j] == WMB_SOFT_NONE) { has[i] = 0; y[c] = 0; }
-            else y[c] = n0 * n1 == 0 ? v : v * 2 * n0 * n1 - (s1 * n0 + s0 * n1);
+            const int64_t v = soft[1 + 6 * i + c];
+            if (v == WMB_SOFT_NONE) has = 0;
+            y[c] = v == WMB_SOFT_NONE ? 0 : a == 0 ? v : v * a - t;
         }
-        uint32_t m, r;
-        wmb_t1_sym_ml(y, &m, &r, &delta[i]);
-        ml[i] = (uint8_t)m; ru[i] = (uint8_t)r;
-        hard[i] = nibble_3of6(bits_at(b, 1 + 6 * i, 6));
+        uint32_t ml, ru;
+        wmb_t1_sym_ml(y, &ml, &ru, &delta);
+        u[i] = (soft_unit){ has << 53 | (uint64_t)delta << 10 | i, (uint16_t)(i / 2), (uint8_t)(i & 1u ? 0 : 4), 15,
+                            nibble_3of6(bits_at(f->bits, 1 + 6 * i, 6)), (uint8_t)ml, (uint8_t)(ml ^ ru) };
     }
+}
 
+/* S1 pair p = 8 l + k, chips 1 + 2 p and 2 + 2 p; key wmb_s1_pair's */
+static void units_s1(const wmb_frame *f, const int16_t *soft, unsigned len, soft_unit *u)
+{
+    for (unsigned p = 8; p < 8 * len; p++) {
+        const unsigned a = WMB_BIT_DATA(f->bits[1 + 2 * p]), c = WMB_BIT_DATA(f->bits[2 + 2 * p]);
+        uint32_t ml;
+        const uint32_t key = wmb_s1_pair(soft[1 + 2 * p], soft[2 + 2 * p], a, c, p, &ml);
+        u[p] = (soft_unit){ key, (uint16_t)(p / 8), (uint8_t)(7 - p % 8), 1, (uint8_t)(a != c ? c : 0xFFu), (uint8_t)ml, 1 };
+    }
+}
+
+/* The block search of the three rules over the units u[W .. W len) of a telegram with L-field L, whose list ends at
+ * P - 1: per block, in frame order, the block's searchable units take their ML values, the K = min(k_max, units)
+ * lowest keys are chosen, and exactly one of the 2^K patterns of alternatives must pass the block's CRC.
+ *   - Pattern 0 is tried for C1 too: a C1 unit's ML value is its hard bit, so pattern 0 is the received block, which
+ *     failed its CRC.
+ *   - erasures counts the units whose final value differs from the hard one; for C1 that is the number of flipped bits
+ *     (ML = hard), at most 6 per block and 17 blocks, below the device record's byte.
+ *   - A frame B block is up to 128 bytes long, hence the trial buffer's size. */
+static void soft_search(const wmb_frame *f, const soft_unit *u, unsigned W, unsigned L, unsigned len, int bframe,
+                        unsigned P, uint32_t k_max, const char *mode, wmb_repaired *out)
+{
     uint8_t pkt[292];
     memset(pkt, 0, sizeof(pkt));
     pkt[0] = (uint8_t)L;
-    for (unsigned l = 1; l < len; l++) pkt[l] = (uint8_t)(((hard[2 * l] & 15u) << 4) | (hard[2 * l + 1] & 15u));
+    for (unsigned i = W; i < W * len; i++)
+        if (u[i].hard != 0xFFu) pkt[u[i].byte] |= (uint8_t)(u[i].hard << u[i].shift);
+    const unsigned nblk = bframe ? wmb_nblk_b(len) : wmb_nblk_a(len);
     unsigned changed = 0, blocks = 0;
-    for (unsigned k = 0; k < wmb_nblk_a(len); k++) {
-        const unsigned off = wmb_blk_off_a(k), blk = wmb_blk_len_a(len, k);
-        const unsigned lo = 2 * (off ? off : 1), hi = 2 * (off + blk);    /* the block's searchable symbols */
+    for (unsigned k = 0; k < nblk; k++) {
+        const unsigned off = bframe ? wmb_blk_off_b(k) : wmb_blk_off_a(k), blk = bframe ? wmb_blk_len_b(len, k) : wmb_blk_len_a(len, k);
+        const unsigned lo = W * (off ? off : 1), hi = W * (off + blk);        /* the block's searchable units */
         int valid = 1;
-        for (unsigned i = lo; i < hi; i++) valid &= hard[i] != 0xFFu;
+        for (unsigned i = lo; i < hi; i++) valid &= u[i].hard != 0xFFu;
         if (valid && block_ok(pkt + off, blk)) continue;
-        for (unsigned i = lo; i < hi; i++) pkt[i / 2] = (uint8_t)(i & 1u ? (pkt[i / 2] & 0xF0u) | ml[i] : (pkt[i / 2] & 0x0Fu) | ml[i] << 4);
-        /* the K symbols of lowest delta, by selection (a symbol with a chip without a value first, ties: lower index) */
-        const unsigned K = s_max < hi - lo ? s_max : hi - lo;
+        for (unsigned i = lo; i < hi; i++)
+            pkt[u[i].byte] = (uint8_t)((pkt[u[i].byte] & ~(u[i].mask << u[i].shift)) | u[i].ml << u[i].shift);
+        /* the K units of lowest key, by selection */
+        const unsigned K = k_max < hi - lo ? k_max : hi - lo;
         unsigned sel[WMB_SOFT_K_MAX];
         for (unsigned t = 0; t < K; t++) {
-            int found = 0;
-            for (unsigned i = lo; i < hi; i++) {
-                int taken = 0;
-                for (unsigned u = 0; u < t; u++) taken |= sel[u] == i;
-                if (taken) continue;
-                if (!found || soft_before(has[i], delta[i], i, has[sel[t]], delta[sel[t]], sel[t])) { sel[t] = i; found = 1; }
-            }
+            uint64_t best = UINT64_MAX;
+            for (unsigned i = lo; i < hi; i++)
+                if (u[i].key < best && (t == 0 || u[i].key > u[sel[t - 1]].key)) { best = u[i].key; sel[t] = i; }
         }
         unsigned pass = 0, first = 0;
         for (unsigned x = 0; x < (1u << K); x++) {
-            uint8_t q[18];
+            uint8_t q[128];
             memcpy(q, pkt + off, blk);
             for (unsigned t = 0; t < K; t++)
-                if (x >> t & 1u) q[sel[t] / 2 - off] ^= (uint8_t)((ml[sel[t]] ^ ru[sel[t]]) << (sel[t] & 1u ? 0 : 4));
+                if (x >> t & 1u) q[u[sel[t]].byte - off] ^= (uint8_t)(u[sel[t]].flip << u[sel[t]].shift);
             if (block_ok(q, blk)) { if (!pass) first = x; pass++; }
         }
         if (pass != 1) { out->outcome = pass ? WMB_REP_AMBIGUOUS : WMB_REP_UNREPAIRABLE; return; }
         for (unsigned t = 0; t < K; t++)
-            if (first >> t & 1u) pkt[sel[t] / 2] ^= (uint8_t)((ml[sel[t]] ^ ru[sel[t]]) << (sel[t] & 1u ? 0 : 4));
-        for (unsigned i = lo; i < hi; i++) changed += hard[i] != (i & 1u ? pkt[i / 2] & 15u : pkt[i / 2] >> 4);
+            if (first >> t & 1u) pkt[u[sel[t]].byte] ^= (uint8_t)(u[sel[t]].flip << u[sel[t]].shift);
+        for (unsigned i = lo; i < hi; i++) changed += u[i].hard != (pkt[u[i].byte] >> u[i].shift & u[i].mask);
         blocks++;
     }
     const cursor c = { f, P - 1, 0 };
-    finish(&c, &out->line, "T1", pkt, len, 0, 0);
+    finish(&c, &out->line, mode, pkt, len, bframe, 0);
     out->outcome = WMB_REP_REPAIRED;
     out->erasures = changed < 255 ? changed : 255;         /* the device record's byte */
     out->blocks = blocks;
+}
+
+/* a T1 / C1 line (mode[0] == m) whose CRCs fail */
+static int crc_failed_line(const wmb_frame *f, char m)
+{
+    wmb_decoded d;
+    wmb_frame_decode(f, &d);
+    return d.status == WMB_DEC_LINE && !d.crc_ok && d.mode[0] == m;
+}
+
+/* the soft rules' own condition: len >= 12 and no rssi drop before P - 1 (a line has none) */
+static int soft_candidate(const wmb_frame *f, unsigned len, unsigned P)
+{
+    if (len < 12) return 0;
+    for (unsigned i = 0; i + 1 < P; i++)
+        if (WMB_BIT_RSSI(f->bits[i]) < CAPTURE_THRESHOLD) return 0;
+    return 1;
+}
+
+/* C1: a line with CRC errors, before the erasure rule (which finds it UNREPAIRABLE) */
+int wmb_frame_repair_soft(const wmb_frame *f, const int16_t *soft, uint32_t e_max, uint32_t k_max, wmb_repaired *out)
+{
+    if (k_max > WMB_SOFT_K_MAX || e_max > REP_MAX_ERASURES) { memset(out, 0, sizeof(*out)); return WMB_E_INVAL; }
+    if (!k_max || !soft || !f->nbits || f->chain != WMB_CHAIN_T1C1 || !crc_failed_line(f, 'C'))
+        return wmb_frame_repair(f, e_max, out);
+    memset(out, 0, sizeof(*out));
+    out->had_line = 1;
+    out->outcome = WMB_REP_UNREPAIRABLE;
+    const int bframe = bits_at(f->bits, 1, 12) == 0x543u;
+    const unsigned L = bits_at(f->bits, 17, 8), len = bframe ? 1 + L : wmb_tlg_length_format_a(L), P = 17 + 8 * len;
+    if (!soft_candidate(f, len, P)) return WMB_OK;
+    units_c1(f, soft, len, g_units);
+    soft_search(f, g_units, 8, L, len, bframe, P, k_max, "C1", out);
+    return WMB_OK;
+}
+
+/* T1 and S1: a candidate the erasure rule ends TOO_MANY or UNREPAIRABLE (T1: a line with CRC errors; S1: also a violation
+ * abort), whose had_line stays; UNREPAIRABLE also stands for len < 12 and an rssi drop, which stay so */
+static int repair_soft_after_erasures(const wmb_frame *f, const int16_t *soft, uint32_t e_max, uint32_t s_max, int chain,
+                                      wmb_repaired *out)
+{
+    if (s_max > WMB_SOFT_K_MAX || e_max > REP_MAX_ERASURES) { memset(out, 0, sizeof(*out)); return WMB_E_INVAL; }
+    const int rc = wmb_frame_repair(f, e_max, out);
+    if (rc || !s_max || !soft || f->chain != chain) return rc;
+    if (out->outcome != WMB_REP_TOO_MANY && out->outcome != WMB_REP_UNREPAIRABLE) return rc;
+    const int t1 = chain == WMB_CHAIN_T1C1;
+    if (t1 && !crc_failed_line(f, 'T')) return rc;
+    unsigned L = 0;
+    if (t1) L = (nibble_3of6(bits_at(f->bits, 1, 6)) << 4) | nibble_3of6(bits_at(f->bits, 7, 6));
+    else for (unsigned k = 0; k < 8; k++) L = (L << 1) | WMB_BIT_DATA(f->bits[2 + 2 * k]);
+    const unsigned len = wmb_tlg_length_format_a(L), P = 1 + (t1 ? 12u : 16u) * len;
+    if (!soft_candidate(f, len, P)) return rc;
+    const uint32_t had_line = out->had_line;
+    memset(out, 0, sizeof(*out));
+    out->had_line = had_line;
+    (t1 ? units_t1 : units_s1)(f, soft, len, g_units);
+    soft_search(f, g_units, t1 ? 2 : 8, L, len, 0, P, s_max, t1 ? "T1" : "S1", out);
+    return WMB_OK;
 }
 
 int wmb_frame_repair_t1_soft(const wmb_frame *f, const int16_t *soft, uint32_t e_max, uint32_t s_max, wmb_repaired *out)
 {
-    if (s_max > WMB_SOFT_K_MAX || e_max > REP_MAX_ERASURES) { memset(out, 0, sizeof(*out)); return WMB_E_INVAL; }
-    const int rc = wmb_frame_repair(f, e_max, out);
-    if (rc || !s_max || !soft || f->chain != WMB_CHAIN_T1C1) return rc;
-    if (out->outcome != WMB_REP_TOO_MANY && out->outcome != WMB_REP_UNREPAIRABLE) return rc;
-    wmb_decoded d;
-    wmb_frame_decode(f, &d);
-    if (d.status != WMB_DEC_LINE || d.crc_ok || d.mode[0] != 'T') return rc;
-    /* a line reaches P and has no rssi drop before P - 1; len >= 12 is the rule's own */
-    const unsigned L = (nibble_3of6(bits_at(f->bits, 1, 6)) << 4) | nibble_3of6(bits_at(f->bits, 7, 6));
-    if (wmb_tlg_length_format_a(L) < 12) return rc;
-    memset(out, 0, sizeof(*out));
-    out->had_line = 1;
-    repair_soft_t1(f, soft, s_max, out);
-    return WMB_OK;
-}
-
-/* ---- S1 soft repair (definition in wmbus_b200_framer.h; device twin: K4S, wmb_kernels.cuh) ------------------------ */
-
-static unsigned s1_bit(const uint8_t *pkt, unsigned p) { return pkt[p / 8] >> (7 - p % 8) & 1u; }
-
-static void repair_soft_s1(const wmb_frame *f, const int16_t *soft, unsigned L, uint32_t s_max, wmb_repaired *out)
-{
-    const wmb_bit *b = f->bits;
-    const unsigned len = wmb_tlg_length_format_a(L), npair = 8 * len;
-    /* per pair p = 8 l + bit: hard bit (2: a violation), ML bit, search key */
-    static __thread uint8_t hard[8 * 292], ml[8 * 292];
-    static __thread uint32_t key[8 * 292];
-    for (unsigned p = 8; p < npair; p++) {
-        const unsigned a = WMB_BIT_DATA(b[1 + 2 * p]), c = WMB_BIT_DATA(b[2 + 2 * p]);
-        uint32_t m;
-        key[p] = wmb_s1_pair(soft[1 + 2 * p], soft[2 + 2 * p], a, c, p, &m);
-        ml[p] = (uint8_t)m;
-        hard[p] = (uint8_t)(a != c ? c : 2u);
-    }
-
-    uint8_t pkt[292];
-    memset(pkt, 0, sizeof(pkt));
-    pkt[0] = (uint8_t)L;
-    for (unsigned p = 8; p < npair; p++) pkt[p / 8] |= (uint8_t)((hard[p] & 1u) << (7 - p % 8));
-    unsigned changed = 0, blocks = 0;
-    for (unsigned k = 0; k < wmb_nblk_a(len); k++) {
-        const unsigned off = wmb_blk_off_a(k), blk = wmb_blk_len_a(len, k);
-        const unsigned lo = 8 * (off ? off : 1), hi = 8 * (off + blk);    /* the block's searchable pairs */
-        int valid = 1;
-        for (unsigned p = lo; p < hi; p++) valid &= hard[p] != 2u;
-        if (valid && block_ok(pkt + off, blk)) continue;
-        for (unsigned p = lo; p < hi; p++) pkt[p / 8] = (uint8_t)((pkt[p / 8] & ~(0x80u >> p % 8)) | ml[p] << (7 - p % 8));
-        /* the K pairs of lowest key, by selection (keys are unique) */
-        const unsigned K = s_max < hi - lo ? s_max : hi - lo;
-        unsigned sel[WMB_SOFT_K_MAX];
-        for (unsigned t = 0; t < K; t++) {
-            uint32_t best = 0xFFFFFFFFu;
-            for (unsigned p = lo; p < hi; p++)
-                if (key[p] < best && (t == 0 || key[p] > key[sel[t - 1]])) { best = key[p]; sel[t] = p; }
-        }
-        unsigned pass = 0, first = 0;
-        for (unsigned x = 0; x < (1u << K); x++) {
-            uint8_t q[18];
-            memcpy(q, pkt + off, blk);
-            for (unsigned t = 0; t < K; t++)
-                if (x >> t & 1u) q[sel[t] / 8 - off] ^= (uint8_t)(0x80u >> sel[t] % 8);
-            if (block_ok(q, blk)) { if (!pass) first = x; pass++; }
-        }
-        if (pass != 1) { out->outcome = pass ? WMB_REP_AMBIGUOUS : WMB_REP_UNREPAIRABLE; return; }
-        for (unsigned t = 0; t < K; t++)
-            if (first >> t & 1u) pkt[sel[t] / 8] ^= (uint8_t)(0x80u >> sel[t] % 8);
-        for (unsigned p = lo; p < hi; p++) changed += hard[p] != s1_bit(pkt, p);
-        blocks++;
-    }
-    const cursor c = { f, 16 * len, 0 };
-    finish(&c, &out->line, "S1", pkt, len, 0, 0);
-    out->outcome = WMB_REP_REPAIRED;
-    out->erasures = changed < 255 ? changed : 255;         /* the device record's byte */
-    out->blocks = blocks;
+    return repair_soft_after_erasures(f, soft, e_max, s_max, WMB_CHAIN_T1C1, out);
 }
 
 int wmb_frame_repair_s1_soft(const wmb_frame *f, const int16_t *soft, uint32_t e_max, uint32_t s_max, wmb_repaired *out)
 {
-    if (s_max > WMB_SOFT_K_MAX || e_max > REP_MAX_ERASURES) { memset(out, 0, sizeof(*out)); return WMB_E_INVAL; }
-    const int rc = wmb_frame_repair(f, e_max, out);
-    if (rc || !s_max || !soft || f->chain != WMB_CHAIN_S1) return rc;
-    /* TOO_MANY / UNREPAIRABLE: a candidate of the erasure rule (a line with crc_ok = 0 or a violation abort) whose list
-     * reaches P; UNREPAIRABLE also stands for len < 12 and an rssi drop, which stay so */
-    if (out->outcome != WMB_REP_TOO_MANY && out->outcome != WMB_REP_UNREPAIRABLE) return rc;
-    unsigned L = 0;
-    for (unsigned k = 0; k < 8; k++) L = (L << 1) | WMB_BIT_DATA(f->bits[2 + 2 * k]);
-    const unsigned len = wmb_tlg_length_format_a(L), P = 1 + 16 * len;
-    if (len < 12) return rc;
-    for (unsigned i = 0; i + 1 < P; i++)
-        if (WMB_BIT_RSSI(f->bits[i]) < CAPTURE_THRESHOLD) return rc;
-    const uint32_t had_line = out->had_line;
-    memset(out, 0, sizeof(*out));
-    out->had_line = had_line;
-    out->outcome = WMB_REP_UNREPAIRABLE;
-    repair_soft_s1(f, soft, L, s_max, out);
-    return WMB_OK;
+    return repair_soft_after_erasures(f, soft, e_max, s_max, WMB_CHAIN_S1, out);
 }
 
 /* ---- output --------------------------------------------------------------------- */
