@@ -262,6 +262,53 @@ int wmb_set_bursts(wmb_ctx *c, int chain, uint32_t level);
  * taken stay queued. */
 int wmb_take_bursts(wmb_ctx *c, wmb_burst *out, size_t cap, size_t *n);
 
+/* ---- burst snippets: the raw cu8 bytes around each burst, replayable ----------------------------------------------
+ * Off by default.  d is the decimation; a granule is 2048 decimated samples, 2048 d IQ samples, 4096 d bytes: granule g
+ * covers decimated samples [2048 g, 2048 g + 2048), and its edges are the positions wmb_seek accepts.
+ *   1. Which bursts: every piece wmb_take_bursts hands out (so snippets need wmb_set_bursts on at least one chain).
+ *   2. Bounds: the snippet of a piece [s, e) covers the granules [lo, hi),
+ *        lo = max(g_first, floor(s / 2048) - WMB_SNIPPET_PRE),  hi = min(ceil(e / 2048) + WMB_SNIPPET_POST, end),
+ *      g_first the first granule pushed since wmb_reset / wmb_seek, end the end of the input consumed (at the end of
+ *      input a last partial granule counts with the bytes consumed).  Its bytes are the input's bytes
+ *      [lo 4096 d, hi 4096 d) relative to the capture (the index wmb_seek sets), as they were pushed.
+ *   3. Decoded: the same chain has a line with CRC_OK = 1, or (repair on) a REPAIRED repair record, whose access-code
+ *      match lies in [s, e) and in the line window.  A piece is handed out once it is closed, its last granule has
+ *      been pushed (or the input ended), and no telegram of its chain matched in [s, e) is still in flight
+ *      (wmb_pending_before's condition): so `decoded` is final.  Mode 1 hands out every piece, mode 2 only those that
+ *      did not decode.
+ *   4. Replay: pushing a snippet into a fresh context with the same options and receiver, repair and burst settings,
+ *      after wmb_seek(start_iq), gives the lines of the full run (same text under timestamp_mode 1, same sync_sample)
+ *      for every line whose match lies in [s, e); it may give more (its decoders start idle).  2048 d is a multiple of
+ *      d and of the mixer's period, so the snippet pushed without a seek has the same decimation and mixer phases.
+ *   5. Device memory: the kept granules of a batch go to a pool of at most 64 MiB per result slot (4 slots, and as
+ *      much pinned host memory).  A snippet with a granule that did not fit is handed out with lost = 1 and no bytes,
+ *      and wmb_stats.overflow_batches counts its batch. */
+#define WMB_SNIPPET_PRE  2
+#define WMB_SNIPPET_POST 2
+
+typedef struct wmb_snippet {
+    uint64_t start_sample;    /* the piece, as in wmb_burst                                                  */
+    uint64_t end_sample;
+    uint64_t start_iq;        /* lo 2048 d: the IQ sample of the snippet's first byte pair (for wmb_seek)      */
+    uint64_t nbytes;          /* (hi - lo) 4096 d, less at the end of input; 0 when lost                      */
+    uint8_t  chain;           /* WMB_CHAIN_*                                                                 */
+    uint8_t  decoded;         /* 1: a CRC-ok or repaired telegram matched in the piece (point 3)              */
+    uint8_t  flags;           /* WMB_BURST_*                                                                 */
+    uint8_t  lost;            /* 1: a granule did not fit the device pool; no bytes                          */
+    uint32_t pad;
+} wmb_snippet;
+
+/* mode 0: off (the default), 1: every burst piece, 2: the pieces that did not decode.  A mode outside 0..2 gives
+ * WMB_E_INVAL (checked first); valid before the first push or right after wmb_reset / wmb_seek (else WMB_E_STATE).
+ * The mode survives wmb_reset and wmb_seek.  The first push fails with WMB_E_STATE when snippets are on and no chain
+ * has the burst report on. */
+int wmb_set_snippets(wmb_ctx *c, int mode);
+
+/* Copy whole snippets in the burst order (start_sample, chain): recs[i] and its nbytes bytes, concatenated in bytes.
+ * Stops at cap records or when the next snippet's bytes do not fit bytes_cap; *n receives the number copied.  Snippets
+ * not taken stay queued. */
+int wmb_take_snippets(wmb_ctx *c, wmb_snippet *recs, size_t cap, uint8_t *bytes, size_t bytes_cap, size_t *n);
+
 /* ---- signal quality: FSK deviation, eye SNR and chip rate of each line and burst --------------------------------
  * Off by default; wmb_set_line_quality(ctx, 1) turns it on.  Over the carrier-offset window [lo, hi) of a line
  * (wmb_line_info: T1/C1 [s-384, s-128), S1 [s-1367, s-586), clipped) or of a burst (wmb_burst: [start + g0,

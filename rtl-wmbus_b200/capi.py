@@ -80,6 +80,17 @@ def burst_dtype():
     return np.dtype(BURST_FIELDS)
 
 
+# numpy mirror of wmb_snippet (one record per saved burst snippet; see include/wmbus_b200.h)
+SNIPPET_FIELDS = [("start_sample", "<u8"), ("end_sample", "<u8"), ("start_iq", "<u8"), ("nbytes", "<u8"),
+                  ("chain", "u1"), ("decoded", "u1"), ("flags", "u1"), ("lost", "u1"), ("pad", "<u4")]
+SNIPPET_PRE, SNIPPET_POST = 2, 2          # WMB_SNIPPET_PRE / WMB_SNIPPET_POST: granules before / after a piece
+
+
+def snippet_dtype():
+    import numpy as np
+    return np.dtype(SNIPPET_FIELDS)
+
+
 # numpy mirrors of wmb_line_quality and wmb_burst_quality (see include/wmbus_b200.h)
 LINE_QUALITY_FIELDS = [("sync_sample", "<u8"), ("end_sample", "<u8"), ("n_hi", "<u4"), ("n_lo", "<u4"),
                        ("s1_hi", "<i8"), ("s1_lo", "<i8"), ("s2_hi", "<u8"), ("s2_lo", "<u8"), ("bits", "<u4"),
@@ -169,6 +180,8 @@ def _bind(lib):
     lib.wmb_set_bursts.argtypes = [C.c_void_p, C.c_int, C.c_uint32]
     lib.wmb_take_bursts.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
     lib.wmb_set_line_quality.argtypes = [C.c_void_p, C.c_int]
+    lib.wmb_set_snippets.argtypes = [C.c_void_p, C.c_int]
+    lib.wmb_take_snippets.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
     lib.wmb_take_lines_quality.argtypes = [C.c_void_p, C.c_char_p, C.c_size_t, C.POINTER(C.c_size_t), C.c_int,
                                            C.c_void_p, C.c_void_p, C.c_size_t]
     lib.wmb_take_lines_quality.restype = C.c_size_t
@@ -207,7 +220,8 @@ EXPORTS = ["wmb_reset", "wmb_host_alloc", "wmb_host_free", "wmb_default_opts", "
            "wmb_process", "wmb_process_device", "wmb_get_stats", "wmb_debug_copy_stage", "wmb_debug_copy_bits", "wmb_debug_copy_events", "wmb_debug_arith",
            "wmb_seek", "wmb_set_line_window", "wmb_boundary_state", "wmb_pending_before", "wmb_set_receiver",
            "wmb_take_lines_info", "wmb_set_bursts", "wmb_take_bursts", "wmb_set_spectrum", "wmb_take_spectrum",
-           "wmb_debug_spectrum_tables", "wmb_set_line_quality", "wmb_take_lines_quality", "wmb_take_bursts_quality"]
+           "wmb_debug_spectrum_tables", "wmb_set_line_quality", "wmb_take_lines_quality", "wmb_take_bursts_quality",
+           "wmb_set_snippets", "wmb_take_snippets"]
 
 
 def load_library(path: str | None = None):
@@ -268,11 +282,14 @@ class WmbusB200:
     soft values of their chips, see wmb_set_repair_s1_soft() (0: off, the default); it survives reset() and seek().
     soft_bits=True (manual_frames=1 only): the soft value of every T1/C1 bit, see wmb_set_soft_bits() (off by default); it
     survives reset() and seek().  frame_soft() returns a polled frame's values and repair_frames(k_max=...) uses them.
-    soft_bits_s1=True (manual_frames=1 only): the soft value of every S1 chip too, see wmb_set_soft_bits_s1()."""
+    soft_bits_s1=True (manual_frames=1 only): the soft value of every S1 chip too, see wmb_set_soft_bits_s1().
+    snippets=mode: the raw bytes around each burst piece, see wmb_set_snippets() (0: off, the default; 1: every piece;
+    2: the pieces that did not decode); needs burst_level on a chain.  It survives reset() and seek().  take_snippets()
+    hands them out."""
 
     def __init__(self, flags: str = "", device: int = 0, lib=None, clock_lock=None, access_code_errors=None,
                  burst_level=None, spectrum=None, quality=False, repair=0, repair_soft=0, soft_bits=False,
-                 repair_t1_soft=0, repair_s1_soft=0, soft_bits_s1=False, **tuning):
+                 repair_t1_soft=0, repair_s1_soft=0, soft_bits_s1=False, snippets=0, **tuning):
         self.lib = lib or load_library()
         self.opts = opts_from_flags(self.lib, flags, **tuning)
         self._ctx = C.c_void_p()
@@ -341,6 +358,12 @@ class WmbusB200:
         if soft_bits:
             try:
                 self.set_soft_bits(True)
+            except Exception:
+                self.close()
+                raise
+        if snippets:
+            try:
+                self.set_snippets(snippets)
             except Exception:
                 self.close()
                 raise
@@ -565,6 +588,31 @@ class WmbusB200:
         if not quality:
             return b
         return b, (np.concatenate(qparts) if qparts else np.zeros(0, burst_quality_dtype()))
+
+    def set_snippets(self, mode: int):
+        """0: off, 1: every burst piece, 2: the pieces that did not decode (before the first push, or after reset/seek)"""
+        self._check(self.lib.wmb_set_snippets(self._ctx, mode))
+
+    def take_snippets(self, cap=1 << 12, bytes_cap=64 << 20):
+        """the snippets ready, in burst order: (records, data), records a numpy structured array of wmb_snippet
+        (snippet_dtype()) and data a list with one bytes object per record.  bytes_cap holds any one snippet: a piece
+        spans at most 2^17 + 2^16 samples, its snippet at most 101 granules of 4096 d bytes (10 MB at d = 25)"""
+        import numpy as np
+        recs, data = [], []
+        buf = np.zeros(bytes_cap, np.uint8)
+        while True:
+            r = np.zeros(cap, snippet_dtype())
+            n = C.c_size_t(0)
+            self._check(self.lib.wmb_take_snippets(self._ctx, r.ctypes.data, cap, buf.ctypes.data, bytes_cap, C.byref(n)))
+            if n.value == 0:
+                break
+            r = r[:n.value]
+            at = 0
+            for x in r:
+                data.append(buf[at:at + int(x["nbytes"])].tobytes())
+                at += int(x["nbytes"])
+            recs.append(r)
+        return (np.concatenate(recs) if recs else np.zeros(0, snippet_dtype())), data
 
     def set_line_quality(self, on: bool):
         """signal-quality report on / off (before the first push, or after reset/seek)"""

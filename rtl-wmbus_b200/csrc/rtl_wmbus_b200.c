@@ -59,6 +59,15 @@
  *                              Manchester pairs of each failing CRC block (wmb_set_repair_s1_soft; DESIGN.md 8).  Unset: S1
  *                              is repaired from hard decisions only.  A bad value, or this variable without
  *                              WMBUS_B200_REPAIRED, is an error at start-up.  stdout does not change.
+ *   WMBUS_B200_SNIPPETS=<dir>  save the raw input around each burst piece (wmb_set_snippets, at the burst levels of
+ *                              WMBUS_B200_BURST_LEVEL): after each hand-over one file <dir>/<START_IQ, 14 digits>_<T1C1|S1>.cu8
+ *                              per snippet, and a line FILE;CHAIN;START_SAMPLE;END_SAMPLE;START_IQ;NBYTES;DECODED appended to
+ *                              <dir>/snippets.txt (FILE "-" when the snippet was lost to a full device pool).  Pieces with
+ *                              the same START_IQ share a file: the later one's snippet holds the earlier one's.  Piped back
+ *                              with the same flags, a file prints the lines of its burst (but the TIMESTAMP column).
+ *   WMBUS_B200_SNIPPET_MODE=undecoded|all   the pieces saved (default undecoded: those without a CRC-ok line).
+ *   A directory that cannot be written, a bad mode, or a mode without WMBUS_B200_SNIPPETS is an error at start-up.
+ *   stdout does not change.
  */
 #define _GNU_SOURCE
 #include <errno.h>
@@ -220,6 +229,8 @@ static void write_info(const char *out, size_t n, size_t nl, int show_algorithm)
  * every CRC-ok line inside a burst (DESIGN.md 8) */
 #define BURST_LEVEL_DEFAULT 14ul
 static FILE *g_burst_file = NULL;
+static const char *g_snip_dir /* WMBUS_B200_SNIPPETS */ = NULL;
+static FILE *g_snip_index = NULL;
 #define BURST_CAP 1024
 static wmb_burst g_bursts[BURST_CAP];
 /* WMBUS_B200_BURST_QUALITY: one record per burst piece, in the burst file's order: CHAIN;START_SAMPLE;DEVIATION_HZ;
@@ -229,7 +240,11 @@ static wmb_burst_quality g_bqual[BURST_CAP];
 
 static void emit_bursts(wmb_ctx *ctx)
 {
-    if (!g_burst_file) return;
+    if (!g_burst_file) {                                 /* on for the snippets alone: nobody reads the records */
+        size_t n = 0;
+        while (g_snip_dir && wmb_take_bursts(ctx, g_bursts, BURST_CAP, &n) == WMB_OK && n == BURST_CAP) {}
+        return;
+    }
     for (;;) {
         size_t n = 0;
         if (wmb_take_bursts_quality(ctx, g_bursts, g_bqual_file ? g_bqual : NULL, BURST_CAP, &n) != WMB_OK || !n) break;
@@ -253,6 +268,46 @@ static void emit_bursts(wmb_ctx *ctx)
     }
     fflush(g_burst_file);
     if (g_bqual_file) fflush(g_bqual_file);
+}
+
+/* WMBUS_B200_SNIPPETS: one cu8 file per snippet and a line per snippet in the directory's index */
+#define SNIP_CAP 256
+#define SNIP_BYTES (32u << 20)                          /* > any one snippet: 101 granules of 4096 x 25 bytes */
+static wmb_snippet g_snips[SNIP_CAP];
+static uint8_t *g_snip_bytes = NULL;
+
+static int emit_snippets(wmb_ctx *ctx)
+{
+    if (!g_snip_dir) return 0;
+    for (;;) {
+        size_t n = 0;
+        if (wmb_take_snippets(ctx, g_snips, SNIP_CAP, g_snip_bytes, SNIP_BYTES, &n) != WMB_OK) {
+            fprintf(stderr, "rtl_wmbus_b200: %s\n", wmb_last_error());
+            return -1;
+        }
+        if (!n) break;
+        size_t at = 0;
+        for (size_t i = 0; i < n; i++) {
+            const wmb_snippet *q = &g_snips[i];
+            const char *chain = q->chain == WMB_CHAIN_T1C1 ? "T1C1" : "S1";
+            char name[64] = "-";
+            if (!q->lost) {
+                snprintf(name, sizeof(name), "%014llu_%s.cu8", (unsigned long long)q->start_iq, chain);
+                char path[4096];
+                snprintf(path, sizeof(path), "%s/%s", g_snip_dir, name);
+                FILE *f = fopen(path, "wb");
+                if (!f || fwrite(g_snip_bytes + at, 1, q->nbytes, f) != q->nbytes || fclose(f) != 0) {
+                    fprintf(stderr, "rtl_wmbus_b200: WMBUS_B200_SNIPPETS: %s: %s\n", path, strerror(errno));
+                    return -1;
+                }
+                at += q->nbytes;
+            }
+            fprintf(g_snip_index, "%s;%s;%llu;%llu;%llu;%llu;%u\n", name, chain, (unsigned long long)q->start_sample,
+                    (unsigned long long)q->end_sample, (unsigned long long)q->start_iq, (unsigned long long)q->nbytes,
+                    q->decoded);
+        }
+    }
+    return fflush(g_snip_index) == 0 ? 0 : -1;
 }
 
 /* WMBUS_B200_SPECTRUM: a mean line and a peak line per closed record of the band survey */
@@ -311,6 +366,7 @@ static void emit_repairs(wmb_ctx *ctx, const char *ts, int show_algorithm)
 
 static int emit_lines(wmb_ctx *ctx, char *out, size_t outcap, int show_algorithm)
 {
+    if (emit_snippets(ctx)) return -1;
     emit_bursts(ctx);
     emit_spectrum(ctx);
     /* the repaired lines carry the hand-over's wall-clock time, taken as its stdout lines are formatted */
@@ -460,6 +516,33 @@ int main(int argc, char *argv[])
         }
     }
 
+    int snip_mode = 0;
+    if ((e = getenv("WMBUS_B200_SNIPPET_MODE")) != NULL) {
+        if (strcmp(e, "undecoded") == 0) snip_mode = 2;
+        else if (strcmp(e, "all") == 0) snip_mode = 1;
+        else {
+            fprintf(stderr, "rtl_wmbus_b200: WMBUS_B200_SNIPPET_MODE=%s: expected undecoded or all\n", e);
+            return EXIT_FAILURE;
+        }
+        if (!getenv("WMBUS_B200_SNIPPETS")) {
+            fprintf(stderr, "rtl_wmbus_b200: WMBUS_B200_SNIPPET_MODE needs WMBUS_B200_SNIPPETS\n");
+            return EXIT_FAILURE;
+        }
+    }
+    if ((g_snip_dir = getenv("WMBUS_B200_SNIPPETS")) != NULL) {
+        char path[4096];
+        snprintf(path, sizeof(path), "%s/snippets.txt", g_snip_dir);
+        if ((g_snip_index = fopen(path, "a")) == NULL) {
+            fprintf(stderr, "rtl_wmbus_b200: WMBUS_B200_SNIPPETS=%s: %s\n", g_snip_dir, strerror(errno));
+            return EXIT_FAILURE;
+        }
+        if (!snip_mode) snip_mode = 2;
+        if ((g_snip_bytes = malloc(SNIP_BYTES)) == NULL) {
+            fprintf(stderr, "rtl_wmbus_b200: out of memory\n");
+            return EXIT_FAILURE;
+        }
+    }
+
     unsigned long repair_e = 1, repair_k = 0, repair_s = 0, repair_s1 = 0;
     if (repair_setting("WMBUS_B200_REPAIR_ERASURES", 3, "1, 2 or 3", &repair_e) ||
         repair_setting("WMBUS_B200_REPAIR_SOFT_BITS", WMB_SOFT_K_MAX, "1 .. " SOFT_K_MAX_STR, &repair_k) ||
@@ -481,7 +564,7 @@ int main(int argc, char *argv[])
             fprintf(stderr, "rtl_wmbus_b200: %s\n", wmb_last_error());
             return EXIT_FAILURE;
         }
-    if (g_burst_file)
+    if (g_burst_file || g_snip_dir)
         for (int ch = 0; ch < 2; ch++)
             if (wmb_set_bursts(ctx, ch, (uint32_t)burst_level[ch]) != WMB_OK) {
                 fprintf(stderr, "rtl_wmbus_b200: %s\n", wmb_last_error());
@@ -494,6 +577,10 @@ int main(int argc, char *argv[])
     if (g_rep_file && (wmb_set_repair(ctx, (uint32_t)repair_e) != WMB_OK || wmb_set_repair_soft(ctx, (uint32_t)repair_k) != WMB_OK ||
                        wmb_set_repair_t1_soft(ctx, (uint32_t)repair_s) != WMB_OK ||
                        wmb_set_repair_s1_soft(ctx, (uint32_t)repair_s1) != WMB_OK)) {
+        fprintf(stderr, "rtl_wmbus_b200: %s\n", wmb_last_error());
+        return EXIT_FAILURE;
+    }
+    if (g_snip_dir && wmb_set_snippets(ctx, snip_mode) != WMB_OK) {
         fprintf(stderr, "rtl_wmbus_b200: %s\n", wmb_last_error());
         return EXIT_FAILURE;
     }
@@ -547,13 +634,13 @@ int main(int argc, char *argv[])
                 set_alarm(0);
                 const double t_in = now_s();
                 rc = wmb_push(ctx, buf, fill);
-                if (rc == WMB_OK) emit_lines(ctx, out, outcap, o.show_algorithm);
+                if (rc == WMB_OK && emit_lines(ctx, out, outcap, o.show_algorithm)) rc = WMB_E_STATE;
                 deadline += now_s() - t_in;             /* the item's two seconds do not run during the hand-over */
                 const double left = deadline - now_s();
                 set_alarm(left > 1e-3 ? left : 1e-3);
             } else {
                 rc = wmb_push(ctx, buf, fill);
-                if (rc == WMB_OK) emit_lines(ctx, out, outcap, o.show_algorithm);
+                if (rc == WMB_OK && emit_lines(ctx, out, outcap, o.show_algorithm)) rc = WMB_E_STATE;
             }
             if (rc != WMB_OK) break;
             fill = 0;
@@ -564,7 +651,7 @@ int main(int argc, char *argv[])
     if (rc == WMB_OK) {
         size_t nframes = 0;
         rc = wmb_poll(ctx, NULL, 0, &nframes, 1);       /* EOF: flush */
-        emit_lines(ctx, out, outcap, o.show_algorithm);
+        if (rc == WMB_OK && emit_lines(ctx, out, outcap, o.show_algorithm)) rc = WMB_E_STATE;
     }
     if (rc != WMB_OK) fprintf(stderr, "rtl_wmbus_b200: %s\n", wmb_last_error());
     free(out);
@@ -590,6 +677,11 @@ int main(int argc, char *argv[])
         fprintf(stderr, "rtl_wmbus_b200: WMBUS_B200_BURST_QUALITY: %s\n", strerror(errno));
         return EXIT_FAILURE;
     }
+    if (g_snip_index && fclose(g_snip_index) != 0 && rc == WMB_OK) {
+        fprintf(stderr, "rtl_wmbus_b200: WMBUS_B200_SNIPPETS: %s\n", strerror(errno));
+        return EXIT_FAILURE;
+    }
+    free(g_snip_bytes);
     if (g_rep_file && fclose(g_rep_file) != 0 && rc == WMB_OK) {
         fprintf(stderr, "rtl_wmbus_b200: WMBUS_B200_REPAIRED: %s\n", strerror(errno));
         return EXIT_FAILURE;

@@ -25,7 +25,9 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <map>
 #include <memory>
+#include <set>
 #include <string>
 #include <vector>
 #include <thread>
@@ -41,6 +43,7 @@
 #include "wmb_framer.h"
 #include "wmb_kernels.cuh"
 #include "wmb_bursts.cuh"
+#include "wmb_snippets.cuh"
 #include "wmb_spectrum.cuh"
 
 #ifndef WMB_VERSION
@@ -238,7 +241,9 @@ struct wmb_ctx {
     uint64_t *d_k3_agg = nullptr;
     /* a gathered batch; per table, the elements its prefix copy fetched (0: the table was not copied) */
     struct InFlight { int slot; bool final; bool has_timers; uint64_t m_end;
-                      uint32_t hdr, dec, qual, pool, brec, bqual, ssum, speak, rep; };
+                      uint32_t hdr, dec, qual, pool, brec, bqual, ssum, speak, rep;
+                      bool sn; uint64_t sn_g0, sn_bytes; uint32_t snlist, snpool;     /* the batch's kept granules */
+                      uint64_t iq_end; };
     std::vector<InFlight> inflight;                  /* gathered batches whose results the host has not read yet */
     uint64_t stat_rerun_seen = 0, stat_fallback_seen = 0;
     double acc_demod_ms = 0, acc_bitsync_ms = 0, acc_pass_ms = 0;    /* timers of the current push */
@@ -270,6 +275,26 @@ struct wmb_ctx {
     BurstSlot *d_bslot = nullptr, *h_bslot = nullptr;
     std::vector<QueuedBurst> bursts;                 /* closed pieces not taken yet */
     uint64_t burst_frontier = 0;                     /* no piece still to come starts before this sample */
+
+    /* burst snippets (wmb_set_snippets; the mode survives wmb_reset).  0: off, nothing is allocated, launched or copied */
+    uint32_t snip_mode = 0;
+    uint32_t *d_snkeep = nullptr;
+    uint64_t *d_snrank = nullptr, *d_snagg = nullptr;
+    SnipDev *d_snd = nullptr;
+    uint64_t *d_snn = nullptr, *h_snn = nullptr;     /* [WMB_NSLOT] granules the slot's batch kept */
+    uint32_t snip_pool_gran = 0;                     /* granules a slot's pool holds */
+    SlotTable<uint32_t> snlist;                      /* [WMB_NSLOT][granules of a batch]: the kept ones, in order */
+    SlotTable<uint8_t> snpool;                       /* [WMB_NSLOT][snip_pool_gran * 4096 d]: their bytes */
+    cudaEvent_t ev_snip[2] = {nullptr, nullptr};     /* ksn_copy is done with d_in[i] */
+    const uint8_t *last_src = nullptr;               /* the last batch's input bytes (d_in[i] or the caller's) */
+    size_t last_bytes = 0;
+    struct SnipGran { std::vector<uint8_t> bytes; bool lost; };
+    std::map<uint64_t, SnipGran> sn_store;           /* kept granules by absolute index */
+    std::vector<wmb_snippet> sn_queue;               /* burst pieces whose snippets are not handed out yet */
+    std::set<uint64_t> sn_ok[WMB_N_CHAINS];          /* access-code matches of CRC-ok lines and repaired telegrams */
+    uint64_t sn_iq_end = 0;                          /* input consumed by the batches booked so far (IQ samples) */
+    uint64_t sn_g_first = 0;                         /* first granule pushed since wmb_reset / wmb_seek */
+    bool sn_flushed = false;                         /* the end-of-input gather has been booked */
 
     /* signal quality (wmb_set_line_quality; survives wmb_reset).  Off: nothing is allocated, launched or copied */
     bool quality = false;
@@ -718,6 +743,29 @@ static int launch_bursts(wmb_ctx *c, const BurstParams &p, uint64_t *agg)
     return WMB_OK;
 }
 
+/* the snippet pass of one batch (wmb_snippets.cuh), on cs behind the burst pass: keep flags, their ranks, the copy */
+static int launch_snippets(wmb_ctx *c, const SnipParams &p, uint64_t *n_keep)
+{
+    const uint32_t blocks = (p.ng + WMB_SNIP_BLOCK - 1) / WMB_SNIP_BLOCK;
+#ifdef WMB_HOSTSIM
+    static uint8_t any[WMB_SNIP_BLOCK + WMB_SNIP_HALO];
+    hs_for(blocks, [&](uint32_t b) {
+        hs_for(WMB_SNIP_BLOCK + WMB_SNIP_HALO, [&](uint32_t i) { ksn_keep_fill(p, b * WMB_SNIP_BLOCK, i, any); });
+        hs_for(WMB_SNIP_BLOCK, [&](uint32_t t) { ksn_keep_decide(p, b * WMB_SNIP_BLOCK, t, any); });
+    });
+    launch_cscan(c, p.keep, c->d_snrank, p.ng, c->d_snagg, n_keep, nullptr, nullptr, 1);
+    p.sd->la1 = p.sd->la1_next;
+    hs_for(p.ng, [&](uint32_t g) { hs_for(WMB_SNIP_BLOCK, [&](uint32_t t) { ksn_copy_part(p, g, t, WMB_SNIP_BLOCK); }); });
+#else
+    ksn_keep_kernel<<<blocks, WMB_SNIP_BLOCK, 0, c->cs>>>(p);
+    launch_cscan(c, p.keep, c->d_snrank, p.ng, c->d_snagg, n_keep, nullptr, nullptr, 1);
+    ksn_copy_kernel<<<p.ng, WMB_SNIP_BLOCK, 0, c->cs>>>(p);
+    CUDA_TRY(cudaGetLastError());
+#endif
+    c->st.kernel_launches += 2;
+    return WMB_OK;
+}
+
 /* the band survey's FFT pass over one batch (wmb_spectrum.cuh), on the demod stream */
 static int launch_spectrum(wmb_ctx *c, const SpecParams &p, cudaStream_t st)
 {
@@ -910,8 +958,12 @@ static void read_tuning()
     if (r >= 32 && r <= K2P2W_THREADS * K2P2W_ITEMS) g_p2_records = r;
 }
 
+static bool bursts_on(const wmb_ctx *c);
+
 static int ctx_alloc(wmb_ctx *c)
 {
+    if (c->snip_mode && !bursts_on(c))
+        return set_err(WMB_E_STATE, "snippets follow the burst report: turn it on for a chain (wmb_set_bursts) before the first push");
     if (c->allocated) return WMB_OK;
     const uint32_t d = c->d;
     c->M_max = (int64_t)(c->max_batch_bytes / (2 * (size_t)d));
@@ -1078,6 +1130,28 @@ static int burst_alloc(wmb_ctx *c)
     TRY(host_alloc(c, &c->h_bslot, WMB_NSLOT));
     CUDA_TRY(cudaDeviceSynchronize());
     c->burst_allocated = true;
+    return WMB_OK;
+}
+
+/* the snippet pass's buffers, at the first gather that needs them.  A slot's pool holds at most 64 MiB (or one batch):
+ * sized to the batch, a jammer that keeps every granule would pin four batches of host memory */
+static int snip_alloc(wmb_ctx *c)
+{
+    if (c->d_snd) return WMB_OK;
+    const size_t gb = (size_t)4096 * c->d;
+    const size_t ng = (size_t)c->M_max / WMB_SNIP_GRAN + 2;
+    c->snip_pool_gran = (uint32_t)std::max<size_t>(std::min<size_t>(WMB_SNIP_POOL_MAX, c->max_batch_bytes) / gb, 1);
+    if (c->o.reserved[1] & 4u) c->snip_pool_gran = 1;      /* tests: reach the lost path with a small capture */
+    TRY(dev_alloc(c, &c->d_snkeep, ng));
+    TRY(dev_alloc(c, &c->d_snrank, ng));
+    TRY(dev_alloc(c, &c->d_snagg, scan_tiles((uint32_t)ng) + 1));
+    TRY(dev_alloc(c, &c->d_snn, WMB_NSLOT, true));
+    TRY(host_alloc(c, &c->h_snn, WMB_NSLOT));
+    TRY(c->snlist.alloc(c, 1, ng, 256, 64));
+    TRY(c->snpool.alloc(c, 1, (size_t)c->snip_pool_gran * gb, (uint32_t)std::min<size_t>(16 * gb, (size_t)c->snip_pool_gran * gb), 0));
+    for (int i = 0; i < 2; i++) CUDA_TRY(cudaEventCreateWithFlags(&c->ev_snip[i], cudaEventDisableTiming));
+    TRY(dev_alloc(c, &c->d_snd, 1, true));
+    CUDA_TRY(cudaDeviceSynchronize());
     return WMB_OK;
 }
 
@@ -1292,7 +1366,7 @@ extern "C" void wmb_destroy(wmb_ctx *c)
     for (void *p : c->host_allocs) cudaFreeHost(p);
     for (cudaStream_t st : { c->k1s, c->as[0], c->as[1], c->as2[0], c->as2[1], c->ts, c->s2, c->rs }) if (st) cudaStreamSynchronize(st);
     for (int i = 0; i < 2; i++) {
-        for (cudaEvent_t e : { c->ev_h2d[i], c->ev_k1done[i], c->ev_k1[i], c->ev_k2a[i], c->ev_k2a2[i], c->ev_chain[i] }) if (e) cudaEventDestroy(e);
+        for (cudaEvent_t e : { c->ev_h2d[i], c->ev_k1done[i], c->ev_k1[i], c->ev_k2a[i], c->ev_k2a2[i], c->ev_chain[i], c->ev_snip[i] }) if (e) cudaEventDestroy(e);
         if (c->as[i]) cudaStreamDestroy(c->as[i]);
         if (c->as2[i]) cudaStreamDestroy(c->as2[i]);
     }
@@ -1747,6 +1821,7 @@ static int run_batch(wmb_ctx *c, const uint8_t *src, size_t nbytes, cudaEvent_t 
     c->st.batches++;
     c->batch_no++;
     c->prev_M = M; c->last_M = M; c->last_set = set;
+    c->last_src = src; c->last_bytes = nbytes;
     return WMB_OK;
 }
 
@@ -1758,6 +1833,41 @@ static double chain_carrier_hz(const wmb_ctx *c, int chain)
     if (c->o.simultaneous == 2) return 25e3 * (double)c->o.carrier_25khz[chain];
     if (c->o.simultaneous) return chain == 0 ? 325e3 : -325e3;
     return 0.0;
+}
+
+/* one slot's kept granules (fetched whole) -> the granule store; those beyond the slot's pool are lost */
+static void book_granules(wmb_ctx *c, const wmb_ctx::InFlight &f, uint64_t n, uint64_t stored)
+{
+    const uint64_t gb = 4096ull * c->d;
+    const uint32_t *list = c->snlist.h + c->snlist.at(f.slot);
+    const uint8_t *pool = c->snpool.h + c->snpool.at(f.slot);
+    for (uint64_t i = 0; i < n; i++) {
+        wmb_ctx::SnipGran &g = c->sn_store[f.sn_g0 + list[i]];
+        g.lost = i >= stored;
+        if (g.lost) { g.bytes.clear(); continue; }
+        const uint64_t at = (uint64_t)list[i] * gb;
+        g.bytes.assign(pool + i * gb, pool + i * gb + std::min(gb, f.sn_bytes - at));
+    }
+    c->st.d2h_bytes += sizeof(uint64_t) + std::max<uint64_t>(n, f.snlist) * sizeof(uint32_t) + std::max<uint64_t>(stored * gb, f.snpool);
+}
+
+/* the granules of a piece's snippet: [max(g_first, floor(s / 2048) - PRE), ceil(e / 2048) + POST), the end clipped to
+ * the input consumed */
+static uint64_t snip_lo(const wmb_ctx *c, uint64_t s)
+{
+    const uint64_t g = s / WMB_SNIP_GRAN;
+    return std::max<uint64_t>(c->sn_g_first, g >= WMB_SNIP_PRE ? g - WMB_SNIP_PRE : 0);
+}
+static uint64_t snip_hi(uint64_t e) { return (e + WMB_SNIP_GRAN - 1) / WMB_SNIP_GRAN + WMB_SNIP_POST; }
+
+/* drop the granules and matches that no piece still queued or still to come (they start at the burst frontier or
+ * later) can need */
+static void snip_prune(wmb_ctx *c)
+{
+    uint64_t s_min = c->burst_frontier;
+    for (const wmb_snippet &q : c->sn_queue) s_min = std::min<uint64_t>(s_min, q.start_sample);
+    c->sn_store.erase(c->sn_store.begin(), c->sn_store.lower_bound(snip_lo(c, s_min)));
+    for (int ch = 0; ch < WMB_N_CHAINS; ch++) c->sn_ok[ch].erase(c->sn_ok[ch].begin(), c->sn_ok[ch].lower_bound(s_min));
 }
 
 /* one slot's burst records (fetched whole) -> the queue; the frontier: where the next piece of any chain may start */
@@ -1784,6 +1894,12 @@ static void book_bursts(wmb_ctx *c, const wmb_ctx::InFlight &f)
             b.carrier_hz = chain_carrier_hz(c, ch);
             b.offset_hz = b.valid ? (double)r.sum / (double)r.n / (double)WMB_OFS_SCALE * 400e3 / c->fir_gain[ch] : NAN;
             c->bursts.push_back(qb);
+            if (c->snip_mode) {
+                wmb_snippet sn;
+                memset(&sn, 0, sizeof(sn));
+                sn.start_sample = r.start; sn.end_sample = r.end; sn.chain = r.chain; sn.flags = r.flags;
+                c->sn_queue.push_back(sn);
+            }
         }
         if (bs.open[ch] && (uint64_t)bs.ps[ch] < frontier) frontier = (uint64_t)bs.ps[ch];
     }
@@ -1805,6 +1921,8 @@ static int enqueue_gather(wmb_ctx *c, bool final, bool after_batch)
     const bool quality = c->quality && !c->manual;  /* (a caller's frames carry no sums: manual mode takes none) */
     const bool bursts = bursts_on(c) && (after_batch || final);
     if (bursts) TRY(burst_alloc(c));
+    const bool snips = c->snip_mode && bursts && after_batch;
+    if (snips) TRY(snip_alloc(c));
     if (quality) TRY(qual_alloc(c));
     const bool repair = c->repair_e && !c->manual;
     const bool repair_soft = repair && (c->repair_k || c->repair_s || c->repair_s1);   /* K4S behind K4R */
@@ -1898,6 +2016,30 @@ static int enqueue_gather(wmb_ctx *c, bool final, bool after_batch)
             if (bqual) TRY(c->bqual.enqueue(slot, ch, c->cs, &f.bqual));
         }
     }
+    /* the snippet pass: behind kb_mask of the burst-on chains, on the batch's input bytes.  A host push's next H2D into
+     * the same input buffer waits for ev_snip; a device push returns only after consume_all, so the caller's buffer is
+     * read before it may be reused */
+    if (snips) {
+        SnipParams p;
+        memset(&p, 0, sizeof(p));
+        for (int ch = 0; ch < WMB_N_CHAINS; ch++)
+            if (c->burst_level[ch] && (c->chains & (1u << ch))) p.mask[ch] = c->bb[ch].mask;
+        const uint64_t m_first = c->m_consumed - (uint64_t)c->last_M;
+        p.nw = (uint32_t)((c->last_M + 31) / 32);
+        p.ng = (uint32_t)((c->last_M + WMB_SNIP_GRAN - 1) / WMB_SNIP_GRAN);
+        p.g0 = m_first / WMB_SNIP_GRAN;
+        p.keep = c->d_snkeep; p.rank = c->d_snrank; p.sd = c->d_snd;
+        p.in = c->last_src; p.in_bytes = c->last_bytes; p.gbytes = 4096u * c->d;
+        p.pool_gran = c->snip_pool_gran;
+        p.pool = c->snpool.d + c->snpool.at(slot); p.list = c->snlist.d + c->snlist.at(slot);
+        TRY(launch_snippets(c, p, c->d_snn + slot));
+        for (int i = 0; i < 2; i++)
+            if (c->last_src == c->d_in[i]) CUDA_TRY(cudaEventRecord(c->ev_snip[i], c->cs));
+        CUDA_TRY(cudaMemcpyAsync(c->h_snn + slot, c->d_snn + slot, sizeof(uint64_t), cudaMemcpyDeviceToHost, c->cs));
+        TRY(c->snlist.enqueue(slot, 0, c->cs, &f.snlist));
+        TRY(c->snpool.enqueue(slot, 0, c->cs, &f.snpool));
+        f.sn = true; f.sn_g0 = p.g0; f.sn_bytes = c->last_bytes;
+    }
     /* the band survey: the rows the batch closed (its kernels ran on the demod stream), or at the end of input the
      * record still open */
     if (c->spec_bins) {
@@ -1937,7 +2079,7 @@ static int enqueue_gather(wmb_ctx *c, bool final, bool after_batch)
         CUDA_TRY(cudaEventRecord(c->ev_chain[c->last_set], c->cs));
         c->chain_recorded[c->last_set] = true;
     }
-    f.slot = slot; f.final = final; f.has_timers = after_batch; f.m_end = c->m_consumed;
+    f.slot = slot; f.final = final; f.has_timers = after_batch; f.m_end = c->m_consumed; f.iq_end = c->iq_consumed;
     c->inflight.push_back(f);
     c->gather_no++;
     return WMB_OK;
@@ -1978,6 +2120,13 @@ static int consume_oldest(wmb_ctx *c)
         if (f.bqual) TRY(c->bqual.fetch(f.slot, ch, f.bqual, n, c->xs, &more));
         most = std::max(most, n);
     }
+    const uint64_t sn_n = f.sn ? c->h_snn[f.slot] : 0;                   /* granules the batch kept */
+    const uint64_t sn_stored = std::min<uint64_t>(sn_n, c->snip_pool_gran);
+    const uint32_t gbytes = 4096u * c->d;
+    if (f.sn) {
+        TRY(c->snlist.fetch(f.slot, 0, f.snlist, (uint32_t)sn_n, c->xs, &more));
+        TRY(c->snpool.fetch(f.slot, 0, f.snpool, (uint32_t)(sn_stored * gbytes), c->xs, &more));
+    }
     TRY(c->hdr.fetch(f.slot, 0, f.hdr, r.n, c->xs, &more));
     if (f.dec) TRY(c->dec.fetch(f.slot, 0, f.dec, r.n, c->xs, &more));
     if (f.qual) TRY(c->qual.fetch(f.slot, 0, f.qual, r.n, c->xs, &more));
@@ -1996,7 +2145,14 @@ static int consume_oldest(wmb_ctx *c)
     /* the next batches probably look like this one: let the prefix copies cover them */
     if (f.brec) { c->brec.grow(most); c->bqual.grow(most); }
     if (f.hdr) { c->hdr.grow(r.n); c->dec.grow(r.n); c->qual.grow(r.n); c->rep.grow(r.n); c->pool.grow(r.pool_n); }
+    if (f.sn) {
+        c->snlist.grow((uint32_t)sn_n); c->snpool.grow((uint32_t)(sn_stored * gbytes));
+        book_granules(c, f, sn_n, sn_stored);
+    }
+    if (f.final) c->sn_flushed = c->snip_mode != 0;
+    c->sn_iq_end = f.iq_end;
     if (f.brec) book_bursts(c, f);
+    if (c->snip_mode) snip_prune(c);
     if (f.ssum) {                                    /* the slot's survey rows -> the queue */
         const std::vector<wmb_spectrum_row> &rows = c->spec_slot_rows[f.slot];
         const size_t at = c->ssum.at(f.slot);        /* = c->speak.at(f.slot): both hold rows x bins */
@@ -2005,14 +2161,17 @@ static int consume_oldest(wmb_ctx *c)
         c->spec_peak.insert(c->spec_peak.end(), c->speak.h + at, c->speak.h + at + f.speak);
         c->st.d2h_bytes += (uint64_t)f.ssum * sizeof(uint64_t) + (uint64_t)f.speak * sizeof(uint32_t);
     }
-    if (!f.hdr) return WMB_OK;
+    if (!f.hdr) {
+        if (sn_n > sn_stored) c->st.overflow_batches++;
+        return WMB_OK;
+    }
     const uint32_t err = r.errors;
     if (err & 2u) return set_err(WMB_E_OVERFLOW, "run-length tracker left its defined range (the reference would spin here)");
     /* lane event buffer (1: a run-length lane emitted more than one bit per four samples plus one capped edge -- the
      * tracker's bit length has collapsed to a fraction of a sample), frame words (4), datagram pool (8), access-code
      * matches (16), pending candidates (64): the device dropped what did not fit and cleared the flags; the reference
      * would have gone on decoding, so does the stream */
-    if (err & K3_SOFT_ERRORS) c->st.overflow_batches++;
+    if ((err & K3_SOFT_ERRORS) || sn_n > sn_stored) c->st.overflow_batches++;
     if (err & 256u) return set_err(WMB_E_STATE, "internal: lane verification does not converge");
     c->st.d2h_bytes += sizeof(BatchRec) + (size_t)r.n * sizeof(FrameHdr) + (f.dec ? (size_t)r.n * sizeof(DecHdr) + r.pool_n : 0);
     if (f.qual) c->st.d2h_bytes += (size_t)r.n * sizeof(QualAcc);
@@ -2110,7 +2269,7 @@ extern "C" int wmb_push_device(wmb_ctx *c, const void *dev_cu8, size_t nbytes)
     const size_t tail = nbytes % batch_granule(c);
     rc = process_device_batches(c, (const uint8_t *)dev_cu8, nbytes - tail, false);
     if (rc) return rc;
-    rc = consume_all(c);                                  /* also: the caller's buffer is no longer in use */
+    rc = consume_all(c);                                  /* also: the caller's buffer is no longer in use (the snippet copy reads it) */
     if (rc || !tail) return rc;
     c->remainder.resize(tail);
     CUDA_TRY(cudaMemcpy(c->remainder.data(), (const uint8_t *)dev_cu8 + (nbytes - tail), tail, cudaMemcpyDeviceToHost));
@@ -2181,6 +2340,7 @@ static int push_host_bytes(wmb_ctx *c, const uint8_t *p, size_t nbytes, bool fin
     c->acc_demod_ms = c->acc_bitsync_ms = c->acc_pass_ms = 0; c->push_started = false;
     int idx = c->buf_idx;
     CUDA_TRY(cudaStreamWaitEvent(c->xs, c->ev_k1done[idx], 0));
+    if (c->ev_snip[idx]) CUDA_TRY(cudaStreamWaitEvent(c->xs, c->ev_snip[idx], 0));     /* the snippet copy read it */
     CUDA_TRY(cudaMemcpyAsync(c->d_in[idx], p, cur_n, cudaMemcpyHostToDevice, c->xs));
     CUDA_TRY(cudaEventRecord(c->ev_h2d[idx], c->xs));
     while (cur_n) {
@@ -2189,6 +2349,7 @@ static int push_host_bytes(wmb_ctx *c, const uint8_t *p, size_t nbytes, bool fin
         if (nxt_n) {
             const int nidx = idx ^ 1;
             CUDA_TRY(cudaStreamWaitEvent(c->xs, c->ev_k1done[nidx], 0));
+            if (c->ev_snip[nidx]) CUDA_TRY(cudaStreamWaitEvent(c->xs, c->ev_snip[nidx], 0));
             CUDA_TRY(cudaMemcpyAsync(c->d_in[nidx], p + nxt_off, nxt_n, cudaMemcpyHostToDevice, c->xs));
             CUDA_TRY(cudaEventRecord(c->ev_h2d[nidx], c->xs));
         }
@@ -2315,6 +2476,7 @@ static int book_frames(wmb_ctx *c, size_t n, Meta meta, Lite lite, Fill fill, st
             fresh.push_back(k);
             c->st.lines[f.chain][f.algo]++;
             if (d.crc_ok) c->st.lines_crc_ok[f.chain][f.algo]++;
+            if (d.crc_ok && c->snip_mode) c->sn_ok[f.chain].insert(f.sync_sample);
         }
     }
     /* the reference prints in the order the per-sample state machines finish:
@@ -2413,6 +2575,7 @@ static void book_repairs(wmb_ctx *c, const FrameHdr *hdr, const DecHdr *dec, con
         r.soft_s1 = (uint8_t)(h.had_line >> 2 & 1u);
         repaired_from(h, hdr[i].sync_sample, rep_mode(hdr[i].chain, dec[i]), pool, r.repair);
         fresh.push_back(r);
+        if (h.outcome == K4R_REPAIRED && c->snip_mode) c->sn_ok[r.chain].insert(r.sync_sample);
     };
     /* the frames of a gather are in stream order: (chain, algo, ordinal) ascending */
     auto find = [&](int ch, int a, uint64_t ord) -> long {
@@ -2840,6 +3003,8 @@ extern "C" int wmb_reset(wmb_ctx *c)
     c->chain_recorded[0] = c->chain_recorded[1] = false;
     c->stat_rerun_seen = 0; c->stat_fallback_seen = 0;
     c->bursts.clear(); c->burst_frontier = 0;
+    c->sn_store.clear(); c->sn_queue.clear(); c->sn_ok[0].clear(); c->sn_ok[1].clear();
+    c->sn_iq_end = 0; c->sn_g_first = 0; c->sn_flushed = false;
     c->spec_open = -1; c->spec_open_blocks = 0; c->spec_batch_rows.clear(); c->spec_enqueued = false;
     c->spec_rows.clear(); c->spec_sum.clear(); c->spec_peak.clear();
     for (int ch = 0; ch < WMB_N_CHAINS; ch++)
@@ -2867,6 +3032,7 @@ extern "C" int wmb_reset(wmb_ctx *c)
         if (c->burst_allocated)                  /* no run open */
             for (int ch = 0; ch < WMB_N_CHAINS; ch++)
                 if (c->bb[ch].bd) CUDA_TRY(cudaMemsetAsync(c->bb[ch].bd, 0, sizeof(BurstDev), c->cs));
+        if (c->d_snd) CUDA_TRY(cudaMemsetAsync(c->d_snd, 0, sizeof(SnipDev), c->cs));      /* no above granule yet */
         if (c->speak.cap) {                      /* no record open */
             CUDA_TRY(cudaMemsetAsync(c->d_ssum_ring, 0, c->speak.cap * sizeof(uint64_t), c->cs));
             CUDA_TRY(cudaMemsetAsync(c->d_speak_ring, 0, c->speak.cap * sizeof(uint32_t), c->cs));
@@ -2885,6 +3051,7 @@ extern "C" int wmb_seek(wmb_ctx *c, uint64_t first_iq_sample)
     if (rc) return rc;
     c->iq_consumed = first_iq_sample;
     c->m_consumed = first_iq_sample / c->d;
+    c->sn_iq_end = first_iq_sample; c->sn_g_first = first_iq_sample / (2048ull * c->d);
     return WMB_OK;
 }
 
@@ -3171,18 +3338,12 @@ extern "C" long wmb_boundary_state(wmb_ctx *c, uint8_t *buf, size_t cap)
     return (long)out.size();
 }
 
-extern "C" long wmb_pending_before(wmb_ctx *c, uint64_t sync_hi)
+/* the access-code matches (decimated samples) of the telegrams in flight, per chain; after consume_all */
+static int pending_matches(wmb_ctx *c, std::vector<uint64_t> *match)
 {
-    if (!c) return set_err(WMB_E_INVAL, "null argument");
-    CUDA_TRY(cudaSetDevice(c->device));
-    int rc = ctx_alloc(c);
-    if (rc) return rc;
-    rc = consume_all(c);                                /* every enqueued batch is gathered and booked first */
-    if (rc) return rc;
     CUDA_TRY(cudaStreamSynchronize(c->cs));
     GatherDev gd;
     CUDA_TRY(cudaMemcpy(&gd, c->d_gd, sizeof(gd), cudaMemcpyDeviceToHost));
-    long n_before = 0;
     std::vector<uint64_t> pend;
     for (int ch = 0; ch < WMB_N_CHAINS; ch++) {
         if (!(c->chains & (1u << ch))) continue;
@@ -3197,12 +3358,97 @@ extern "C" long wmb_pending_before(wmb_ctx *c, uint64_t sync_hi)
                 if ((int64_t)ord <= s.busy_until && !rep_waiting(c, s, ord)) continue;
                 uint64_t ev = 0;                                         /* the flagged bit's event: its sample is the match */
                 CUDA_TRY(cudaMemcpy(&ev, s.ring + (ord & (s.ring_cap - 1)), 8, cudaMemcpyDeviceToHost));
-                const uint64_t m = c->m_consumed - ((c->m_consumed - EVG_M(ev)) & EVG_M_MASK);   /* 40 bits -> stream position */
-                if (m < sync_hi) n_before++;
+                match[ch].push_back(c->m_consumed - ((c->m_consumed - EVG_M(ev)) & EVG_M_MASK));   /* 40 bits -> stream position */
             }
         }
     }
+    return WMB_OK;
+}
+
+extern "C" long wmb_pending_before(wmb_ctx *c, uint64_t sync_hi)
+{
+    if (!c) return set_err(WMB_E_INVAL, "null argument");
+    CUDA_TRY(cudaSetDevice(c->device));
+    int rc = ctx_alloc(c);
+    if (rc) return rc;
+    rc = consume_all(c);                                /* every enqueued batch is gathered and booked first */
+    if (rc) return rc;
+    std::vector<uint64_t> match[WMB_N_CHAINS];
+    rc = pending_matches(c, match);
+    if (rc) return rc;
+    long n_before = 0;
+    for (int ch = 0; ch < WMB_N_CHAINS; ch++)
+        for (uint64_t m : match[ch]) if (m < sync_hi) n_before++;
     return n_before;
+}
+
+extern "C" int wmb_set_snippets(wmb_ctx *c, int mode)
+{
+    if (!c) return set_err(WMB_E_INVAL, "null argument");
+    if (mode < 0 || mode > 2) return set_err(WMB_E_INVAL, "snippet mode %d: 0 (off), 1 (every burst) or 2 (undecoded bursts)", mode);
+    if (c->batch_no != 0 || !c->remainder.empty())
+        return set_err(WMB_E_STATE, "wmb_set_snippets after samples were pushed (call it before the first push or after wmb_reset / wmb_seek)");
+    c->snip_mode = (uint32_t)mode;
+    return WMB_OK;
+}
+
+/* a match of the chain's set in [lo, hi) */
+static bool any_in(const std::set<uint64_t> &s, uint64_t lo, uint64_t hi)
+{
+    const auto it = s.lower_bound(lo);
+    return it != s.end() && *it < hi;
+}
+static bool any_in(const std::vector<uint64_t> &v, uint64_t lo, uint64_t hi)
+{
+    for (uint64_t m : v) if (m >= lo && m < hi) return true;
+    return false;
+}
+
+extern "C" int wmb_take_snippets(wmb_ctx *c, wmb_snippet *recs, size_t cap, uint8_t *bytes, size_t bytes_cap, size_t *n)
+{
+    if (!c || !n || (!recs && cap) || (!bytes && bytes_cap)) return set_err(WMB_E_INVAL, "null argument");
+    *n = 0;
+    if (!c->snip_mode || c->sn_queue.empty()) return WMB_OK;
+    CUDA_TRY(cudaSetDevice(c->device));
+    TRY(consume_all(c));
+    /* per chain the queue is in start order; across chains a piece closed later may start earlier */
+    std::stable_sort(c->sn_queue.begin(), c->sn_queue.end(), [](const wmb_snippet &a, const wmb_snippet &b) {
+        return a.start_sample != b.start_sample ? a.start_sample < b.start_sample : a.chain < b.chain;
+    });
+    const uint64_t gi = 2048ull * c->d;
+    const uint64_t g_whole = c->sn_iq_end / gi, g_end = (c->sn_iq_end + gi - 1) / gi;
+    std::vector<uint64_t> pend[WMB_N_CHAINS];
+    bool have_pend = c->sn_flushed;                      /* nothing is in flight after the end of input */
+    size_t k = 0, used = 0, i = 0;
+    for (; i < c->sn_queue.size(); i++) {
+        wmb_snippet q = c->sn_queue[i];
+        if (q.start_sample >= c->burst_frontier) break;                  /* the burst report has not handed it out */
+        if (!c->sn_flushed && snip_hi(q.end_sample) > g_whole) break;    /* its last granules are still to come */
+        if (!have_pend) { TRY(pending_matches(c, pend)); have_pend = true; }
+        if (any_in(pend[q.chain], q.start_sample, q.end_sample)) break;  /* decoded or not is not known yet */
+        q.decoded = any_in(c->sn_ok[q.chain], q.start_sample, q.end_sample) ? 1 : 0;
+        if (q.decoded && c->snip_mode == 2) continue;
+        const uint64_t lo = snip_lo(c, q.start_sample), hi = std::min(snip_hi(q.end_sample), g_end);
+        uint64_t nb = 0;
+        for (uint64_t g = lo; g < hi; g++) {
+            const auto it = c->sn_store.find(g);
+            if (it == c->sn_store.end() || it->second.lost) { q.lost = 1; break; }
+            nb += it->second.bytes.size();
+        }
+        if (q.lost) nb = 0;
+        if (k >= cap || used + nb > bytes_cap) break;
+        q.start_iq = lo * gi; q.nbytes = nb;
+        for (uint64_t g = lo; g < hi && !q.lost; g++) {
+            const std::vector<uint8_t> &b = c->sn_store[g].bytes;
+            memcpy(bytes + used, b.data(), b.size());
+            used += b.size();
+        }
+        recs[k++] = q;
+    }
+    c->sn_queue.erase(c->sn_queue.begin(), c->sn_queue.begin() + (long)i);
+    snip_prune(c);
+    *n = k;
+    return WMB_OK;
 }
 
 extern "C" int wmb_get_stats(wmb_ctx *c, wmb_stats *s)

@@ -105,6 +105,37 @@ def merge_bursts(parts, quals=None):
     return recs[order], q[order]
 
 
+def merge_snippets(parts, infos=None, repairs=None, undecoded=False):
+    """Snippets ((records, data) of take_snippets()) of several time chunks, each holding those of the pieces that start
+    in its chunk -> the sequential run's, in burst order.  A line whose match lies after a chunk's end belongs to the next
+    chunk, so a chunk cannot decide `decoded` for a piece that runs past its end: with infos (the merged line records,
+    merge_lines(..., infos)) and repairs (the merged repair records, when repair is on) it is decided here, and
+    undecoded=True keeps the pieces that did not decode (the chunks take every piece, mode 1)."""
+    import numpy as np
+    recs = np.concatenate([p[0] for p in parts])
+    data = [x for p in parts for x in p[1]]
+    order = np.lexsort((recs["chain"], recs["start_sample"]))
+    recs, data = recs[order], [data[i] for i in order]
+    if infos is None:
+        assert not undecoded, "deciding which pieces decoded needs the merged line records"
+        return recs, data
+    ok = {0: [], 1: []}
+    for r in infos:
+        if r["crc_ok"]:
+            ok[int(r["chain"])].append(int(r["sync_sample"]))
+    for r in repairs or []:
+        if r.repair.outcome == 1:                        # WMB_REP_REPAIRED
+            ok[int(r.chain)].append(int(r.sync_sample))
+    ok = {ch: np.sort(np.asarray(v, np.uint64)) for ch, v in ok.items()}
+    for i, r in enumerate(recs):
+        m = ok[int(r["chain"])]
+        recs[i]["decoded"] = int(np.searchsorted(m, r["end_sample"]) > np.searchsorted(m, r["start_sample"]))
+    if undecoded:
+        keep = recs["decoded"] == 0
+        recs, data = recs[keep], [x for x, k in zip(data, keep) if k]
+    return recs, data
+
+
 def merge_spectrum(parts):
     """Band-survey records (rows, sum, peak) of several time chunks -> the sequential run's records: sum and blocks
     added, peak the max, over the rows of one record (a record that straddles a chunk border has a row in each)."""
@@ -186,7 +217,7 @@ def find_carriers(rows, sum, peak, fs: float, threshold_db: float = 15.0, bridge
 
 
 def decode_time_chunk(ctx, push, n_bytes: int, d: int, rank: int, world: int, halo_m: int = 1 << 18, info=False,
-                      bursts=False, spectrum=False, quality=False, repairs=False):
+                      bursts=False, spectrum=False, quality=False, repairs=False, snippets=False):
     """Decode rank `rank`'s chunk of a capture of n_bytes cu8 bytes.  `push(byte_lo, byte_hi)` feeds that byte
     range of the capture to ctx (host or device memory: the caller's business).
     Returns (lines, digest_start, digest_end, halo_start_iq): digest_start is None for a chunk that starts at 0.
@@ -205,7 +236,12 @@ def decode_time_chunk(ctx, push, n_bytes: int, d: int, rank: int, world: int, ha
     repairs=True (ctx made with repair=e_max, repair_soft=k_max for the C1, repair_t1_soft=s_max for the T1 and
     repair_s1_soft=s_max for the S1 soft repair; the settings survive the chunk's seek): the repair records (take_repairs()) of the candidates matched in the chunk
     come last; merge_repairs() over the chunks gives the sequential records.  A candidate that waits for its repair
-    counts in pending_before(), so the right halo goes on until its record is made."""
+    counts in pending_before(), so the right halo goes on until its record is made.
+    snippets=True (ctx made with a burst level and snippets=1): the snippets (take_snippets(): records, data) of the pieces
+    that start in the chunk come after the bursts and the survey's records.  The left halo holds their PRE granules, and
+    the right halo (MAX_TELEGRAM_M = 2^18 samples) holds the rest: a piece that starts before hi ends at most 2^17 + 2^16
+    samples later, its end is decided 196 after that, and its POST granules follow within 3 x 2048.  merge_snippets() joins them; it decides `decoded` from the merged line
+    records, since a line whose match lies past hi belongs to the next chunk."""
     import hashlib
     recs = []
     qrecs = []
@@ -213,8 +249,13 @@ def decode_time_chunk(ctx, push, n_bytes: int, d: int, rank: int, world: int, ha
     bqrecs = []
     srecs = []
     rrecs = []
+    snrecs, sndata = [], []
 
     def take_s():
+        if snippets:
+            r, b = ctx.take_snippets()
+            snrecs.append(r)
+            sndata.extend(b)
         if spectrum:
             srecs.append(ctx.take_spectrum())
 
@@ -295,6 +336,11 @@ def decode_time_chunk(ctx, push, n_bytes: int, d: int, rank: int, world: int, ha
         srecs = [x for x in srecs if len(x[0])] or srecs[:1]
         out.append((np.concatenate([x[0] for x in srecs]), np.concatenate([x[1] for x in srecs]),
                     np.concatenate([x[2] for x in srecs])))
+    if snippets:
+        r = np.concatenate(snrecs)
+        m_lo, m_hi = lo // d, (hi // d if rank + 1 < world else 1 << 63)
+        keep = (r["start_sample"] >= m_lo) & (r["start_sample"] < m_hi)
+        out.append((r[keep], [x for x, kk in zip(sndata, keep) if kk]))
     if repairs:
         out.append(rrecs)
     lines = tuple(out) if len(out) > 1 else lines
