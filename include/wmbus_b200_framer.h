@@ -283,6 +283,81 @@ int wmb_frame_repair_s1_soft_device(wmb_ctx *ctx, const wmb_frame *frames, const
  * tag and s_max when s_max is not 0. */
 int wmb_set_repair_s1_soft(wmb_ctx *ctx, uint32_t s_max);
 
+/* ---- telegrams: one record per transmission, from both bit syncs and the repairs ----------------------------------
+ * Each chain runs two bit syncs, so one transmission usually gives two lines (t2a and rla), and with repair on a
+ * REPAIRED record beside a CRC-failed twin.  wmb_group_telegrams() joins them by this rule:
+ *   1. Candidates, per chain: every line (CRC ok or not) and every repair record whose outcome is WMB_REP_REPAIRED.
+ *      A candidate is verified when it is a CRC-ok line or a repaired line; its datagram is then the datagram column
+ *      (CRC bytes removed: wmb_decoded.datagram[0 .. len)).
+ *   2. Same transmission: two candidates of one chain whose access-code matches (sync_sample) lie at most W[chain]
+ *      decimated samples apart belong together; a group is the transitive closure.  Spans are not compared: the
+ *      end_sample of a failed candidate comes from an L-field that may itself be wrong.  W is WMB_TLG_W_T1C1 /
+ *      WMB_TLG_W_S1, chosen from the distance of the t2a and rla matches of one telegram (DESIGN.md section 8).
+ *   3. Records: one per distinct verified datagram of a group (the same mode and the same bytes), decoded = 1, with
+ *      sources the WMB_TLG_* bits of the candidates that carry it.  failed counts the group's candidates that are not
+ *      verified (a CRC-failed line, also when its repair is in the group).  A group without a verified candidate gives
+ *      one record with decoded = 0, its failed count, no bytes and no valid header field.
+ *   4. Header fields, from the datagram (L C M M A A A A V T CI ...): l = byte 0, c = byte 1, m = bytes 2..3 (little
+ *      endian) and manuf its three letters ((m >> 10) & 31) + 64, ((m >> 5) & 31) + 64, (m & 31) + 64, id = bytes 4..7
+ *      (little endian: the line's LINK_LAYER_IDENT_NO column), version = byte 8, type = byte 9, ci = byte 10.  valid
+ *      holds the WMB_TLG_F_* bit of each field the datagram is long enough for; the others are 0.
+ *   5. Order: sync_sample is the group's earliest match (all records of a group share it); records are ordered by
+ *      (sync_sample, chain), the records of one group by (mode, len, bytes). */
+#define WMB_TLG_W_T1C1 128
+#define WMB_TLG_W_S1   256
+
+#define WMB_TLG_T2A_LINE   1u
+#define WMB_TLG_RLA_LINE   2u
+#define WMB_TLG_T2A_REPAIR 4u
+#define WMB_TLG_RLA_REPAIR 8u
+
+#define WMB_TLG_F_L       1u
+#define WMB_TLG_F_C       2u
+#define WMB_TLG_F_M       4u
+#define WMB_TLG_F_ID      8u
+#define WMB_TLG_F_VERSION 16u
+#define WMB_TLG_F_TYPE    32u
+#define WMB_TLG_F_CI      64u
+
+typedef struct wmb_telegram {
+    uint64_t sync_sample;     /* the group's earliest access-code match (decimated sample)                      */
+    uint32_t id;              /* bytes 4..7, little endian                                                      */
+    uint16_t m;               /* bytes 2..3, little endian                                                      */
+    uint16_t len;             /* datagram bytes (0 when decoded = 0)                                            */
+    uint32_t failed;          /* the group's candidates without a verified datagram                            */
+    uint8_t  chain;           /* WMB_CHAIN_*                                                                    */
+    uint8_t  decoded;
+    uint8_t  sources;         /* WMB_TLG_* bits                                                                 */
+    uint8_t  valid;           /* WMB_TLG_F_* bits                                                               */
+    char     mode[3];         /* "T1", "C1", "S1"; "" when decoded = 0                                          */
+    char     manuf[4];        /* three letters; "" without WMB_TLG_F_M                                          */
+    uint8_t  l, c, version, type, ci;
+    uint8_t  pad[4];
+} wmb_telegram;
+
+/* The rule above over n_lines lines (info[i] and their decodes line[i]: sync_sample, chain, algo and crc_ok of info,
+ * mode, len and datagram of line) and n_repairs repair records (those not REPAIRED are ignored), in any order.  The
+ * records go to out in order and their datagrams, concatenated, to data.  out must hold n_lines + n_repairs records and
+ * data_cap the sum of len over the verified candidates (bounds that hold for any input), else WMB_E_INVAL.  *n receives
+ * the number of records. */
+int wmb_group_telegrams(const wmb_line_info *info, const wmb_decoded *line, size_t n_lines,
+                        const wmb_repair_record *repairs, size_t n_repairs,
+                        wmb_telegram *out, size_t cap, uint8_t *data, size_t data_cap, size_t *n);
+
+/* Telegrams on the streaming path.  wmb_set_telegrams(ctx, on), on 0 (off, the default) or 1; WMB_E_INVAL on a
+ * manual_frames context (its caller frames its own candidates: it calls wmb_group_telegrams); the state rules of
+ * wmb_set_repair, and the setting survives wmb_reset / wmb_seek.  On, the context keeps its lines and (repair on) its
+ * REPAIRED records and groups them as wmb_group_telegrams does.  A group is handed out once it is final: no telegram of
+ * its chain still in flight (wmb_pending_before's condition) and no match still to come lies within W of a member, so
+ * neither a line nor a repair can join it later; and once no group still to come can come before it.  After the end of
+ * input (flush) every group is final.  The records do not depend on batch size, push size or thread order.  Off, the
+ * context keeps nothing.  It is host work only: no launch and no copy. */
+int wmb_set_telegrams(wmb_ctx *ctx, int on);
+
+/* Copy whole records in order: recs[i] and its len bytes, concatenated in data.  Stops at cap records or when the next
+ * record's bytes do not fit data_cap; *n receives the number copied.  Records not taken stay queued. */
+int wmb_take_telegrams(wmb_ctx *ctx, wmb_telegram *recs, size_t cap, uint8_t *data, size_t data_cap, size_t *n);
+
 /* CRC-16, polynomial 0x3D65, complemented (t1_c1_packet_decoder.h:463-469) */
 uint16_t wmb_crc16(const uint8_t *data, size_t n);
 

@@ -12,8 +12,8 @@ reference's hyphen).
 """
 from .capi import (WmbOpts, WmbStats, WmbFrame, WmbLineInfo, WmbDecoded, WmbRepaired, WmbRepairRecord, WmbusB200, load_library, library_path, build,
                    opts_from_flags, line_info_dtype, burst_dtype, BURST_CONTINUED, BURST_CUT, BURST_AT_END, spectrum_dtype,
-                   line_quality_dtype, burst_quality_dtype, snippet_dtype, LIB_NAME)
+                   line_quality_dtype, burst_quality_dtype, snippet_dtype, telegram_dtype, group_telegrams, LIB_NAME)
 
 __all__ = ["WmbOpts", "WmbStats", "WmbFrame", "WmbLineInfo", "WmbDecoded", "WmbRepaired", "WmbRepairRecord", "WmbusB200", "load_library", "library_path", "build",
            "opts_from_flags", "line_info_dtype", "burst_dtype", "BURST_CONTINUED", "BURST_CUT", "BURST_AT_END", "spectrum_dtype",
-           "line_quality_dtype", "burst_quality_dtype", "snippet_dtype", "LIB_NAME"]
+           "line_quality_dtype", "burst_quality_dtype", "snippet_dtype", "telegram_dtype", "group_telegrams", "LIB_NAME"]

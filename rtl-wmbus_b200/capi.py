@@ -91,6 +91,52 @@ def snippet_dtype():
     return np.dtype(SNIPPET_FIELDS)
 
 
+# numpy mirror of wmb_telegram (one record per transmission; see include/wmbus_b200_framer.h)
+TELEGRAM_FIELDS = [("sync_sample", "<u8"), ("id", "<u4"), ("m", "<u2"), ("len", "<u2"), ("failed", "<u4"),
+                   ("chain", "u1"), ("decoded", "u1"), ("sources", "u1"), ("valid", "u1"), ("mode", "S3"),
+                   ("manuf", "S4"), ("l", "u1"), ("c", "u1"), ("version", "u1"), ("type", "u1"), ("ci", "u1"),
+                   ("pad", "u1", (4,))]
+TLG_W = (128, 256)                        # WMB_TLG_W_T1C1, WMB_TLG_W_S1: decimated samples between matches of one group
+TLG_T2A_LINE, TLG_RLA_LINE, TLG_T2A_REPAIR, TLG_RLA_REPAIR = 1, 2, 4, 8      # wmb_telegram.sources
+TLG_F_L, TLG_F_C, TLG_F_M, TLG_F_ID, TLG_F_VERSION, TLG_F_TYPE, TLG_F_CI = 1, 2, 4, 8, 16, 32, 64   # wmb_telegram.valid
+
+
+def telegram_dtype():
+    import numpy as np
+    return np.dtype(TELEGRAM_FIELDS)
+
+
+def group_telegrams(lib, info, lines, repairs=()):
+    """wmb_group_telegrams over line records (a numpy array of wmb_line_info), their decodes (a sequence of WmbDecoded,
+    one per record) and repair records (WmbRepairRecord) -> (records, data): records a numpy array of wmb_telegram
+    (telegram_dtype()), data a list with the datagram bytes of each record"""
+    import numpy as np
+    info = np.ascontiguousarray(info, dtype=line_info_dtype())
+    assert len(info) == len(lines), "one decode per line record"
+    dec = (WmbDecoded * max(len(lines), 1))(*lines)
+    rep = (WmbRepairRecord * max(len(repairs), 1))(*repairs)
+    cap = len(lines) + len(repairs)
+    need = sum(int(d.len) for d, r in zip(lines, info) if r["crc_ok"]) + sum(int(r.repair.line.len) for r in repairs
+                                                                           if r.repair.outcome == REP_REPAIRED)
+    out = np.zeros(max(cap, 1), telegram_dtype())
+    buf = np.zeros(max(need, 1), np.uint8)
+    n = C.c_size_t(0)
+    rc = lib.wmb_group_telegrams(info.ctypes.data if len(info) else None, dec, len(lines), rep, len(repairs),
+                                 out.ctypes.data, cap, buf.ctypes.data, need, C.byref(n))
+    if rc != 0:
+        raise RuntimeError(f"wmb_group_telegrams failed ({rc})")
+    out = out[:n.value]
+    return out, _split(buf, out["len"])
+
+
+def _split(buf, lens):
+    """the concatenated datagrams in buf -> one bytes object per record"""
+    import numpy as np
+    ends = np.cumsum(lens, dtype=np.int64).tolist()
+    raw = buf[:ends[-1] if ends else 0].tobytes()
+    return [raw[a:b] for a, b in zip([0] + ends[:-1], ends)]
+
+
 # numpy mirrors of wmb_line_quality and wmb_burst_quality (see include/wmbus_b200.h)
 LINE_QUALITY_FIELDS = [("sync_sample", "<u8"), ("end_sample", "<u8"), ("n_hi", "<u4"), ("n_lo", "<u4"),
                        ("s1_hi", "<i8"), ("s1_lo", "<i8"), ("s2_hi", "<u8"), ("s2_lo", "<u8"), ("bits", "<u4"),
@@ -182,6 +228,10 @@ def _bind(lib):
     lib.wmb_set_line_quality.argtypes = [C.c_void_p, C.c_int]
     lib.wmb_set_snippets.argtypes = [C.c_void_p, C.c_int]
     lib.wmb_take_snippets.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
+    lib.wmb_set_telegrams.argtypes = [C.c_void_p, C.c_int]
+    lib.wmb_take_telegrams.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
+    lib.wmb_group_telegrams.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p,
+                                        C.c_size_t, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
     lib.wmb_take_lines_quality.argtypes = [C.c_void_p, C.c_char_p, C.c_size_t, C.POINTER(C.c_size_t), C.c_int,
                                            C.c_void_p, C.c_void_p, C.c_size_t]
     lib.wmb_take_lines_quality.restype = C.c_size_t
@@ -221,7 +271,7 @@ EXPORTS = ["wmb_reset", "wmb_host_alloc", "wmb_host_free", "wmb_default_opts", "
            "wmb_seek", "wmb_set_line_window", "wmb_boundary_state", "wmb_pending_before", "wmb_set_receiver",
            "wmb_take_lines_info", "wmb_set_bursts", "wmb_take_bursts", "wmb_set_spectrum", "wmb_take_spectrum",
            "wmb_debug_spectrum_tables", "wmb_set_line_quality", "wmb_take_lines_quality", "wmb_take_bursts_quality",
-           "wmb_set_snippets", "wmb_take_snippets"]
+           "wmb_set_snippets", "wmb_take_snippets", "wmb_set_telegrams", "wmb_take_telegrams", "wmb_group_telegrams"]
 
 
 def load_library(path: str | None = None):
@@ -285,11 +335,13 @@ class WmbusB200:
     soft_bits_s1=True (manual_frames=1 only): the soft value of every S1 chip too, see wmb_set_soft_bits_s1().
     snippets=mode: the raw bytes around each burst piece, see wmb_set_snippets() (0: off, the default; 1: every piece;
     2: the pieces that did not decode); needs burst_level on a chain.  It survives reset() and seek().  take_snippets()
-    hands them out."""
+    hands them out.
+    telegrams=True: one record per transmission from both bit syncs and the repairs, see wmb_set_telegrams() (off by
+    default); it survives reset() and seek().  take_telegrams() hands out the final ones."""
 
     def __init__(self, flags: str = "", device: int = 0, lib=None, clock_lock=None, access_code_errors=None,
                  burst_level=None, spectrum=None, quality=False, repair=0, repair_soft=0, soft_bits=False,
-                 repair_t1_soft=0, repair_s1_soft=0, soft_bits_s1=False, snippets=0, **tuning):
+                 repair_t1_soft=0, repair_s1_soft=0, soft_bits_s1=False, snippets=0, telegrams=False, **tuning):
         self.lib = lib or load_library()
         self.opts = opts_from_flags(self.lib, flags, **tuning)
         self._ctx = C.c_void_p()
@@ -364,6 +416,12 @@ class WmbusB200:
         if snippets:
             try:
                 self.set_snippets(snippets)
+            except Exception:
+                self.close()
+                raise
+        if telegrams:
+            try:
+                self.set_telegrams(True)
             except Exception:
                 self.close()
                 raise
@@ -613,6 +671,27 @@ class WmbusB200:
                 at += int(x["nbytes"])
             recs.append(r)
         return (np.concatenate(recs) if recs else np.zeros(0, snippet_dtype())), data
+
+    def set_telegrams(self, on: bool):
+        """telegram records on / off (before the first push, or after reset/seek; not with manual_frames)"""
+        self._check(self.lib.wmb_set_telegrams(self._ctx, 1 if on else 0))
+
+    def take_telegrams(self, cap=1 << 12):
+        """the final telegram records, in order: (records, data), records a numpy structured array of wmb_telegram
+        (telegram_dtype()) and data a list with the datagram bytes of each record"""
+        import numpy as np
+        recs, data = [], []
+        buf = np.zeros(cap * 292, np.uint8)          # any cap records' datagrams fit
+        while True:
+            r = np.zeros(cap, telegram_dtype())
+            n = C.c_size_t(0)
+            self._check(self.lib.wmb_take_telegrams(self._ctx, r.ctypes.data, cap, buf.ctypes.data, len(buf), C.byref(n)))
+            if n.value == 0:
+                break
+            r = r[:n.value]
+            data += _split(buf, r["len"])
+            recs.append(r)
+        return (np.concatenate(recs) if recs else np.zeros(0, telegram_dtype())), data
 
     def set_line_quality(self, on: bool):
         """signal-quality report on / off (before the first push, or after reset/seek)"""

@@ -68,6 +68,15 @@
  *   WMBUS_B200_SNIPPET_MODE=undecoded|all   the pieces saved (default undecoded: those without a CRC-ok line).
  *   A directory that cannot be written, a bad mode, or a mode without WMBUS_B200_SNIPPETS is an error at start-up.
  *   stdout does not change.
+ *   WMBUS_B200_TELEGRAMS=<path> write one record per transmission (wmb_set_telegrams: the lines of both bit syncs and,
+ *                              with WMBUS_B200_REPAIRED, the repaired ones, grouped by their access-code matches), once
+ *                              it is final, flushed after each hand-over:
+ *                              MODE;DECODED;SOURCES;FAILED;SYNC_SAMPLE;MANUF;ID;VERSION;TYPE;CI;0xDATAGRAM
+ *                              SOURCES the WMB_TLG_* bits (1 t2a line, 2 rla line, 4 t2a repair, 8 rla repair), ID %08X
+ *                              (the LINK_LAYER_IDENT_NO of its lines), VERSION, TYPE and CI %02X.  A record with DECODED 0
+ *                              has the chain (T1C1 or S1) as MODE and "-" for every field after SYNC_SAMPLE, and so has a
+ *                              field the datagram is too short for.  A path that cannot be opened is an error at start-up.
+ *                              stdout does not change.
  */
 #define _GNU_SOURCE
 #include <errno.h>
@@ -364,6 +373,50 @@ static void emit_repairs(wmb_ctx *ctx, const char *ts, int show_algorithm)
     fflush(g_rep_file);
 }
 
+/* WMBUS_B200_TELEGRAMS: one line per final telegram record */
+static FILE *g_tlg_file = NULL;
+#define TLG_CAP 256
+static wmb_telegram g_tlgs[TLG_CAP];
+static uint8_t g_tlg_bytes[TLG_CAP * 292];
+
+static void put_field(uint8_t valid, uint8_t bit, const char *fmt, unsigned v)
+{
+    if (valid & bit) fprintf(g_tlg_file, fmt, v);
+    else fputs(";-", g_tlg_file);
+}
+
+static int emit_telegrams(wmb_ctx *ctx)
+{
+    if (!g_tlg_file) return 0;
+    for (;;) {
+        size_t n = 0;
+        if (wmb_take_telegrams(ctx, g_tlgs, TLG_CAP, g_tlg_bytes, sizeof(g_tlg_bytes), &n) != WMB_OK) {
+            fprintf(stderr, "rtl_wmbus_b200: %s\n", wmb_last_error());
+            return -1;
+        }
+        if (!n) break;
+        size_t at = 0;
+        for (size_t i = 0; i < n; i++) {
+            const wmb_telegram *t = &g_tlgs[i];
+            const char *mode = t->decoded ? t->mode : t->chain == WMB_CHAIN_T1C1 ? "T1C1" : "S1";
+            fprintf(g_tlg_file, "%s;%u;%u;%u;%llu", mode, t->decoded, t->sources, t->failed, (unsigned long long)t->sync_sample);
+            if (t->valid & WMB_TLG_F_M) fprintf(g_tlg_file, ";%s", t->manuf);
+            else fputs(";-", g_tlg_file);
+            put_field(t->valid, WMB_TLG_F_ID, ";%08X", t->id);
+            put_field(t->valid, WMB_TLG_F_VERSION, ";%02X", t->version);
+            put_field(t->valid, WMB_TLG_F_TYPE, ";%02X", t->type);
+            put_field(t->valid, WMB_TLG_F_CI, ";%02X", t->ci);
+            if (t->len) {
+                fputs(";0x", g_tlg_file);
+                for (unsigned k = 0; k < t->len; k++) fprintf(g_tlg_file, "%02x", g_tlg_bytes[at + k]);
+                fputc('\n', g_tlg_file);
+            } else fputs(";-\n", g_tlg_file);
+            at += t->len;
+        }
+    }
+    return fflush(g_tlg_file) == 0 ? 0 : -1;
+}
+
 static int emit_lines(wmb_ctx *ctx, char *out, size_t outcap, int show_algorithm)
 {
     if (emit_snippets(ctx)) return -1;
@@ -379,7 +432,7 @@ static int emit_lines(wmb_ctx *ctx, char *out, size_t outcap, int show_algorithm
             : wmb_take_lines(ctx, out, outcap, &nl, 0);
         if (!nl) {
             emit_repairs(ctx, ts, show_algorithm);
-            return 0;
+            return emit_telegrams(ctx);
         }
         fwrite(out, 1, n, stdout);
         fflush(stdout);                                 /* t1_c1_packet_decoder.h:698-699 */
@@ -554,6 +607,11 @@ int main(int argc, char *argv[])
         return EXIT_FAILURE;
     }
 
+    if ((e = getenv("WMBUS_B200_TELEGRAMS")) != NULL && (g_tlg_file = fopen(e, "w")) == NULL) {
+        fprintf(stderr, "rtl_wmbus_b200: WMBUS_B200_TELEGRAMS=%s: %s\n", e, strerror(errno));
+        return EXIT_FAILURE;
+    }
+
     wmb_ctx *ctx = NULL;
     if (wmb_create(&o, device, &ctx) != WMB_OK) {
         fprintf(stderr, "rtl_wmbus_b200: %s\n", wmb_last_error());
@@ -577,6 +635,10 @@ int main(int argc, char *argv[])
     if (g_rep_file && (wmb_set_repair(ctx, (uint32_t)repair_e) != WMB_OK || wmb_set_repair_soft(ctx, (uint32_t)repair_k) != WMB_OK ||
                        wmb_set_repair_t1_soft(ctx, (uint32_t)repair_s) != WMB_OK ||
                        wmb_set_repair_s1_soft(ctx, (uint32_t)repair_s1) != WMB_OK)) {
+        fprintf(stderr, "rtl_wmbus_b200: %s\n", wmb_last_error());
+        return EXIT_FAILURE;
+    }
+    if (g_tlg_file && wmb_set_telegrams(ctx, 1) != WMB_OK) {
         fprintf(stderr, "rtl_wmbus_b200: %s\n", wmb_last_error());
         return EXIT_FAILURE;
     }
@@ -682,6 +744,10 @@ int main(int argc, char *argv[])
         return EXIT_FAILURE;
     }
     free(g_snip_bytes);
+    if (g_tlg_file && fclose(g_tlg_file) != 0 && rc == WMB_OK) {
+        fprintf(stderr, "rtl_wmbus_b200: WMBUS_B200_TELEGRAMS: %s\n", strerror(errno));
+        return EXIT_FAILURE;
+    }
     if (g_rep_file && fclose(g_rep_file) != 0 && rc == WMB_OK) {
         fprintf(stderr, "rtl_wmbus_b200: WMBUS_B200_REPAIRED: %s\n", strerror(errno));
         return EXIT_FAILURE;

@@ -294,7 +294,16 @@ struct wmb_ctx {
     std::set<uint64_t> sn_ok[WMB_N_CHAINS];          /* access-code matches of CRC-ok lines and repaired telegrams */
     uint64_t sn_iq_end = 0;                          /* input consumed by the batches booked so far (IQ samples) */
     uint64_t sn_g_first = 0;                         /* first granule pushed since wmb_reset / wmb_seek */
-    bool sn_flushed = false;                         /* the end-of-input gather has been booked */
+
+    /* telegrams (wmb_set_telegrams; survives wmb_reset).  Off: nothing is kept */
+    bool telegrams = false;
+    std::vector<wmb_line_info> tg_info;              /* the lines and REPAIRED records of groups not final yet */
+    std::vector<wmb_decoded> tg_line;                /* parallel to tg_info */
+    std::vector<wmb_repair_record> tg_rep;
+    struct ReadyTelegram { wmb_telegram t; std::vector<uint8_t> bytes; };
+    std::vector<ReadyTelegram> tg_ready;             /* records of final groups not handed out yet, in order */
+
+    bool flushed = false;                            /* the end-of-input gather has been booked (snippets, telegrams) */
 
     /* signal quality (wmb_set_line_quality; survives wmb_reset).  Off: nothing is allocated, launched or copied */
     bool quality = false;
@@ -2149,7 +2158,7 @@ static int consume_oldest(wmb_ctx *c)
         c->snlist.grow((uint32_t)sn_n); c->snpool.grow((uint32_t)(sn_stored * gbytes));
         book_granules(c, f, sn_n, sn_stored);
     }
-    if (f.final) c->sn_flushed = c->snip_mode != 0;
+    if (f.final) c->flushed = true;
     c->sn_iq_end = f.iq_end;
     if (f.brec) book_bursts(c, f);
     if (c->snip_mode) snip_prune(c);
@@ -2513,6 +2522,14 @@ static int book_frames(wmb_ctx *c, size_t n, Meta meta, Lite lite, Fill fill, st
         q.ofs_valid = m.ofs_valid; q.ofs_sum = m.ofs_sum; q.ofs_n = m.ofs_n;
         if (m.qual) q.qual = *m.qual; else qual_zero(q.qual);
         fill(fresh[i].fi, q.d);
+        if (c->telegrams) {
+            wmb_line_info r;
+            memset(&r, 0, sizeof(r));
+            r.sync_sample = q.sync_sample; r.end_sample = q.end_sample;
+            r.chain = q.chain; r.algo = q.algo; r.crc_ok = q.d.crc_ok;
+            c->tg_info.push_back(r);
+            c->tg_line.push_back(q.d);
+        }
     }
     return WMB_OK;
 }
@@ -2576,6 +2593,7 @@ static void book_repairs(wmb_ctx *c, const FrameHdr *hdr, const DecHdr *dec, con
         repaired_from(h, hdr[i].sync_sample, rep_mode(hdr[i].chain, dec[i]), pool, r.repair);
         fresh.push_back(r);
         if (h.outcome == K4R_REPAIRED && c->snip_mode) c->sn_ok[r.chain].insert(r.sync_sample);
+        if (h.outcome == K4R_REPAIRED && c->telegrams) c->tg_rep.push_back(r);
     };
     /* the frames of a gather are in stream order: (chain, algo, ordinal) ascending */
     auto find = [&](int ch, int a, uint64_t ord) -> long {
@@ -3004,7 +3022,8 @@ extern "C" int wmb_reset(wmb_ctx *c)
     c->stat_rerun_seen = 0; c->stat_fallback_seen = 0;
     c->bursts.clear(); c->burst_frontier = 0;
     c->sn_store.clear(); c->sn_queue.clear(); c->sn_ok[0].clear(); c->sn_ok[1].clear();
-    c->sn_iq_end = 0; c->sn_g_first = 0; c->sn_flushed = false;
+    c->sn_iq_end = 0; c->sn_g_first = 0; c->flushed = false;
+    c->tg_info.clear(); c->tg_line.clear(); c->tg_rep.clear(); c->tg_ready.clear();
     c->spec_open = -1; c->spec_open_blocks = 0; c->spec_batch_rows.clear(); c->spec_enqueued = false;
     c->spec_rows.clear(); c->spec_sum.clear(); c->spec_peak.clear();
     for (int ch = 0; ch < WMB_N_CHAINS; ch++)
@@ -3418,12 +3437,12 @@ extern "C" int wmb_take_snippets(wmb_ctx *c, wmb_snippet *recs, size_t cap, uint
     const uint64_t gi = 2048ull * c->d;
     const uint64_t g_whole = c->sn_iq_end / gi, g_end = (c->sn_iq_end + gi - 1) / gi;
     std::vector<uint64_t> pend[WMB_N_CHAINS];
-    bool have_pend = c->sn_flushed;                      /* nothing is in flight after the end of input */
+    bool have_pend = c->flushed;                         /* nothing is in flight after the end of input */
     size_t k = 0, used = 0, i = 0;
     for (; i < c->sn_queue.size(); i++) {
         wmb_snippet q = c->sn_queue[i];
         if (q.start_sample >= c->burst_frontier) break;                  /* the burst report has not handed it out */
-        if (!c->sn_flushed && snip_hi(q.end_sample) > g_whole) break;    /* its last granules are still to come */
+        if (!c->flushed && snip_hi(q.end_sample) > g_whole) break;       /* its last granules are still to come */
         if (!have_pend) { TRY(pending_matches(c, pend)); have_pend = true; }
         if (any_in(pend[q.chain], q.start_sample, q.end_sample)) break;  /* decoded or not is not known yet */
         q.decoded = any_in(c->sn_ok[q.chain], q.start_sample, q.end_sample) ? 1 : 0;
@@ -3447,6 +3466,107 @@ extern "C" int wmb_take_snippets(wmb_ctx *c, wmb_snippet *recs, size_t cap, uint
     }
     c->sn_queue.erase(c->sn_queue.begin(), c->sn_queue.begin() + (long)i);
     snip_prune(c);
+    *n = k;
+    return WMB_OK;
+}
+
+extern "C" int wmb_set_telegrams(wmb_ctx *c, int on)
+{
+    if (!c) return set_err(WMB_E_INVAL, "null argument");
+    if (on != 0 && on != 1) return set_err(WMB_E_INVAL, "telegrams %d: 0 (off) or 1 (on)", on);
+    if (c->manual) return set_err(WMB_E_INVAL, "wmb_set_telegrams on a manual_frames context (group its lines with wmb_group_telegrams)");
+    TRY(repair_setter_check(c, "wmb_set_telegrams", false, nullptr, nullptr, 0, 0));
+    c->telegrams = on != 0;
+    return WMB_OK;
+}
+
+/* Telegrams: the groups of the kept candidates that are final go through wmb_group_telegrams into tg_ready.  A group
+ * [lo, hi] of a chain is final when no match still to come can lie within W of it: a telegram in flight (its match is
+ * known) outside [lo - W, hi + W], and a match not seen yet lies at or after the samples booked, m_consumed > hi + W.
+ * Returns in *bound the sample before which no group still to come starts: the first match of the groups that are not
+ * final, of the telegrams in flight, and m_consumed.  After consume_all. */
+static int tlg_settle(wmb_ctx *c, uint64_t *bound)
+{
+    static const uint64_t W[WMB_N_CHAINS] = { WMB_TLG_W_T1C1, WMB_TLG_W_S1 };
+    std::vector<uint64_t> pend[WMB_N_CHAINS];
+    if (!c->flushed) TRY(pending_matches(c, pend));                   /* nothing is in flight after the end of input */
+    const uint64_t seen = c->flushed ? ~0ull : c->m_consumed;
+    *bound = seen;
+    for (int ch = 0; ch < WMB_N_CHAINS; ch++)
+        for (uint64_t p : pend[ch]) *bound = std::min(*bound, p);
+    struct Cand { uint64_t sync; size_t i; uint8_t chain; };         /* i: line i, or repair record i - lines */
+    const size_t nl = c->tg_info.size(), nr = c->tg_rep.size();
+    std::vector<Cand> cand;
+    cand.reserve(nl + nr);
+    for (size_t i = 0; i < nl; i++) cand.push_back({ c->tg_info[i].sync_sample, i, c->tg_info[i].chain });
+    for (size_t i = 0; i < nr; i++) cand.push_back({ c->tg_rep[i].sync_sample, nl + i, c->tg_rep[i].chain });
+    std::sort(cand.begin(), cand.end(), [](const Cand &a, const Cand &b) {
+        return a.chain != b.chain ? a.chain < b.chain : a.sync < b.sync;
+    });
+    std::vector<char> fin(nl + nr, 0);
+    bool any = false;
+    for (size_t g = 0, e; g < cand.size(); g = e) {
+        const int ch = cand[g].chain;
+        for (e = g + 1; e < cand.size() && cand[e].chain == ch && cand[e].sync - cand[e - 1].sync <= W[ch]; e++) {}
+        const uint64_t lo = cand[g].sync, hi = cand[e - 1].sync;
+        bool final = seen == ~0ull || hi + W[ch] < seen;
+        for (uint64_t p : pend[ch]) if (p + W[ch] >= lo && p <= hi + W[ch]) final = false;
+        if (!final) { *bound = std::min(*bound, lo); continue; }
+        for (size_t k = g; k < e; k++) fin[cand[k].i] = 1;
+        any = true;
+    }
+    if (!any) return WMB_OK;
+    std::vector<wmb_line_info> info, keep_info;
+    std::vector<wmb_decoded> line, keep_line;
+    std::vector<wmb_repair_record> rep, keep_rep;
+    size_t bytes = 0;
+    for (size_t i = 0; i < nl; i++) {
+        if (!fin[i]) { keep_info.push_back(c->tg_info[i]); keep_line.push_back(c->tg_line[i]); continue; }
+        info.push_back(c->tg_info[i]); line.push_back(c->tg_line[i]);
+        bytes += c->tg_line[i].len;
+    }
+    for (size_t i = 0; i < nr; i++) {
+        if (!fin[nl + i]) { keep_rep.push_back(c->tg_rep[i]); continue; }
+        rep.push_back(c->tg_rep[i]);
+        bytes += c->tg_rep[i].repair.line.len;
+    }
+    std::vector<wmb_telegram> out(info.size() + rep.size());
+    std::vector<uint8_t> data(bytes);
+    size_t n = 0;
+    if (wmb_group_telegrams(info.data(), line.data(), info.size(), rep.data(), rep.size(), out.data(), out.size(), data.data(),
+                            data.size(), &n) != WMB_OK)
+        return set_err(WMB_E_STATE, "internal: wmb_group_telegrams refused the context's candidates");
+    size_t at = 0;
+    for (size_t k = 0; k < n; k++) {
+        c->tg_ready.push_back({ out[k], std::vector<uint8_t>(data.begin() + (long)at, data.begin() + (long)(at + out[k].len)) });
+        at += out[k].len;
+    }
+    /* records of earlier groups may wait behind the bound; a group's records share (sync_sample, chain) */
+    std::stable_sort(c->tg_ready.begin(), c->tg_ready.end(), [](const wmb_ctx::ReadyTelegram &a, const wmb_ctx::ReadyTelegram &b) {
+        return a.t.sync_sample != b.t.sync_sample ? a.t.sync_sample < b.t.sync_sample : a.t.chain < b.t.chain;
+    });
+    c->tg_info.swap(keep_info); c->tg_line.swap(keep_line); c->tg_rep.swap(keep_rep);
+    return WMB_OK;
+}
+
+extern "C" int wmb_take_telegrams(wmb_ctx *c, wmb_telegram *recs, size_t cap, uint8_t *data, size_t data_cap, size_t *n)
+{
+    if (!c || !n || (!recs && cap) || (!data && data_cap)) return set_err(WMB_E_INVAL, "null argument");
+    *n = 0;
+    if (!c->telegrams || (c->tg_info.empty() && c->tg_rep.empty() && c->tg_ready.empty())) return WMB_OK;
+    CUDA_TRY(cudaSetDevice(c->device));
+    TRY(consume_all(c));
+    uint64_t bound = 0;
+    TRY(tlg_settle(c, &bound));
+    size_t k = 0, used = 0;
+    for (; k < c->tg_ready.size() && k < cap; k++) {
+        const wmb_ctx::ReadyTelegram &r = c->tg_ready[k];
+        if (r.t.sync_sample >= bound || used + r.bytes.size() > data_cap) break;
+        recs[k] = r.t;
+        if (!r.bytes.empty()) memcpy(data + used, r.bytes.data(), r.bytes.size());
+        used += r.bytes.size();
+    }
+    c->tg_ready.erase(c->tg_ready.begin(), c->tg_ready.begin() + (long)k);
     *n = k;
     return WMB_OK;
 }

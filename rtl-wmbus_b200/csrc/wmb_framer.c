@@ -11,6 +11,7 @@
 #include "wmb_frame_a.h"
 
 #include <stdio.h>
+#include <stdlib.h>
 #include <string.h>
 #include <sys/time.h>
 #include <time.h>
@@ -646,4 +647,147 @@ size_t wmb_format_line(const wmb_decoded *d, const char *algo_prefix, const char
     if (len + 1 < cap) buf[len++] = '\n';
     buf[len] = 0;
     return len;
+}
+
+/* ---- telegrams: one record per transmission (include/wmbus_b200_framer.h) ------------------------------------------ */
+
+typedef struct tlg_cand {
+    uint64_t sync;
+    const wmb_decoded *d;       /* the line, or the repaired line                                               */
+    size_t idx;                 /* input position: lines first, then repair records                             */
+    uint8_t chain, src, verified;
+} tlg_cand;
+
+typedef struct tlg_rec {
+    wmb_telegram t;
+    const wmb_decoded *d;       /* the first candidate that carries the datagram; NULL when decoded = 0          */
+} tlg_rec;
+
+static int tlg_cand_cmp(const void *pa, const void *pb)
+{
+    const tlg_cand *a = (const tlg_cand *)pa, *b = (const tlg_cand *)pb;
+    if (a->chain != b->chain) return a->chain < b->chain ? -1 : 1;
+    if (a->sync != b->sync) return a->sync < b->sync ? -1 : 1;
+    return a->idx < b->idx ? -1 : a->idx > b->idx;
+}
+
+/* (sync_sample, chain), then (mode, len, bytes) inside a group */
+static int tlg_rec_cmp(const void *pa, const void *pb)
+{
+    const tlg_rec *a = (const tlg_rec *)pa, *b = (const tlg_rec *)pb;
+    if (a->t.sync_sample != b->t.sync_sample) return a->t.sync_sample < b->t.sync_sample ? -1 : 1;
+    if (a->t.chain != b->t.chain) return a->t.chain < b->t.chain ? -1 : 1;
+    const int m = strncmp(a->t.mode, b->t.mode, sizeof(a->t.mode));
+    if (m) return m;
+    if (a->t.len != b->t.len) return a->t.len < b->t.len ? -1 : 1;
+    return a->t.len ? memcmp(a->d->datagram, b->d->datagram, a->t.len) : 0;
+}
+
+static int same_datagram(const wmb_decoded *a, const wmb_decoded *b)
+{
+    return strncmp(a->mode, b->mode, sizeof(a->mode)) == 0 && a->len == b->len && memcmp(a->datagram, b->datagram, a->len) == 0;
+}
+
+/* point 4: the link-layer header fields the datagram is long enough for */
+static void tlg_header(wmb_telegram *t, const uint8_t *p, unsigned len)
+{
+    if (len >= 1) { t->l = p[0]; t->valid |= WMB_TLG_F_L; }
+    if (len >= 2) { t->c = p[1]; t->valid |= WMB_TLG_F_C; }
+    if (len >= 4) {
+        t->m = (uint16_t)(p[2] | p[3] << 8);
+        t->manuf[0] = (char)(((t->m >> 10) & 31) + 64);
+        t->manuf[1] = (char)(((t->m >> 5) & 31) + 64);
+        t->manuf[2] = (char)((t->m & 31) + 64);
+        t->valid |= WMB_TLG_F_M;
+    }
+    if (len >= 8) { t->id = (uint32_t)p[4] | (uint32_t)p[5] << 8 | (uint32_t)p[6] << 16 | (uint32_t)p[7] << 24; t->valid |= WMB_TLG_F_ID; }
+    if (len >= 9) { t->version = p[8]; t->valid |= WMB_TLG_F_VERSION; }
+    if (len >= 10) { t->type = p[9]; t->valid |= WMB_TLG_F_TYPE; }
+    if (len >= 11) { t->ci = p[10]; t->valid |= WMB_TLG_F_CI; }
+}
+
+int wmb_group_telegrams(const wmb_line_info *info, const wmb_decoded *line, size_t n_lines,
+                        const wmb_repair_record *repairs, size_t n_repairs,
+                        wmb_telegram *out, size_t cap, uint8_t *data, size_t data_cap, size_t *n)
+{
+    static const uint64_t W[2] = { WMB_TLG_W_T1C1, WMB_TLG_W_S1 };
+    if (!n || (n_lines && (!info || !line)) || (n_repairs && !repairs) || (cap && !out) || (data_cap && !data))
+        return WMB_E_INVAL;
+    *n = 0;
+    size_t need = 0;
+    for (size_t i = 0; i < n_lines; i++) {
+        if (info[i].chain > WMB_CHAIN_S1 || line[i].len > sizeof(line[i].datagram)) return WMB_E_INVAL;
+        if (info[i].crc_ok) need += line[i].len;
+    }
+    for (size_t i = 0; i < n_repairs; i++) {
+        if (repairs[i].chain > WMB_CHAIN_S1 || repairs[i].repair.line.len > sizeof(repairs[i].repair.line.datagram)) return WMB_E_INVAL;
+        if (repairs[i].repair.outcome == WMB_REP_REPAIRED) need += repairs[i].repair.line.len;
+    }
+    if (cap < n_lines + n_repairs || data_cap < need) return WMB_E_INVAL;
+    const size_t nc_max = n_lines + n_repairs;
+    if (!nc_max) return WMB_OK;
+    tlg_cand *cand = (tlg_cand *)malloc(nc_max * sizeof(tlg_cand));
+    tlg_rec *rec = (tlg_rec *)malloc(nc_max * sizeof(tlg_rec));
+    if (!cand || !rec) { free(cand); free(rec); return WMB_E_NOMEM; }
+    size_t nc = 0;
+    for (size_t i = 0; i < n_lines; i++) {                      /* 1. candidates */
+        tlg_cand *k = &cand[nc++];
+        k->sync = info[i].sync_sample; k->d = &line[i]; k->idx = i; k->chain = info[i].chain;
+        k->src = (uint8_t)(info[i].algo == WMB_ALGO_T2A ? WMB_TLG_T2A_LINE : WMB_TLG_RLA_LINE);
+        k->verified = info[i].crc_ok ? 1 : 0;
+    }
+    for (size_t i = 0; i < n_repairs; i++) {
+        const wmb_repair_record *r = &repairs[i];
+        if (r->repair.outcome != WMB_REP_REPAIRED) continue;
+        tlg_cand *k = &cand[nc++];
+        k->sync = r->sync_sample; k->d = &r->repair.line; k->idx = n_lines + i; k->chain = r->chain;
+        k->src = (uint8_t)(r->algo == WMB_ALGO_T2A ? WMB_TLG_T2A_REPAIR : WMB_TLG_RLA_REPAIR);
+        k->verified = 1;
+    }
+    qsort(cand, nc, sizeof(tlg_cand), tlg_cand_cmp);
+    size_t nr = 0;
+    for (size_t g = 0; g < nc;) {                               /* 2. groups: runs of matches at most W apart */
+        size_t e = g + 1;
+        while (e < nc && cand[e].chain == cand[g].chain && cand[e].sync - cand[e - 1].sync <= W[cand[g].chain]) e++;
+        uint32_t failed = 0;
+        const size_t first = nr;
+        for (size_t i = g; i < e; i++) {                        /* 3. one record per distinct verified datagram */
+            if (!cand[i].verified) { failed++; continue; }
+            size_t r = first;
+            while (r < nr && !same_datagram(cand[i].d, rec[r].d)) r++;
+            if (r == nr) {
+                tlg_rec *q = &rec[nr++];
+                memset(&q->t, 0, sizeof(q->t));
+                q->t.decoded = 1;
+                q->t.len = (uint16_t)cand[i].d->len;
+                memcpy(q->t.mode, cand[i].d->mode, sizeof(q->t.mode));
+                q->t.mode[2] = 0;
+                q->d = cand[i].d;
+                tlg_header(&q->t, q->d->datagram, q->t.len);
+            }
+            rec[r].t.sources |= cand[i].src;
+        }
+        if (nr == first) {                                      /* no verified datagram */
+            tlg_rec *q = &rec[nr++];
+            memset(&q->t, 0, sizeof(q->t));
+            q->d = NULL;
+        }
+        for (size_t r = first; r < nr; r++) {
+            rec[r].t.sync_sample = cand[g].sync;
+            rec[r].t.chain = cand[g].chain;
+            rec[r].t.failed = failed;
+        }
+        g = e;
+    }
+    qsort(rec, nr, sizeof(tlg_rec), tlg_rec_cmp);               /* 5. order */
+    size_t at = 0;
+    for (size_t r = 0; r < nr; r++) {
+        out[r] = rec[r].t;
+        if (rec[r].t.len) memcpy(data + at, rec[r].d->datagram, rec[r].t.len);
+        at += rec[r].t.len;
+    }
+    *n = nr;
+    free(cand);
+    free(rec);
+    return WMB_OK;
 }

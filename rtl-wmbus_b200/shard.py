@@ -172,6 +172,35 @@ def merge_repairs(parts):
     return sorted((r for part in parts for r in part), key=repair_key)
 
 
+def line_decoded(line: str):
+    """a datagram line ("[rla;|t2a;]MODE;CRC_OK;3OUTOF6OK;TIMESTAMP;PACKET_RSSI;CURRENT_RSSI;IDENT;0xHEX") -> the
+    WmbDecoded that wmb_format_line prints as it"""
+    import ctypes
+    from .capi import WmbDecoded
+    f = line.split(";")
+    if f[0] in ("rla", "t2a"):
+        f = f[1:]
+    d = WmbDecoded()
+    d.status = 1                                      # WMB_DEC_LINE
+    d.mode = f[0].encode()
+    d.crc_ok, d.ok_3of6 = int(f[1]), int(f[2])
+    d.packet_rssi, d.current_rssi = int(f[4]), int(f[5])
+    d.serial = int(f[6], 16)
+    data = bytes.fromhex(f[7][2:])
+    d.len = len(data)
+    ctypes.memmove(d.datagram, data, len(data))
+    return d
+
+
+def merge_telegrams(lines, infos, repairs=(), lib=None):
+    """Telegram records of a time-sharded run: wmb_group_telegrams (of lib, default the product library) over the merged
+    lines and line records (merge_lines(..., infos)) and the merged repair records (merge_repairs(), when repair is on)
+    -> (records, data) as WmbusB200.take_telegrams() gives them in the sequential run.  The chunks need no telegram
+    records of their own."""
+    from .capi import group_telegrams, load_library
+    return group_telegrams(lib or load_library(), infos, [line_decoded(l) for l in lines], list(repairs))
+
+
 def find_carriers(rows, sum, peak, fs: float, threshold_db: float = 15.0, bridge_hz: float = 110e3,
                   tone_hz: float = 20e3):
     """Carriers worth decoding in a band survey (take_spectrum / merge_spectrum output, or a CLI spectrum file read
